@@ -4,6 +4,7 @@
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference ...      # the CPU path (oracle port of the reference) on the host cores
+    python bench.py ... --dump-outputs DIR    # what the last timed step computed, as DIR/<name>.npy
 
 Default workload (BASELINE.json configs[1]): synthetic RMAT 1 M nodes / 20 M edges, one partition per GPU
 (random partition), 3-layer GraphSAGE, hidden 256, bf16 activations, --enable-pipeline.  A step is one
@@ -12,7 +13,7 @@ epoch: forward, loss, backward (with the gradient halo exchange), gradient all-r
 Order of a run: set-up -> (N > 1) parity of the real multi-GPU path against the CPU oracle -> warm-up -> a short
 Python-launched region instrumented with CUDA events (roofline of the aggregate kernel) -> the timed region: K epochs
 replayed from CUDA graphs (`--no-graph`: launched from Python), exposed communication accumulated ON THE DEVICE by the
-flag-wait kernel inside that region -> the end-to-end region (host buffers, H2D + D2H per step) -> (N = 1) the CPU
+flag-wait kernel inside that region -> (--dump-outputs) the last timed step's results -> the end-to-end region (host buffers, H2D + D2H per step) -> (N = 1) the CPU
 baseline -> ONE JSON line from rank 0.  The process returns normally (no os._exit).
 """
 from __future__ import annotations
@@ -49,11 +50,13 @@ WORKLOADS = {
                             feat_corr=False, grad_corr=False,
                             desc="ogbn-products-shaped RMAT 2.4M nodes / 62M edges, F=100, C=47, 3-layer GraphSAGE "
                                  "hidden 128, fp32, no pipeline"),
-    # configs[4]: per-rank graph construction (no rank holds the global edge list), see pipegcn_b200/distgraph.py
-    "papers100m-shaped": dict(shape="papers100m-shaped", n_layers=3, n_hidden=128, dtype="bf16", enable_pipeline=True,
-                              feat_corr=False, grad_corr=False, distributed_build=True,
-                              desc="ogbn-papers100M-shaped RMAT 111M nodes / 1.6B edges, F=128, C=172, 3-layer GraphSAGE "
-                                   "hidden 128, bf16, --enable-pipeline, per-rank graph construction"),
+    # configs[4]: per-rank graph construction (no rank holds the global edge list), see pipegcn_b200/distgraph.py.
+    # A quarter of the shape: one rank of an 8-way split of the full 111 M / 1.6 B graph holds 13.9 M inner rows and
+    # 211 M edges, and those alone, before any halo row, take 75 GB of an 80 GB H100 (DESIGN.md §6)
+    "papers100m-shaped": dict(shape="papers100m-shaped", scale_down=4, n_layers=3, n_hidden=128, dtype="bf16",
+                              enable_pipeline=True, feat_corr=False, grad_corr=False, distributed_build=True,
+                              desc="a quarter of ogbn-papers100M's shape: RMAT 27.8M nodes / 0.4B edges, F=128, C=172, "
+                                   "3-layer GraphSAGE hidden 128, bf16, --enable-pipeline, per-rank graph construction"),
     "small": dict(shape="small", n_layers=3, n_hidden=64, dtype="bf16", enable_pipeline=True,
                   feat_corr=False, grad_corr=False, desc="20K-node RMAT (debug)"),
 }
@@ -80,6 +83,9 @@ def parse():
     p.add_argument("--use-pp", action="store_true", help="--use-pp of the reference scripts: layer-0 aggregate precomputed once")
     p.add_argument("--ncu-region", action="store_true", help="cudaProfilerStart/Stop around the instrumented steps")
     p.add_argument("--no-graph", action="store_true", help="launch every kernel from Python instead of replaying CUDA graphs")
+    p.add_argument("--dump-outputs", metavar="DIR", default=None,
+                   help="write what the last timed step computed (loss, logits, updated parameters; with --gpus N those of "
+                        "rank 0's partition) as DIR/<name>.npy")
     return p.parse_args()
 
 
@@ -93,7 +99,7 @@ def engine_args(w, n_feat, n_class, n_train, n_parts, dropout, cuda_graph=False,
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
          "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
@@ -134,7 +140,7 @@ def peaks():
     if f.exists():
         d = json.loads(f.read_text())
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 def shape_spec(w, scale_down=1):
@@ -202,6 +208,28 @@ def cpu_reference_run(w, args, steps, warmup, full=True):
     }
 
 
+DUMP_LOGIT_ROWS = 65536      # rows of the logits kept by --dump-outputs (a fixed, seeded sample of larger outputs)
+
+
+def dump_outputs(out_dir, engine, loss):
+    """What a caller of `RankEngine.run_epoch` holds after the last timed step: the summed loss, the logits of the
+    step (a seeded row sample when there are more than DUMP_LOGIT_ROWS rows) and the parameters it updated; float32
+    .npy files, well under 64 MB in all.  Keeping the logits alive (`engine.keep_logits`) holds one more [N, classes]
+    tensor in the captured graphs' pool than a run without --dump-outputs."""
+    import numpy as np
+    out_dir.mkdir(parents=True, exist_ok=True)
+    torch.cuda.synchronize()
+    np.save(out_dir / "loss.npy", loss.detach().float().reshape(1).cpu().numpy())
+    logits = engine.last_logits
+    if logits.shape[0] > DUMP_LOGIT_ROWS:
+        rows = torch.randperm(logits.shape[0], generator=torch.Generator().manual_seed(0))[:DUMP_LOGIT_ROWS].sort().values
+        np.save(out_dir / "logits_rows.npy", rows.numpy().astype(np.float64))
+        logits = logits[rows.to(logits.device)]
+    np.save(out_dir / "logits.npy", logits.float().cpu().numpy())
+    for name, p in engine.model.named_parameters():
+        np.save(out_dir / f"param.{name}.npy", p.detach().float().cpu().numpy())
+
+
 def teardown(world_size, engine_holder):
     """Leave like a library user would: drop the captured graphs (they hold NCCL kernels), free the engine, destroy
     the process group, return.  A watchdog only fires if communicator teardown hangs."""
@@ -225,6 +253,7 @@ def teardown(world_size, engine_holder):
 def main():
     args = parse()
     w = WORKLOADS[args.workload]
+    args.scale_down *= w.get("scale_down", 1)       # the workload's own fraction of its named shape
     world_size = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -233,13 +262,6 @@ def main():
         if rank != 0:
             return
         steps, warmup = max(1, args.steps), max(0, args.warmup)
-        # the whole run has to end within the driver's limit: ~20 s per full-graph epoch on rmat-1m -> cap the epochs
-        budget = int(os.environ.get("PG_REF_MAX_EPOCHS", "12"))
-        note = None
-        if steps + warmup > budget:
-            warmup = min(warmup, 2)
-            steps = max(1, budget - warmup)
-            note = f"asked for --steps {args.steps} --warmup {args.warmup}; ran {steps} + {warmup} full-graph epochs (time bound)"
         cb = cpu_reference_run(w, args, steps, warmup, full=True)
         line = {"impl": "reference", "metric": "epochs_per_sec", "value": cb["value"], "unit": "epochs/s",
                 "n_gpus": args.gpus, "steps": steps, "warmup": warmup, "ms_per_step": 1e3 / cb["value"],
@@ -248,13 +270,13 @@ def main():
                 "config": {"workload": f"{args.workload}: {w['desc']}", "n_nodes": cb["n_nodes"], "n_edges": cb["n_edges"],
                            "partitions": 1, "partitions_note": "the CPU arm runs ONE partition at every --gpus N "
                            "(all host threads in one process; splitting it over gloo processes shares the same cores)",
-                           "dropout": args.dropout, "steps_note": note},
+                           "dropout": args.dropout},
                 "cpu_baseline": cb,
                 "e2e": {"value": cb["value"], "unit": "epochs/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}
         print(json.dumps(line), flush=True)
         return
 
-    assert torch.cuda.is_available(), "bench.py needs a GPU (use gpurun)"
+    assert torch.cuda.is_available(), "bench.py needs a GPU"
     torch.cuda.set_device(local_rank)
     dev = torch.device(f"cuda:{local_rank}")
     import torch.distributed as dist
@@ -313,6 +335,7 @@ def main():
     eargs = engine_args(w, n_feat, n_class, n_train, world_size, args.dropout, cuda_graph=not args.no_graph,
                         use_pp=args.use_pp)
     engine = RankEngine(layout, eargs, world)
+    engine.keep_logits = args.dump_outputs is not None
     holder = {"engine": engine}
     feat_host = layout.feat.to(engine.dtype).cpu().pin_memory()
     label_host = engine.labels.cpu().pin_memory()
@@ -344,8 +367,10 @@ def main():
         barrier()
         return max_over_ranks(e0.elapsed_time(e1))
 
+    last = {}
+
     def step():
-        engine.run_epoch()
+        last["loss"] = engine.run_epoch()
 
     def step_e2e():
         engine.set_features(feat_host)
@@ -398,6 +423,8 @@ def main():
         ms_total = ms_eager_total * args.steps / n_eager
         wait_s = eager_wait_s
     engine.buffer.check_status()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(Path(args.dump_outputs), engine, last["loss"])
     exposed_s = max_over_ranks(wait_s)
     launches = int(round(launches_per_step * args.steps))
     ms_step = ms_total / args.steps
@@ -409,16 +436,7 @@ def main():
     agg_bytes = sum(nb for _, _, nb in prof)
     n_agg = len(prof)
     achieved = (agg_bytes / 1e9) / (agg_ms / 1e3) if agg_ms > 0 else 0.0
-    traffic, traffic_src = None, None
-    tf = ROOT / "profiles" / "agg_traffic.json"
-    if tf.exists():       # per-launch DRAM bytes of the aggregate kernel from the committed `ncu --set full` captures
-        ent = json.loads(tf.read_text()).get(f"{args.workload}:{world_size}")
-        if isinstance(ent, dict):
-            traffic, traffic_src = ent.get("bytes"), ent.get("source")
-        else:
-            traffic = ent
     roofline = {"bound": "hbm", "achieved": achieved, "peak": hbm_peak, "unit": "GB/s", "frac": achieved / hbm_peak,
-                "traffic": traffic, "traffic_source": traffic_src,
                 "kernel": "pg::agg2_kernel (+fix-up), forward and backward aggregate",
                 "launches": n_agg, "avg_launch_ms": agg_ms / max(n_agg, 1),
                 "algorithmic_bytes_per_launch": agg_bytes / max(n_agg, 1),
@@ -456,6 +474,11 @@ def main():
                       "the features (double-buffered: step i+1's copy overlaps step i's compute) + labels, one D2H read "
                       "of the loss; all K copies inside the timed region"}
 
+    # device memory of this rank: the caching allocator's peak plus what the exchange heaps (cudaMalloc) and the context hold
+    free_b, total_b = torch.cuda.mem_get_info(dev)
+    memory = {"torch_peak_allocated_gb": torch.cuda.max_memory_allocated(dev) / 1e9,
+              "torch_peak_reserved_gb": torch.cuda.max_memory_reserved(dev) / 1e9,
+              "device_used_gb": (total_b - free_b) / 1e9, "device_total_gb": total_b / 1e9}
     clocks = sampler.stop() if sampler else None      # sampled across the eager, replayed and end-to-end regions
     cb = None
     if rank == 0 and world_size == 1 and not args.no_cpu_baseline:
@@ -464,13 +487,6 @@ def main():
         cb = cpu_reference_run(w, args, steps=1 if cpu_full else 2, warmup=1, full=cpu_full)
 
     if rank == 0:
-        secondary = None
-        sf = ROOT / "profiles" / "r2_secondary.json"
-        if sf.exists() and args.workload == "rmat-1m":
-            try:
-                secondary = json.loads(sf.read_text())
-            except Exception:   # noqa: BLE001
-                secondary = None
         line = {
             "metric": "epochs_per_sec", "value": value, "unit": "epochs/s", "n_gpus": world_size,
             "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms_step, "higher_is_better": True,
@@ -481,7 +497,7 @@ def main():
                        "use_pp": args.use_pp, "scale_down": args.scale_down,
                        "n_in_rank0": layout_info["n_in"], "halo_rank0": layout_info["halo"],
                        "nnz_rank0": layout_info["nnz"], "linear": ops.LINEAR_IMPL,
-                       "l2": "per-epoch working set (features, activations, indices) exceeds the 126 MB L2; no flush",
+                       "l2": "per-epoch working set (features, activations, indices) exceeds the 50 MB L2; no flush",
                        "setup_s": round(setup_s, 1)},
             "exposed_comm_s_per_epoch": exposed_s,
             "exposed_comm_frac": exposed_s / (ms_step / 1e3) if ms_step else None,
@@ -489,7 +505,7 @@ def main():
                                 "timed region (graph replays), max over ranks",
             "eager_ms_per_step": ms_eager, "eager_exposed_comm_s_per_epoch": eager_wait_s, "cuda_graph": graph_info,
             "parity": parity, "roofline": roofline, "e2e": e2e, "cpu_baseline": cb, "gpu_launches": launches,
-            "clocks": clocks, "secondary": secondary,
+            "clocks": clocks, "memory": memory,
         }
         print(json.dumps(line), flush=True)
     sys.stdout.flush()

@@ -1,5 +1,5 @@
 /*
- * pipegcn_b200 -- C ABI of the B200-native PipeGCN hot path (libpipegcn_b200.so).
+ * pipegcn_b200 -- C ABI of the H100-native (sm_90a) PipeGCN hot path (libpipegcn_b200.so).
  *
  * The reference (GATECH-EIC/PipeGCN @ 73ab949) is pure Python; it has no FFI.  Its
  * plug-in seam is a set of Python objects (helper/context.py:4-5, module/layer.py:8).
@@ -43,8 +43,8 @@ int pg_device_info(int device, int* sm_arch, int* sm_count, int64_t* l2_bytes);
  * flight per lane group; "agg_pack_short" = 0 | 1; "agg_occ" = 4 | 5; "agg_overlap" = 0 | 1 (short rows on a side
  * stream); "agg_narrow" = 0 | 1 (sub-warp kernels for rows of <= 16 vectors); "agg_l2_hint" = 0 | 1;
  * "ln_stage" = 0 | 1 | 2 (LayerNorm rows through the cp.async ring: never / one vector per lane / always);
- * "ce_subwarp" = 0 | 1 (several cross-entropy rows per warp); "gemm_epi_batch" = 0 | 1, "gemm_epi_slabs" = 1 | 2
- * (GEMM epilogue: TMEM loads of a chunk batched, staging slabs per warp).  Unknown names return PG_ERR_INVALID. */
+ * "ce_subwarp" = 0 | 1 (several cross-entropy rows per warp); "gemm_epi_slabs" = 1 | 2 (GEMM epilogue: staging
+ * slabs per warp).  Unknown names return PG_ERR_INVALID. */
 int pg_set_option(const char* name, int value);
 
 /* ------------------------------------------------------------------------------------------
@@ -102,7 +102,7 @@ typedef struct pg_drop {
  * element (within 1 ulp of `/`).  scratch: fp32 [n_seg * d_pad] where
  * d_pad = d rounded up to 8; may be NULL when n_seg == 0.
  * Replaces graph['_E'].update_all(fn.copy_src, fn.sum) and `/ degs` at
- * /root/reference/module/layer.py:47-50, and their autograd.
+ * PipeGCN/module/layer.py:47-50, and their autograd.
  */
 int pg_aggregate(const pg_csr* g, const void* x, int64_t ldx, void* out, int64_t ldo, int32_t d, int dtype,
                  const float* row_div, int32_t acc_rows, float* scratch, void* stream);
@@ -116,13 +116,13 @@ int pg_row_div(const void* x, int64_t ldx, void* out, int64_t ldo, int32_t n_row
                const float* row_div, void* stream);
 
 /*
- * Dense part of the layer on the tcgen05 tensor cores (SURVEY.md K8/K10):
+ * Dense part of the layer on the Hopper tensor cores (wgmma) (SURVEY.md K8/K10):
  *   c[m, n] = sum_s a_s[m, k_s] * b_s[n, k_s]^T  (+ bias[n])  (/ row_div[m])      1 <= n_src <= 6
- * dtype_in PG_BF16 -> kind::f16 MMA, PG_F32 -> kind::tf32 MMA; fp32 accumulation in TMEM;
+ * dtype_in PG_BF16 -> bf16 wgmma, PG_F32 -> tf32 wgmma; fp32 accumulation in registers;
  * dtype_out selects the element type of c.  n <= 256.  All operands row-major with 16-byte
  * aligned rows (TMA); k tails and the m tail are zero-filled / masked.  `srcs` is a HOST array.
  * Replaces `self.linear1(feat[0:num_dst]) + self.linear2(ah)` at
- * /root/reference/module/layer.py:51 (two pairs: inner rows x W1, neighbour mean x W2,
+ * PipeGCN/module/layer.py:51 (two pairs: inner rows x W1, neighbour mean x W2,
  * bias = b1 + b2) and, with one pair, the dX products of its autograd (row_div = in_deg fuses the
  * `/ degs` gradient).  fp32 parity mode passes the hi/lo halves of pg_split_tf32 as three pairs
  * per product (hi*hi + hi*lo + lo*hi: the "3xTF32" product, fp32-grade accuracy).
@@ -144,10 +144,11 @@ int pg_linear_drop(int dtype_in, int dtype_out, const pg_gemm_src* srcs, int32_t
                    int64_t drop_row0, void* stream);
 
 /*
- * Weight gradients on the tcgen05 tensor cores (MN-major operands, split-K over the rows, deterministic):
+ * Weight gradients on the Hopper tensor cores (MN-major bf16 operands, split-K over the rows, deterministic;
+ * dtype_in must be PG_BF16 -- wgmma transposes 16-bit operands only -- else PG_ERR_UNSUPPORTED):
  *   out[n, k] = sum_s sum_m a_s[m, n] * b_s[m, k]        n, k <= 256, fp32 output, 1 <= n_src <= 6
  * a_s = upstream gradient g [m, n], b_s = layer input [m, k], both row-major with 16-byte aligned rows; `srcs[s].k`
- * is ignored.  Replaces the autograd of /root/reference/module/layer.py:51 for the weights: gW1 = g^T feat[:N_in],
+ * is ignored.  Replaces the autograd of PipeGCN/module/layer.py:51 for the weights: gW1 = g^T feat[:N_in],
  * gW2 = g^T ah (one call each; three pairs per call for the split-fp32 product).  `workspace`: fp32 scratch of
  * pg_wgrad_workspace(m, n, k, dtype_in) floats for the split-K partials.
  */

@@ -1,4 +1,4 @@
-"""Launcher: one process per partition / GPU (entry point of /root/reference/main.py).
+"""Launcher: one process per partition / GPU (entry point of PipeGCN/main.py).
 
     python main.py --dataset synthetic:rmat-1m --n-partitions 4 --n-layers 3 --n-hidden 256 \
         --enable-pipeline --dtype bf16 --partition-method random --no-eval --fix-seed

@@ -1,7 +1,7 @@
 """Oracle: the halo exchange buffer (SURVEY.md §8a rows A1-A9), CPU fp32.
 
 TEST INFRASTRUCTURE (see oracle/__init__.py).  Restates
-/root/reference/helper/feature_buffer.py for one rank, on host tensors, with the
+PipeGCN/helper/feature_buffer.py for one rank, on host tensors, with the
 gloo transfer replaced by an oracle fabric.  What the reference does with
 threads, side streams and events is stated here as the value semantics those
 mechanisms implement (SURVEY.md Appendix A.3/A.4):
@@ -162,7 +162,7 @@ class _Null:
 
 
 class OracleCommTimer:
-    """/root/reference/helper/timer/comm_timer.py:6-33."""
+    """PipeGCN/helper/timer/comm_timer.py:6-33."""
 
     def __init__(self):
         self._time = {}

@@ -2,9 +2,9 @@
  * Oracle SpMM (TEST INFRASTRUCTURE, see oracle/__init__.py).
  *
  * CPU restatement of DGL's `update_all(fn.copy_src, fn.sum)` as used at
- * /root/reference/module/layer.py:47-49 (and its backward on the reversed graph):
+ * PipeGCN/module/layer.py:47-49 (and its backward on the reversed graph):
  *     out[r, :] = sum over e in [indptr[r], indptr[r+1]) of x[indices[e], :]
- * DGL is absent from /root/reference (fork chwan-rice/dgl, unpinned); copy_src + sum
+ * DGL is absent from PipeGCN (fork chwan-rice/dgl, unpinned); copy_src + sum
  * over a 0/1 adjacency is exactly this row-wise sum.  fp32 accumulation in edge order,
  * rows distributed over OpenMP threads (DGL's CPU SpMM is OpenMP-parallel over rows too).
  */

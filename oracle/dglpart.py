@@ -1,9 +1,9 @@
 """Oracle: what `dgl.distributed.partition_graph` + `load_partition` hand to `train.run`.
 
 TEST INFRASTRUCTURE (see oracle/__init__.py).  DGL is a third-party dependency
-absent from /root/reference (fork `chwan-rice/dgl`, unpinned HEAD,
-/root/reference/setup.sh:3); its documented behaviour for the call at
-/root/reference/helper/utils.py:143-144 (`reshuffle=True, balance_edges=False`,
+absent from PipeGCN (fork `chwan-rice/dgl`, unpinned HEAD,
+PipeGCN/setup.sh:3); its documented behaviour for the call at
+PipeGCN/helper/utils.py:143-144 (`reshuffle=True, balance_edges=False`,
 default 1-hop halo) is restated here:
 
 * nodes of partition p get the contiguous global id range
@@ -14,7 +14,7 @@ default 1-hop halo) is restated here:
 * `ndata[dgl.NID]` = reshuffled global ids, `ndata['part_id']` = owner of every
   node, `ndata['inner_node']` = 1 for inner nodes;
 * node features (`feat`, `label`, `in_degree`, `train_mask`) cover inner nodes
-  only (/root/reference/helper/utils.py:105-123).
+  only (PipeGCN/helper/utils.py:105-123).
 """
 from __future__ import annotations
 
@@ -27,7 +27,7 @@ NID = "_ID"   # value of dgl.NID
 
 
 class GraphPartitionBook:
-    """`gpb.partid2nids(i)` (used at /root/reference/train.py:91-92,127; utils.py:171)."""
+    """`gpb.partid2nids(i)` (used at PipeGCN/train.py:91-92,127; utils.py:171)."""
 
     def __init__(self, starts: torch.Tensor):
         self._starts = starts

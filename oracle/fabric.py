@@ -2,11 +2,11 @@
 
 TEST INFRASTRUCTURE (see oracle/__init__.py).  Stands in for the reference's
 `torch.distributed` gloo calls (`dist.isend/irecv` with tags at
-/root/reference/helper/feature_buffer.py:173,179 and `dist.all_reduce` at
-/root/reference/helper/reducer.py:30).  `ThreadFabric` runs a whole world inside
+PipeGCN/helper/feature_buffer.py:173,179 and `dist.all_reduce` at
+PipeGCN/helper/reducer.py:30).  `ThreadFabric` runs a whole world inside
 one process (one Python thread per rank); `GlooFabric` uses a real gloo process
 group, one process per rank, like the reference's launcher
-(/root/reference/main.py:51-57).
+(PipeGCN/main.py:51-57).
 """
 from __future__ import annotations
 

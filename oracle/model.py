@@ -1,7 +1,7 @@
 """Oracle: GraphSAGE-mean layer and model (SURVEY.md §8a rows B1-B6), CPU fp32.
 
 TEST INFRASTRUCTURE (see oracle/__init__.py).  Restates
-/root/reference/module/layer.py and /root/reference/module/model.py with DGL's
+PipeGCN/module/layer.py and PipeGCN/module/model.py with DGL's
 `update_all(fn.copy_src, fn.sum)` (layer.py:47-49) written as the 0/1 CSR product
 `A @ X` and its autograd as `A^T @ g`.
 """

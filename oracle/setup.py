@@ -3,13 +3,13 @@
 TEST INFRASTRUCTURE (see oracle/__init__.py).  Restates, on plain host tensors
 and for all ranks of a simulated world at once:
 
-  get_boundary      /root/reference/helper/utils.py:154-188
-  get_pos           /root/reference/train.py:84-98
-  create_inner_graph/root/reference/train.py:113-117
-  order_graph       /root/reference/train.py:120-131
-  construct         /root/reference/train.py:206-229
-  move_train_first  /root/reference/train.py:134-155
-  get_recv_shape    /root/reference/train.py:101-110
+  get_boundary      PipeGCN/helper/utils.py:154-188
+  get_pos           PipeGCN/train.py:84-98
+  create_inner_graphPipeGCN/train.py:113-117
+  order_graph       PipeGCN/train.py:120-131
+  construct         PipeGCN/train.py:206-229
+  move_train_first  PipeGCN/train.py:134-155
+  get_recv_shape    PipeGCN/train.py:101-110
 """
 from __future__ import annotations
 

@@ -1,7 +1,7 @@
 """Oracle: the per-process training loop (SURVEY.md §8a rows R1, S6; §3.3), CPU fp32.
 
 TEST INFRASTRUCTURE (see oracle/__init__.py).  Restates the part of
-/root/reference/train.py:`run` that the hot path lives in:
+PipeGCN/train.py:`run` that the hot path lives in:
 
   model creation from `torch.manual_seed(args.seed)`   train.py:298-300
   reducer: grad <- sum_ranks(grad / n_train)          helper/reducer.py:23-33, train.py:200-203,304-305

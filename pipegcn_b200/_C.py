@@ -102,7 +102,6 @@ for _k, _v in (("agg_unroll", os.environ.get("PG_AGG_UNROLL")), ("agg_pack_short
                ("agg_occ", os.environ.get("PG_AGG_OCC")), ("agg_overlap", os.environ.get("PG_AGG_OVERLAP")),
                ("agg_narrow", os.environ.get("PG_AGG_NARROW")), ("ln_stage", os.environ.get("PG_LN_STAGE")),
                ("ce_subwarp", os.environ.get("PG_CE_SUBWARP")),
-               ("gemm_epi_batch", os.environ.get("PG_GEMM_EPI_BATCH")),
                ("gemm_epi_slabs", os.environ.get("PG_GEMM_EPI_SLABS"))):
     if _v:
         lib.pg_set_option(_k.encode(), int(_v))

@@ -1,7 +1,7 @@
-"""Builds libpipegcn_b200.so in-tree with nvcc for sm_100a (no torch, no JIT cache).
+"""Builds libpipegcn_b200.so in-tree with nvcc for sm_90a (no torch, no JIT cache).
 
-`python -m pipegcn_b200.build` or `__graft_entry__.build()`.  The shared object is
-git-ignored but travels to the GPU box with the repo snapshot.
+`python -m pipegcn_b200.build` or `__graft_entry__.build()`.  The shared object, its objects and the stamp of the
+sources it was built from are git-ignored: a fresh checkout builds them.
 """
 from __future__ import annotations
 
@@ -16,11 +16,9 @@ CSRC = HERE / "csrc"
 LIB = HERE / "libpipegcn_b200.so"
 STAMP = HERE / ".libpipegcn_b200.stamp"
 
-NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
-    "-O3", "-lineinfo", "-std=c++17", "--shared", "-Xcompiler", "-fPIC",
-    "-cudart", "static",
-]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+COMPILE_FLAGS = ARCH + ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC"]
+LINK_FLAGS = ["--shared", "-cudart", "static"]
 
 
 def sources():
@@ -32,7 +30,7 @@ def _digest() -> str:
     for p in sorted(list(CSRC.glob("*.cu")) + list(CSRC.glob("*.cuh")) + [HERE.parent / "include" / "pipegcn_b200.h"]):
         h.update(p.name.encode())
         h.update(p.read_bytes())
-    h.update(" ".join(NVCC_FLAGS).encode())
+    h.update(" ".join(COMPILE_FLAGS + LINK_FLAGS).encode())
     return h.hexdigest()
 
 
@@ -47,8 +45,7 @@ def build(force: bool = False, verbose: bool = True) -> Path:
     build_dir.mkdir(exist_ok=True)
     for src in sources():
         obj = build_dir / (src.stem + ".o")
-        cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
-               "-Xcompiler", "-fPIC", "-c", str(src), "-o", str(obj)]
+        cmd = [nvcc] + COMPILE_FLAGS + ["-c", str(src), "-o", str(obj)]
         if verbose:
             print(" ".join(cmd), flush=True)
         procs.append((src, subprocess.Popen(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)))
@@ -63,7 +60,7 @@ def build(force: bool = False, verbose: bool = True) -> Path:
             failed = True
     if failed:
         raise RuntimeError("nvcc failed")
-    link = [nvcc, "--shared", "-cudart", "static", "-o", str(LIB)] + objs
+    link = [nvcc] + LINK_FLAGS + ["-o", str(LIB)] + objs
     if verbose:
         print(" ".join(link), flush=True)
     subprocess.run(link, check=True)

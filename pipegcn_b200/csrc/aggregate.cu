@@ -1,4 +1,4 @@
-// CSR neighbour aggregate (SURVEY.md K6/K7 forward, K11 backward) for sm_100a.
+// CSR neighbour aggregate (SURVEY.md K6/K7 forward, K11 backward) for sm_90a.
 //
 //   out[r,:] = ( sum_{e in row r} x[indices[e],:] ) / row_div[r]  (+ out[r,:] if r < acc_rows)
 //
@@ -191,7 +191,7 @@ agg_fixup_kernel(pg_csr g, T* __restrict__ out, int64_t ldo, int nvec, const flo
 }
 
 extern int g_ln_stage, g_ce_subwarp;   // rowops.cu
-extern int g_gemm_epi_batch, g_gemm_epi_slabs;   // linear_tcgen05.cu
+extern int g_gemm_epi_slabs;   // linear_wgmma.cu
 int g_agg_narrow = 1;  // pg_set_option("agg_narrow", 0|1): chunked sub-warp kernels for rows of at most 16 vectors
 int g_agg_overlap = 1; // pg_set_option("agg_overlap", 0|1): short-row kernel on a side stream next to the long-row kernel
 int g_agg_impl = 2;     // pg_set_option("agg_impl", 1|2|3): 1 = row-per-group kernel, 2 = chunked kernels (need pg_csr::chunks),
@@ -199,13 +199,12 @@ int g_agg_impl = 2;     // pg_set_option("agg_impl", 1|2|3): 1 = row-per-group k
 int g_agg_unroll = 8;   // pg_set_option("agg_unroll", 4|8): neighbour rows in flight per group (VPL == 1, agg_impl 1)
 int g_agg_occ = 4;      // pg_set_option("agg_occ", 4|5): resident CTAs per SM the long-row kernel is compiled for (64 / 48 registers)
 int g_agg_l2_hint = 0; // pg_set_option("agg_l2_hint", 0|1): L2 eviction policies by source hotness in the chunked kernels.
-                       // OFF: the policy select costs 5 of 23 instructions per edge on an issue-bound kernel and bought -3 % / +4 %
-                       // (rmat-1m at 1 / 8 partitions) and -2 % (Reddit-shaped): profiles/r2d_agg_bench_*.jsonl
+                       // OFF by default: the policy select costs 5 of 23 instructions per edge; not measured on H100
 
 // ---------------------------------------------------------------------------------------------------------
 // v2: chunked walk over the degree-sorted, permuted CSR (pg_csr::chunks / pidx / prow).
 //
-// ncu on v1 (profiles/r2_agg_v1_stalls.txt): long-scoreboard stalls on a chain of DEPENDENT loads per row --
+// v1 walks a chain of DEPENDENT loads per row --
 // row_order -> indptr -> index -> feature row, then one index + one row load per edge in the scalar tail -- while
 // 77 % of the rows of an RMAT graph have fewer than 8 entries.  Here a warp takes one CHUNK: either up to 32
 // edges' worth of whole rows of equal length (the rows are sorted by length, so a chunk is `n_rows` x `len`), or
@@ -213,10 +212,9 @@ int g_agg_l2_hint = 0; // pg_set_option("agg_l2_hint", 0|1): L2 eviction policie
 // chunk's (next 32) column indices, which are broadcast by shuffles; neighbour rows are fetched U at a time with
 // warp-uniform predicates on the ragged end: the dependent chain per chunk is descriptor -> indices -> rows.
 // L2 residency by source hotness: bit 31 of a permuted column id marks a source row that is referenced often enough
-// to be worth keeping in the 126 MB L2 (the plan marks the most-referenced rows up to a byte budget).  Hot rows are
+// to be worth keeping in the 50 MB L2 (the plan marks the most-referenced rows up to a byte budget).  Hot rows are
 // loaded with an evict_last policy, everything that is touched once or rarely (cold rows, the index stream, the
-// output) with evict_first / streaming hints, so that the long tail does not flush the hubs
-// (profiles/r2_gather_micro.jsonl: an L2-resident gather runs at 20 TB/s, a DRAM-bound one at 8).
+// output) with evict_first / streaming hints, so that the long tail does not flush the hubs.
 __device__ __forceinline__ uint64_t l2_policy_evict_last() {
   uint64_t p;
   asm volatile("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
@@ -451,13 +449,11 @@ agg2_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __res
 
 // ---------------------------------------------------------------------------------------------------------
 // v3 of the long-row kernel: neighbour rows are STAGED THROUGH SHARED MEMORY with asynchronous copies.
-// profiles/r2b_*: the register-landing kernels are bound by latency x bytes in flight -- a load in flight owns its
-// destination registers, and 32 warps x 8 rows x 512 B = 131 KB per SM against ~1.5 us of DRAM-miss latency is
-// ~13 TB/s, where the L2 can feed 20 (tools/gather_micro.cu).  Here every warp owns a ring of D row slots in shared
+// The register-landing kernels are bound by latency x bytes in flight -- a load in flight owns its
+// destination registers (32 warps x 8 rows x 512 B = 131 KB per SM).  Here every warp owns a ring of D row slots in shared
 // memory; `cp.async` (LDGSTS) moves 16 bytes per lane straight from global memory into the ring, one commit group
 // per row, D - 1 rows ahead of the row being added.  A lane reads back exactly the 16 bytes it copied itself, so the
-// ring needs no barrier at all: `cp.async.wait_group` is the only synchronisation.  (TMA `tile::gather4` into the
-// same kind of ring was measured first: 6.2 TB/s against 20 for plain loads -- profiles/r2_gather_micro.jsonl.)
+// ring needs no barrier at all: `cp.async.wait_group` is the only synchronisation.
 __device__ __forceinline__ void cp_async16(uint32_t smem, const void* gmem) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 16;" ::"r"(smem), "l"(gmem) : "memory");
 }
@@ -886,7 +882,7 @@ static int launch_agg2(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t
 }
 
 int g_agg_pack_short = 0;   // pg_set_option("agg_pack_short", 0|1): 16 lanes x 2 vectors per row when rows are short.
-                            // OFF: measured slower (tools/agg_micro.py, P=8 partition: bwd 277 -> 312 us)
+                            // OFF by default; not measured on H100
 
 template <typename T, int VB, int G, int VPL, int U>
 static int launch_agg_u(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec,
@@ -1008,7 +1004,7 @@ static int row_div_t(const void* x, int64_t ldx, void* out, int64_t ldo, int n_r
   const int nvec = static_cast<int>(round_up(d, v) / v);
   const int64_t total = static_cast<int64_t>(n_rows) * nvec;
   if (total == 0) return PG_OK;
-  const unsigned blocks = static_cast<unsigned>(std::min<int64_t>((total + 255) / 256, 148 * 16));
+  const unsigned blocks = static_cast<unsigned>(std::min<int64_t>((total + 255) / 256, sm_count() * 16));
   const T* xp = static_cast<const T*>(x);
   T* op = static_cast<T*>(out);
   switch (vb) {
@@ -1066,10 +1062,6 @@ extern "C" int pg_set_option(const char* name, int value) {
   if (strcmp(name, "gemm_epi_slabs") == 0) {
     PG_REQUIRE(value == 1 || value == 2, "gemm_epi_slabs must be 1 or 2");
     pg::g_gemm_epi_slabs = value;
-    return PG_OK;
-  }
-  if (strcmp(name, "gemm_epi_batch") == 0) {
-    pg::g_gemm_epi_batch = value ? 1 : 0;
     return PG_OK;
   }
   if (strcmp(name, "ce_subwarp") == 0) {

@@ -12,6 +12,18 @@ void set_error(const char* fmt, ...) {
   vsnprintf(g_err, sizeof(g_err), fmt, ap);
   va_end(ap);
 }
+int sm_count() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0;
+    if (cudaGetDevice(&dev) != cudaSuccess ||
+        cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || n <= 0) {
+      cudaGetLastError();
+      n = 132;
+    }
+  }
+  return n;
+}
 }  // namespace pg
 
 extern "C" int pg_abi_version(void) { return PG_ABI_VERSION; }

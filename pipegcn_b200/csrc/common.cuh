@@ -1,4 +1,4 @@
-// Shared device/host helpers of libpipegcn_b200 (sm_100a only).
+// Shared device/host helpers of libpipegcn_b200 (sm_90a).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -10,6 +10,10 @@
 namespace pg {
 
 void set_error(const char* fmt, ...);
+
+// SMs of the current device (132 on an H100 SXM, also the answer without a device): persistent grids and the caps of
+// the grid-stride kernels are multiples of it
+int sm_count();
 
 #define PG_CHECK_CUDA(expr)                                                              \
   do {                                                                                   \
@@ -54,9 +58,15 @@ __device__ __forceinline__ void st_vec(void* p, typename RawVec<VB>::type v) {
   *reinterpret_cast<typename RawVec<VB>::type*>(p) = v;
 }
 
+// ---- fp32 pairs: two round-to-nearest scalar operations (never contracted into a different rounding) ------
+__device__ __forceinline__ float2 add2(float2 a, float2 b) { return make_float2(__fadd_rn(a.x, b.x), __fadd_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 mul2(float2 a, float2 b) { return make_float2(__fmul_rn(a.x, b.x), __fmul_rn(a.y, b.y)); }
+__device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+
 // ---- unpack VB bytes of T into floats / pack back / accumulate -------------------------------
-// Accumulators are float2 pairs so that the adds are the packed fp32x2 instruction of sm_100
-// (FADD2: `__fadd2_rn`), half the issue slots of scalar FADD on this issue-bound gather.
+// Accumulators are float2 pairs: one bf16x2 word unpacks into one pair.
 template <typename T, int VB> struct Pack;
 
 template <int VB> struct Pack<float, VB> {
@@ -81,7 +91,7 @@ template <int VB> struct Pack<float, VB> {
       acc[0].x += p[0];
     } else {
 #pragma unroll
-      for (int i = 0; i < NA; ++i) acc[i] = __fadd2_rn(acc[i], make_float2(p[2 * i], p[2 * i + 1]));
+      for (int i = 0; i < NA; ++i) acc[i] = add2(acc[i], make_float2(p[2 * i], p[2 * i + 1]));
     }
   }
 };
@@ -116,7 +126,7 @@ template <int VB> struct Pack<__nv_bfloat16, VB> {
       const uint32_t* w = reinterpret_cast<const uint32_t*>(&r);
 #pragma unroll
       for (int i = 0; i < NA; ++i)
-        acc[i] = __fadd2_rn(acc[i], make_float2(__uint_as_float(w[i] << 16), __uint_as_float(w[i] & 0xffff0000u)));
+        acc[i] = add2(acc[i], make_float2(__uint_as_float(w[i] << 16), __uint_as_float(w[i] & 0xffff0000u)));
     }
   }
 };
@@ -167,7 +177,14 @@ __device__ __forceinline__ void drop_apply(float (&f)[V], uint64_t i, uint32_t t
     if (k + 1 < V) f[k + 1] = ((h >> 16) >= thresh16) ? f[k + 1] * scale : 0.f;
   }
 }
-// the same function on float2 pairs (packed fp32x2 multiply)
+// one pair of a vector: elements (2 * pair, 2 * pair + 1) of 16-byte vector i, for a kernel whose threads hold pairs
+__device__ __forceinline__ void drop_pair(float& a, float& b, uint64_t i, int pair, uint32_t thresh16, float scale,
+                                          uint32_t seed_lo, uint32_t key) {
+  const uint32_t h = drop_bits(drop_base(i, seed_lo, key), pair);
+  a = ((h & 0xffffU) >= thresh16) ? a * scale : 0.f;
+  b = ((h >> 16) >= thresh16) ? b * scale : 0.f;
+}
+// the same function on float2 pairs
 template <int H>
 __device__ __forceinline__ void drop_apply2(float2 (&f)[H], uint64_t i, uint32_t thresh16, float scale, uint32_t seed_lo,
                                             uint32_t key) {
@@ -176,7 +193,7 @@ __device__ __forceinline__ void drop_apply2(float2 (&f)[H], uint64_t i, uint32_t
 #pragma unroll
   for (int k = 0; k < H; ++k) {
     const uint32_t h = drop_bits(base, k);
-    const float2 m = __fmul2_rn(f[k], sc);
+    const float2 m = mul2(f[k], sc);
     f[k].x = ((h & 0xffffU) >= thresh16) ? m.x : 0.f;
     f[k].y = ((h >> 16) >= thresh16) ? m.y : 0.f;
   }

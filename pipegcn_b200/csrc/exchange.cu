@@ -1,7 +1,7 @@
-// Halo exchange kernels (SURVEY.md K1/K3/K12/K13) for sm_100a: in-kernel P2P stores over
+// Halo exchange kernels (SURVEY.md K1/K3/K12/K13) for sm_90a: in-kernel P2P stores over
 // NVLink/NVSwitch into peer-mapped buffers, sender-side EMA mirror, flag publish / wait,
 // and the ordered boundary add.  These replace the gather -> pinned host -> gloo -> pinned
-// host -> device path of /root/reference/helper/feature_buffer.py:165-194.
+// host -> device path of PipeGCN/helper/feature_buffer.py:165-194.
 #include <algorithm>
 #include <string.h>
 #include "common.cuh"
@@ -317,7 +317,7 @@ extern "C" int pg_scale_rows(const void* src, int64_t ld_src, void* dst, int64_t
   const int v = vb / es;
   const int nvec = static_cast<int>(pg::round_up(d, v) / v);
   const int64_t total = static_cast<int64_t>(n_rows) * nvec;
-  const unsigned blocks = static_cast<unsigned>(std::min<int64_t>((total + 255) / 256, 148 * 16));
+  const unsigned blocks = static_cast<unsigned>(std::min<int64_t>((total + 255) / 256, pg::sm_count() * 16));
 #define PG_SCALE(T_, VB_) pg::scale_rows_kernel<T_, VB_><<<blocks, 256, 0, st>>>(static_cast<const T_*>(src), ld_src, static_cast<T_*>(dst), ld_dst, n_rows, nvec, momentum, corr, k_host, k_dev)
   if (dtype == PG_F32) {
     if (vb == 16) PG_SCALE(float, 16); else if (vb == 8) PG_SCALE(float, 8); else PG_SCALE(float, 4);

@@ -1,8 +1,8 @@
-// Row-wise epilogue kernels of the layer loop (SURVEY.md K9, K14), sm_100a, HBM-bound:
-//   * LayerNorm + ReLU forward in one pass              (/root/reference/module/model.py:53-56)
+// Row-wise epilogue kernels of the layer loop (SURVEY.md K9, K14), sm_90a, HBM-bound:
+//   * LayerNorm + ReLU forward in one pass              (PipeGCN/module/model.py:53-56)
 //   * its backward, fused with the three column reductions the step needs (d gamma, d beta and the
 //     bias gradient of the linear that produced the pre-norm tensor)
-//   * summed soft-max cross-entropy forward / backward  (/root/reference/train.py:320,351)
+//   * summed soft-max cross-entropy forward / backward  (PipeGCN/train.py:320,351)
 // One warp owns one row; a row of up to 32 lanes x kMaxVec 16-byte vectors stays in registers between
 // the statistics pass and the output pass, so every tensor is read once and written once.
 // Column reductions are two-stage and deterministic: per-CTA partials, then a fixed-order sum.
@@ -16,8 +16,7 @@ namespace pg {
 constexpr int kRowThreads = 256;
 constexpr int kMaxVec = 4;          // vectors per lane kept in registers (bf16: d <= 1024, fp32: d <= 512)
 // pg_set_option("ln_stage", 0|1|2): LayerNorm kernels read their rows through the cp.async ring never / when a lane
-// holds one 16-byte vector per row (rows of up to 512 bytes: measured 0.237 -> 0.210 ms forward, 0.351 -> 0.312 ms
-// backward on [1 M, 256] bf16; at two vectors per lane plain loads are 2-5 % faster) / always
+// holds one 16-byte vector per row (rows of up to 512 bytes) / always.  The default has not been re-measured on H100.
 int g_ln_stage = 1;
 int g_ce_subwarp = 1;               // pg_set_option("ce_subwarp", 0|1): cross-entropy kernels with several rows per warp
 
@@ -71,7 +70,7 @@ __device__ __forceinline__ float max_nan(float v, float lo) {
 }
 // the affine LayerNorm output of one element; forward and backward (ReLU mask recomputation) MUST round identically
 __device__ __forceinline__ float2 ln_affine2(float2 centered, float2 rstd, float2 g, float2 b) {
-  return __ffma2_rn(__fmul2_rn(centered, rstd), g, b);
+  return fma2(mul2(centered, rstd), g, b);
 }
 
 // ---- per-lane asynchronous staging ring ----------------------------------------------------------------------------
@@ -104,8 +103,8 @@ __device__ __forceinline__ void load_affine(const float* sm, int nv, int vec, fl
   }
 }
 
-// a 16-byte vector as H float2 pairs: the row kernels do their arithmetic with the packed fp32x2 instructions of
-// sm_100 (FADD2 / FMUL2 / FFMA2: two IEEE round-to-nearest results per issue slot, bit-identical to the scalar ops)
+// a 16-byte vector as H float2 pairs: the row kernels do their arithmetic on pairs (add2 / mul2 / fma2 of common.cuh:
+// IEEE round-to-nearest, never contracted, so forward and backward round identically)
 template <typename T> struct Pair;
 template <> struct Pair<float> {
   static constexpr int H = 2;
@@ -193,7 +192,7 @@ ln_relu_fwd_kernel(const T* __restrict__ y, int64_t ldy, const float* __restrict
           for (int k = 0; k < H; ++k) x[r][j][k] = make_float2(0.f, 0.f);
         }
 #pragma unroll
-        for (int k = 0; k < H; ++k) acc = __fadd2_rn(acc, x[r][j][k]);
+        for (int k = 0; k < H; ++k) acc = add2(acc, x[r][j][k]);
       }
       s[r] = acc.x + acc.y;
     }
@@ -208,9 +207,9 @@ ln_relu_fwd_kernel(const T* __restrict__ y, int64_t ldy, const float* __restrict
       for (int j = 0; j < VPL; ++j)
 #pragma unroll
         for (int k = 0; k < H; ++k) {
-          const float2 c = act[j] ? __fadd2_rn(x[r][j][k], neg) : make_float2(0.f, 0.f);
+          const float2 c = act[j] ? add2(x[r][j][k], neg) : make_float2(0.f, 0.f);
           x[r][j][k] = c;
-          acc = __ffma2_rn(c, c, acc);
+          acc = fma2(c, c, acc);
         }
       q[r] = acc.x + acc.y;
     }
@@ -360,11 +359,11 @@ ln_relu_bwd_kernel(const T* __restrict__ g_out, int64_t ldg, const T* __restrict
       if (MODE == 2) load_affine<H>(sb, NV, lane + j * 32, bt);
 #pragma unroll
       for (int k = 0; k < H; ++k) {
-        const float2 c = __fadd2_rn(yy[k], neg_mu);
-        const float2 xx = __fmul2_rn(c, rs2);
+        const float2 c = add2(yy[k], neg_mu);
+        const float2 xx = mul2(c, rs2);
         float2 gg = g[k];
         if (MODE == 2) {
-          const float2 v = __ffma2_rn(xx, gm[k], bt[k]);          // == ln_affine2(c, rs2, gm, bt): the forward's value
+          const float2 v = fma2(xx, gm[k], bt[k]);          // == ln_affine2(c, rs2, gm, bt): the forward's value
           gg.x = v.x > 0.f ? gg.x : 0.f;
           gg.y = v.y > 0.f ? gg.y : 0.f;
         }
@@ -372,13 +371,13 @@ ln_relu_bwd_kernel(const T* __restrict__ g_out, int64_t ldg, const T* __restrict
           gg.x = o[k].x > 0.f ? gg.x : 0.f;
           gg.y = o[k].y > 0.f ? gg.y : 0.f;
         }
-        const float2 gv = __fmul2_rn(gg, gm[k]);
+        const float2 gv = mul2(gg, gm[k]);
         xh[j][k] = xx;
         gx[j][k] = gv;
-        s1 = __fadd2_rn(s1, gv);
-        s2 = __ffma2_rn(gv, xx, s2);
-        cg[j][k] = __ffma2_rn(gg, xx, cg[j][k]);
-        cb[j][k] = __fadd2_rn(cb[j][k], gg);
+        s1 = add2(s1, gv);
+        s2 = fma2(gv, xx, s2);
+        cg[j][k] = fma2(gg, xx, cg[j][k]);
+        cb[j][k] = add2(cb[j][k], gg);
       }
     }
     float st[2] = {s1.x + s1.y, s2.x + s2.y};
@@ -390,12 +389,12 @@ ln_relu_bwd_kernel(const T* __restrict__ g_out, int64_t ldg, const T* __restrict
       if (act[j]) {
         float2 o[H];
 #pragma unroll
-        for (int k = 0; k < H; ++k) o[k] = __ffma2_rn(xh[j][k], k2, __ffma2_rn(gx[j][k], rs2, k1));
+        for (int k = 0; k < H; ++k) o[k] = fma2(xh[j][k], k2, fma2(gx[j][k], rs2, k1));
         st_vec<16>(g_y + off(row, ldgy, j), Q::pack(o));
         // the tensor handed upstream is stored in T: reduce what is stored
         Q::round_trip(o);
 #pragma unroll
-        for (int k = 0; k < H; ++k) cy[j][k] = __fadd2_rn(cy[j][k], o[k]);
+        for (int k = 0; k < H; ++k) cy[j][k] = add2(cy[j][k], o[k]);
       }
   };
 
@@ -725,7 +724,7 @@ dropout_kernel(const T* __restrict__ x, int64_t ldx, T* __restrict__ out, int64_
 
 static int row_grid(int n_rows) {
   const int need = (n_rows + (kRowThreads / 32) - 1) / (kRowThreads / 32);
-  return need < 148 * 8 ? (need > 0 ? need : 1) : 148 * 8;
+  return need < sm_count() * 8 ? (need > 0 ? need : 1) : sm_count() * 8;
 }
 
 }  // namespace pg
@@ -742,7 +741,7 @@ extern "C" int pg_dropout_rows(const void* x, int64_t ldx, void* out, int64_t ld
   const int nvec = static_cast<int>(round_up(d, v) / v);
   const int64_t total = static_cast<int64_t>(n_rows) * nvec;
   if (total == 0) return PG_OK;
-  const unsigned blocks = static_cast<unsigned>((total + 255) / 256 < 148 * 16 ? (total + 255) / 256 : 148 * 16);
+  const unsigned blocks = static_cast<unsigned>((total + 255) / 256 < sm_count() * 16 ? (total + 255) / 256 : sm_count() * 16);
   DropArg a = make_drop(drop);
   if (drop->p == 0.f) { a.thresh16 = 0u; a.scale = 1.f; }
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -782,7 +781,7 @@ extern "C" int pg_ln_relu_drop_fwd(const void* y, int64_t ldy, const float* gamm
   const int vpl = (d / v + 31) / 32;
   const bool full = d / v == 32 * vpl;
   // one resident wave (the kernels are compiled for 4 CTAs per SM, 3 when a lane holds more than 16 floats)
-  const int grid = std::min(row_grid(n_rows), 148 * 4);
+  const int grid = std::min(row_grid(n_rows), sm_count() * 4);
   // rows per warp iteration R and ring stages S by vectors per lane: R * VPL * S * 16 bytes per lane = 32 KB per CTA
 #define PG_LNF__(T_, VPL_, R_, F_, S_) ln_relu_fwd_kernel<T_, VPL_, R_, F_, S_><<<grid, kRowThreads, (S_) * (R_) * (VPL_) * kRowThreads * 16, st>>>(static_cast<const T_*>(y), ldy, gamma, beta, eps, relu, static_cast<T_*>(out), ldo, mean, rstd, n_rows, d, static_cast<T_*>(out_clean), ldc, da)
 #define PG_LNF_(T_, VPL_, R_, S_) do { if (full) PG_LNF__(T_, VPL_, R_, true, S_); else PG_LNF__(T_, VPL_, R_, false, S_); } while (0)
@@ -821,7 +820,7 @@ extern "C" int pg_ln_relu_bwd2(const void* g_out, int64_t ldg, const void* out, 
   const size_t red_bytes = 3 * static_cast<size_t>(d) * sizeof(float);
   const int vpl = (d / v + 31) / 32;
   // one resident wave: every CTA pays the column-partial epilogue once (`partial` is sized for row_grid(n_rows) CTAs)
-  const int grid = std::min(row_grid(n_rows), 148 * (vpl * v <= 8 ? 3 : (vpl * v <= 16 ? 2 : 1)));
+  const int grid = std::min(row_grid(n_rows), sm_count() * (vpl * v <= 8 ? 3 : (vpl * v <= 16 ? 2 : 1)));
   const bool full = d / v == 32 * vpl;
   const int mode = !relu ? 0 : (beta != nullptr ? 2 : 1);
 #define PG_LNB___(T_, VPL_, M_, F_, S_) ln_relu_bwd_kernel<T_, VPL_, M_, F_, S_><<<grid, kRowThreads, (S_) * 2 * (VPL_) * kRowThreads * 16 + red_bytes, st>>>(static_cast<const T_*>(g_out), ldg, static_cast<const T_*>(out), ldo, static_cast<const T_*>(y), ldy, mean, rstd, gamma, static_cast<T_*>(g_y), ldgy, partial, n_rows, d, beta)

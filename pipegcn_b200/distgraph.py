@@ -1,7 +1,7 @@
 """Per-rank construction of a large synthetic graph and of this rank's `PartitionLayout`.
 
 `PartitionPlan` (pipegcn_b200/partition.py) starts from the GLOBAL edge list, like the reference, whose every process
-loads the whole DGL graph before `partition_graph` (/root/reference/helper/utils.py:132-144).  At the
+loads the whole DGL graph before `partition_graph` (PipeGCN/helper/utils.py:132-144).  At the
 ogbn-papers100M shape (111 M nodes, 1.6 B edges) no rank can hold that.  Here every rank streams the SAME seeded RMAT
 pair stream in chunks and keeps only the edges whose destination it owns, so the largest array a rank ever holds is its
 own ~1/P of the edges:

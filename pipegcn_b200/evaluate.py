@@ -1,9 +1,9 @@
 """Accuracy evaluation and checkpointing around the hot path.
 
-Counterparts of /root/reference/train.py: `calc_acc` (:11-17), `evaluate_induc`
+Counterparts of PipeGCN/train.py: `calc_acc` (:11-17), `evaluate_induc`
 (:20-39), `evaluate_trans` (:42-61) and the best-model bookkeeping of `run`
 (:377-400).  The reference deep-copies the model, moves it to the CPU and evaluates on
-the whole DGL graph from a worker thread; here the SAME sm_100a kernels evaluate the
+the whole DGL graph from a worker thread; here the SAME sm_90a kernels evaluate the
 homogeneous full graph on the GPU (the eval branch of GraphSAGELayer, layer.py:52-62),
 on the training stream, from the live weights.
 """

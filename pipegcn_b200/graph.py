@@ -1,8 +1,8 @@
 """The graph object handed to the layers: CSR + CSC of one partition on the GPU.
 
 Takes the place of the DGL heterograph `('_U','_E','_V')` that
-/root/reference/train.py:`construct` builds (train.py:206-229) and
-/root/reference/module/layer.py:38-51 consumes; only `num_nodes('_U' | '_V')`
+PipeGCN/train.py:`construct` builds (train.py:206-229) and
+PipeGCN/module/layer.py:38-51 consumes; only `num_nodes('_U' | '_V')`
 and the adjacency survive.
 """
 from __future__ import annotations
@@ -73,9 +73,10 @@ class CsrPlan:
             start = self.indptr.to(torch.int64)[order]
             pos = torch.repeat_interleave(start - pptr[:-1], ldeg) + torch.arange(self.nnz, **i64)
             pidx = self.indices[pos]
-            # "hot" source rows: the most referenced ones, as many as fit a byte budget of the L2 (126 MB); the kernel
-            # loads them with an evict_last policy and everything else with evict_first (bit 31 of the column id)
-            budget_rows = int(float(os.environ.get("PG_HOT_MB", "64")) * 2 ** 20) // max(self.row_bytes_hint, 1)
+            # "hot" source rows: the most referenced ones, as many as fit a byte budget of about half the 50 MB L2; the
+            # kernel loads them with an evict_last policy and everything else with evict_first (bit 31 of the column id).
+            # The hints are off by default (agg_l2_hint) and have not been measured on H100.
+            budget_rows = int(float(os.environ.get("PG_HOT_MB", "24")) * 2 ** 20) // max(self.row_bytes_hint, 1)
             refs = torch.bincount(self.indices.to(torch.int64))
             if budget_rows > 0:
                 if refs.numel() > budget_rows:

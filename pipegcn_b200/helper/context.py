@@ -1,8 +1,8 @@
 """Process-global hot-path objects -- the plug-in seam of the reference.
 
-/root/reference/helper/context.py:4-5 holds `buffer = Buffer()` and
+PipeGCN/helper/context.py:4-5 holds `buffer = Buffer()` and
 `reducer = Reducer()`; model code reaches them as `ctx.buffer` / `ctx.reducer`
-(/root/reference/module/model.py:46, /root/reference/train.py:283,302,357,360).
+(PipeGCN/module/model.py:46, PipeGCN/train.py:283,302,357,360).
 Replacing these two objects is how this engine drops in.
 """
 from .feature_buffer import Buffer

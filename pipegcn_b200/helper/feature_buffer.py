@@ -1,6 +1,6 @@
 """`Buffer`: the halo feature / gradient exchange of one rank, NVLink-native.
 
-Same public surface as /root/reference/helper/feature_buffer.py (`init_buffer`
+Same public surface as PipeGCN/helper/feature_buffer.py (`init_buffer`
 :45-46, `update` :143, `next_epoch` :129) with the data path replaced:
 
 reference                                             here

@@ -1,4 +1,4 @@
-"""Command line of the trainer: the flags of /root/reference/helper/parser.py:8-69.
+"""Command line of the trainer: the flags of PipeGCN/helper/parser.py:8-69.
 
 Same names, aliases and defaults, with three deliberate differences: `--backend`
 defaults to `nccl` (the reference implements gloo only; this engine implements the
@@ -47,7 +47,7 @@ _FLAGS = [
 
 
 def build_parser():
-    parser = argparse.ArgumentParser(description='PipeGCN on B200')
+    parser = argparse.ArgumentParser(description='PipeGCN on H100')
     for flag, kw in _FLAGS:
         names = ["--" + flag]
         if "-" in flag:

@@ -1,6 +1,6 @@
 """`Reducer`: gradient all-reduce, kept as a plain NCCL call (BASELINE north_star).
 
-Semantics of /root/reference/helper/reducer.py:23-33 + train.py:200-203,304-305:
+Semantics of PipeGCN/helper/reducer.py:23-33 + train.py:200-203,304-305:
 every parameter gradient becomes  sum over ranks of (grad / n_train)  with n_train the
 GLOBAL number of training nodes.  The reference copies each gradient to pinned host
 memory and all-reduces it over gloo in its own process group from a pool thread; here

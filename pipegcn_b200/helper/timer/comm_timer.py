@@ -1,6 +1,6 @@
 """`CommTimer`: exposed (non-overlapped) communication time per epoch.
 
-Keeps the interface of /root/reference/helper/timer/comm_timer.py:6-33 -- named
+Keeps the interface of PipeGCN/helper/timer/comm_timer.py:6-33 -- named
 sections `forward_<l>` / `backward_<l>`, `tot_time()`, `clear()`, duplicate names
 raise -- but measures on the device: a section is the pair of CUDA events that
 brackets the flag-wait kernel on the compute stream, i.e. the time the compute

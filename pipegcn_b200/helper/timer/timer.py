@@ -1,4 +1,4 @@
-"""Process-global communication timer (mirrors /root/reference/helper/timer/timer.py:3)."""
+"""Process-global communication timer (mirrors PipeGCN/helper/timer/timer.py:3)."""
 from .comm_timer import CommTimer
 
 comm_timer = CommTimer()

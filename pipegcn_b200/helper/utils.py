@@ -1,6 +1,6 @@
 """Data / partition helpers on the path into the hot loop.
 
-Counterparts of /root/reference/helper/utils.py: `load_data` (:74-96),
+Counterparts of PipeGCN/helper/utils.py: `load_data` (:74-96),
 `graph_partition` (:132-144), `load_partition` (:99-129), `get_layer_size` (:147-151).
 The reference's datasets need DGL, ogb and a network; this engine accepts
 `synthetic:<shape>` datasets (pipegcn_b200/synthetic.py).  The reference's own dataset

@@ -1,4 +1,4 @@
-"""`--partition-method metis` (/root/reference/helper/parser.py:39-41, helper/utils.py:143-144).
+"""`--partition-method metis` (PipeGCN/helper/parser.py:39-41, helper/utils.py:143-144).
 
 The reference partitions through DGL, which calls METIS `PartGraphKway` with the `cut` or `vol` objective.  DGL is
 absent; METIS itself ships as a static library inside the CUDA toolkit (`libmetis_static.a`, idx_t = int64,

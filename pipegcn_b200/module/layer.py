@@ -1,6 +1,6 @@
-"""`GraphSAGELayer`: neighbour mean + two linears, on the sm_100a kernels.
+"""`GraphSAGELayer`: neighbour mean + two linears, on the sm_90a kernels.
 
-API and parameters of /root/reference/module/layer.py:8-63 (state_dict keys
+API and parameters of PipeGCN/module/layer.py:8-63 (state_dict keys
 `linear1.*`, `linear2.*`, or `linear.*` with use_pp; init U(-1/sqrt(in), 1/sqrt(in))
 for weights and biases drawn in the reference's order so that equal seeds give equal
 weights).  `graph` is a `pipegcn_b200.graph.PartGraph` instead of a DGL heterograph.

@@ -1,4 +1,4 @@
-"""`GraphSAGE` (alias `GCN`): the layer loop of /root/reference/module/model.py:25-58.
+"""`GraphSAGE` (alias `GCN`): the layer loop of PipeGCN/module/model.py:25-58.
 
 Per graph layer: `buffer.update` (halo exchange) -> dropout -> GraphSAGELayer -> norm ->
 activation; trailing `n_linear` plain linears.  The reference defines no `GCN` class

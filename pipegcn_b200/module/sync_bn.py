@@ -1,4 +1,4 @@
-"""`SyncBatchNorm` for `--norm batch` (/root/reference/module/sync_bn.py:7-56).
+"""`SyncBatchNorm` for `--norm batch` (PipeGCN/module/sync_bn.py:7-56).
 
 Batch statistics over the rows of ALL partitions: sum(x) and sum(x^2) are all-reduced in the forward, sum(g) and
 sum(g * x_hat) in the backward; `whole_size` is the divisor (the reference passes the global number of training

@@ -1,6 +1,6 @@
 """torch-facing wrappers of the C-ABI kernels (PyTorch tensors in, PyTorch tensors out).
 
-Each autograd Function mirrors one step of /root/reference/module/layer.py:44-51 and
+Each autograd Function mirrors one step of the reference's module/layer.py:44-51 and
 its autograd; nothing here computes on the host or falls back to torch kernels for
 the aggregate / exchange path.
 """
@@ -136,8 +136,8 @@ def sage_aggregate(feat: torch.Tensor, graph: PartGraph, deg_f: torch.Tensor = N
     return SageAggregate.apply(feat, graph, graph.in_deg_f if deg_f is None else deg_f)
 
 
-# ---- dense part: hand-written tcgen05 GEMM (csrc/linear_tcgen05.cu) -----------------------------
-LINEAR_IMPL = "tcgen05 (pg_linear / pg_wgrad: TMA + tcgen05.mma kind::f16 / 3xTF32, TMEM accumulators; dW MN-major split-K)"
+# ---- dense part: hand-written wgmma GEMMs (csrc/linear_wgmma.cu, csrc/wgrad_wgmma.cu) -----------
+LINEAR_IMPL = "wgmma (pg_linear / pg_wgrad: TMA + wgmma.mma_async bf16 / 3xTF32, register accumulators; dW MN-major bf16 split-K)"
 
 
 def _tma_ready(t: torch.Tensor) -> torch.Tensor:
@@ -171,7 +171,7 @@ def split_tf32(x: torch.Tensor):
 
 
 # fp32 activations: "3xtf32" = hi*hi + hi*lo + lo*hi on the tf32 tensor cores (fp32-grade accuracy, the
-# parity mode); "tf32" = one pass (rel. error ~1e-3).  bf16 activations always use one kind::f16 pass.
+# parity mode); "tf32" = one pass (rel. error ~1e-3).  bf16 activations always use one bf16 pass.
 FP32_GEMM = os.environ.get("PG_FP32_GEMM", "3xtf32")
 
 
@@ -206,7 +206,7 @@ def _halves(t):
 
 def gemm_nt(a0, b0, a1=None, b1=None, bias=None, row_div=None, out=None, out_dtype=None, drop=None,
             drop_row0: int = 0) -> torch.Tensor:
-    """out[m, n] = a0 @ b0^T (+ a1 @ b1^T) (+ bias) (/ row_div[:, None]) on the tcgen05 tensor cores.  Operands may be
+    """out[m, n] = a0 @ b0^T (+ a1 @ b1^T) (+ bias) (/ row_div[:, None]) on the tensor cores.  Operands may be
     `Split` objects (fp32 operands split once by the caller).  `drop`: dropout mask applied to `out` as it is written
     (out's first row is row `drop_row0` of the tensor the mask is defined on)."""
     raw = [(a0, b0)] + ([(a1, b1)] if a1 is not None else [])
@@ -259,13 +259,10 @@ def gemm_nt(a0, b0, a1=None, b1=None, bias=None, row_div=None, out=None, out_dty
     return out
 
 
-# fp32 weight gradients: "3xtf32" = MN-major kind::tf32 with hi/lo splits, "bf16x3" = six MN-major kind::f16 products
-WGRAD_FP32 = os.environ.get("PG_WGRAD_FP32", "3xtf32")
-
-
-def _split_bf16x3(x: torch.Tensor):
+def _split_bf16(x: torch.Tensor, terms: int):
+    """x = b0 + b1 + ... in bf16 (three terms carry every bit of an fp32 value)."""
     out, r = [], x.float()
-    for _ in range(3):
+    for _ in range(terms):
         b = alloc_rows(x.shape[0], x.shape[1], torch.bfloat16, x.device)
         b.copy_(r)
         out.append(b)
@@ -275,22 +272,23 @@ def _split_bf16x3(x: torch.Tensor):
 
 
 def wgrad(g: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
-    """g^T @ x  -> fp32 [n, k]: the weight gradient of `x @ W^T` on the tcgen05 tensor cores (pg_wgrad: MN-major
-    operands straight from the row-major activations, split-K over the rows, fixed-order reduction)."""
-    gs, xs = g, x
+    """g^T @ x  -> fp32 [n, k]: the weight gradient of `x @ W^T` on the tensor cores (pg_wgrad: MN-major bf16
+    operands straight from the row-major activations, split-K over the rows, fixed-order reduction).  The tensor core
+    transposes 16-bit operands only, so fp32 activations go in as sums of bf16 terms."""
     g, x = _rows(_plain(g)), _rows(_plain(x))
     m, n, k = g.shape[0], g.shape[1], x.shape[1]
     assert x.shape[0] == m and g.dtype == x.dtype
     out = torch.empty(n, k, dtype=torch.float32, device=g.device)
     if m == 0:
         return out.zero_()
-    if g.dtype == torch.float32 and FP32_GEMM == "3xtf32" and WGRAD_FP32 == "3xtf32":
-        (gh, gl), (xh, xl) = _halves(gs), _halves(xs)
-        pairs = [(gh, xh), (gh, xl), (gl, xh)]
-    elif g.dtype == torch.float32 and FP32_GEMM == "3xtf32":
+    if g.dtype == torch.float32 and FP32_GEMM == "3xtf32":
         # fp32 = b0 + b1 + b2 exactly (three bf16 terms): six bf16 products carry the product to ~2^-24
-        g3, x3 = _split_bf16x3(g), _split_bf16x3(x)
+        g3, x3 = _split_bf16(g, 3), _split_bf16(x, 3)
         pairs = [(g3[0], x3[0]), (g3[0], x3[1]), (g3[1], x3[0]), (g3[0], x3[2]), (g3[2], x3[0]), (g3[1], x3[1])]
+    elif g.dtype == torch.float32:
+        # one-pass mode: two bf16 terms, three products (~2^-16, finer than one tf32 pass)
+        g2, x2 = _split_bf16(g, 2), _split_bf16(x, 2)
+        pairs = [(g2[0], x2[0]), (g2[0], x2[1]), (g2[1], x2[0])]
     else:
         pairs = [(_tma_ready(g), _tma_ready(x))]
     code = _C.dtype_code(pairs[0][0].dtype)
@@ -396,7 +394,7 @@ class SageLayerNarrowFn(torch.autograd.Function):
         out = feat[:N_in] @ W1^T + (b1 + b2)       [N_in, d_out]      pg_linear
         out += (A @ z) / in_deg                                       pg_aggregate, accumulating, division fused
 
-    (A F) W = A (F W): the aggregate -- the HBM/L2-bound part of /root/reference/module/layer.py:47-51 -- moves
+    (A F) W = A (F W): the aggregate -- the HBM/L2-bound part of PipeGCN/module/layer.py:47-51 -- moves
     d_out-wide rows instead of d_in-wide ones (4x fewer bytes for the 256 -> 64 output layer of the headline config).
     Backward: dz = A^T (g / in_deg) [num_all, d_out], g_feat = dz @ W2 (+ g @ W1 on the inner rows),
     gW2 = dz^T feat, gW1 = g^T feat[:N_in].  Same sums, different association: fp32 results agree with the

@@ -1,8 +1,8 @@
 """Per-partition index spaces of the hot path (SURVEY.md §8a rows S1-S4, Appendix A).
 
 The reference derives these per process from a DGL partition through
-`get_boundary` (/root/reference/helper/utils.py:154-188), `get_pos`
-(/root/reference/train.py:84-98), `order_graph`/`construct` (train.py:120-131,
+`get_boundary` (PipeGCN/helper/utils.py:154-188), `get_pos`
+(PipeGCN/train.py:84-98), `order_graph`/`construct` (train.py:120-131,
 206-229), `move_train_first` (train.py:134-155) and `get_recv_shape`
 (train.py:101-110).  Here the same layouts are produced in one vectorised pass
 over the global edge list (torch, host or GPU), without DGL:
@@ -179,5 +179,5 @@ def build_layouts(g: GlobalGraph, part: torch.Tensor, n_parts: int, ranks=None) 
 
 
 def get_layer_size(n_feat: int, n_hidden: int, n_class: int, n_layers: int) -> List[int]:
-    """[n_feat, h, ..., h, n_class] with n_layers+1 entries (/root/reference/helper/utils.py:147-151)."""
+    """[n_feat, h, ..., h, n_class] with n_layers+1 entries (PipeGCN/helper/utils.py:147-151)."""
     return [n_feat] + [n_hidden] * (n_layers - 1) + [n_class]

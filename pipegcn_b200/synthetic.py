@@ -1,7 +1,7 @@
 """Synthetic graphs of the shapes BASELINE.json names (SURVEY.md §8d).
 
 The reference loads Reddit / ogbn-* through DGL + network downloads
-(/root/reference/helper/utils.py:74-96); neither is available, so the engine is
+(PipeGCN/helper/utils.py:74-96); neither is available, so the engine is
 fed seeded RMAT graphs with the same global preprocessing the reference applies
 after loading: drop self loops, then add exactly one self loop per node
 (utils.py:94-95).  Everything is plain torch so the same code runs on the host
@@ -143,7 +143,7 @@ def make_graph(shape: str | dict, seed_graph: int = 0, seed_feat: int = 2, seed_
 
 
 def random_partition(n_nodes: int, n_parts: int, seed: int = 1, device="cpu") -> torch.Tensor:
-    """`--partition-method random` (/root/reference/helper/parser.py:41): uniform assignment."""
+    """`--partition-method random` (PipeGCN/helper/parser.py:41): uniform assignment."""
     gen = torch.Generator(device=torch.device(device))
     gen.manual_seed(seed)
     part = torch.randint(0, n_parts, (n_nodes,), generator=gen, device=device)
@@ -165,5 +165,5 @@ def induced_subgraph(g: GlobalGraph, keep: torch.Tensor):
 
 def train_subgraph(g: GlobalGraph) -> GlobalGraph:
     """`--inductive`: the graph induced by the training nodes (`g.subgraph(g.ndata['train_mask'])`,
-    /root/reference/main.py:34-35, helper/utils.py:226-230)."""
+    PipeGCN/main.py:34-35, helper/utils.py:226-230)."""
     return induced_subgraph(g, g.train_mask)[0]

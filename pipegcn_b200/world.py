@@ -1,7 +1,7 @@
 """Who the peers are and how their memory is reached.
 
 `DistWorld`: one process per GPU under torch.distributed (the reference's process
-model, /root/reference/main.py:51-57); peers' symmetric heaps are mapped with CUDA
+model, PipeGCN/main.py:51-57); peers' symmetric heaps are mapped with CUDA
 IPC and written over NVLink/NVSwitch from inside the exchange kernels.
 
 `LocalWorld`: all ranks of a world live in this process on ONE GPU (peer pointers

@@ -1,15 +1,16 @@
-"""Generate the golden fixtures by running the UNMODIFIED reference (/root/reference) on the host.
+"""Generate the golden fixtures by running the UNMODIFIED reference (a checkout of GATECH-EIC/PipeGCN,
+named by the environment variable PIPEGCN_REF) on the host.
 
-    python tests/golden/make_golden.py            # writes tests/golden/ref_*.pt   (build container only)
+    python tests/golden/make_golden.py            # writes tests/golden/ref_*.pt
 
-One gloo process per partition, exactly like /root/reference/main.py:51-57.  Every hot-path object is the
+One gloo process per partition, exactly like PipeGCN/main.py:51-57.  Every hot-path object is the
 reference's own: `helper.context.buffer` (helper/feature_buffer.py), `module.model.GraphSAGE` /
 `module.layer.GraphSAGELayer`, `helper.context.reducer` (helper/reducer.py), and the set-up helpers of train.py /
 helper/utils.py (`create_inner_graph`, `move_to_cuda`, `get_boundary`, `get_pos`, `order_graph`, `construct`,
 `move_train_first`, `get_recv_shape`, `get_layer_size`, `create_model`, `reduce_hook`).  Only what cannot exist
 here is stood in for (tests/golden/ref_shims.py): CUDA streams/events/devices -> host no-ops, and the DGL graph
 container.  The DGL *partitioner* output is produced by oracle/dglpart.py.  The epoch loop below repeats
-/root/reference/train.py:341-362 line by line so that per-layer tensors can be recorded.
+PipeGCN/train.py:341-362 line by line so that per-layer tensors can be recorded.
 """
 import argparse
 import os
@@ -18,7 +19,7 @@ from pathlib import Path
 
 HERE = Path(__file__).resolve().parent
 ROOT = HERE.parent.parent
-REF = Path("/root/reference")
+REF = Path(os.environ["PIPEGCN_REF"]).resolve()
 
 CONFIGS = {
     "sync_p2": dict(n_parts=2),
@@ -43,8 +44,8 @@ def worker(rank, size, name, cfg, port, q):
     dist.init_process_group("gloo", rank=rank, world_size=size)
 
     import dgl                                         # the shim
-    import train as T                                  # /root/reference/train.py  (star-imports helper.utils, module.model)
-    from helper import context as ctx                  # /root/reference/helper/context.py
+    import train as T                                  # PipeGCN/train.py  (star-imports helper.utils, module.model)
+    from helper import context as ctx                  # PipeGCN/helper/context.py
     assert T.__file__.startswith(str(REF)) and ctx.__file__.startswith(str(REF))
     import torch.nn.functional as F
 
@@ -65,7 +66,7 @@ def worker(rank, size, name, cfg, port, q):
                               feat_corr=cfg.get("feat_corr", False), grad_corr=cfg.get("grad_corr", False),
                               corr_momentum=cfg.get("corr_momentum", 0.95), seed=SEED, lr=1e-2, weight_decay=0)
 
-    # ---- /root/reference/train.py:262-305, the reference's own functions -------------------------------------
+    # ---- PipeGCN/train.py:262-305, the reference's own functions -------------------------------------
     part_g = T.create_inner_graph(graph.clone(), node_dict)
     num_in = node_dict["inner_node"].bool().sum().item()
     graph, part_g, node_dict = T.move_to_cuda(graph, part_g, node_dict)
@@ -110,7 +111,7 @@ def worker(rank, size, name, cfg, port, q):
     for i, layer in enumerate(model.layers):
         layer.register_forward_hook(hook(i))
 
-    # ---- /root/reference/train.py:341-362 ------------------------------------------------------------------------
+    # ---- PipeGCN/train.py:341-362 ------------------------------------------------------------------------
     for epoch in range(N_EPOCHS):
         state = {k: t.clone() for k, t in model.state_dict().items()}
         model.train()

@@ -1,10 +1,12 @@
-"""Dump the flags and defaults of the reference's command line (/root/reference/helper/parser.py) -> ref_parser.json."""
+"""Dump the flags and defaults of the reference's command line (helper/parser.py of the PipeGCN checkout named by
+PIPEGCN_REF) -> ref_parser.json."""
 import importlib.util
 import json
+import os
 import sys
 from pathlib import Path
 
-spec = importlib.util.spec_from_file_location("ref_parser", "/root/reference/helper/parser.py")
+spec = importlib.util.spec_from_file_location("ref_parser", os.path.join(os.environ["PIPEGCN_REF"], "helper", "parser.py"))
 mod = importlib.util.module_from_spec(spec)
 spec.loader.exec_module(mod)
 sys.argv = ["main.py"]

@@ -1,11 +1,11 @@
-"""Shims that let the UNMODIFIED reference modules run in the build container (no GPU, no DGL, no ogb).
+"""Shims that let the UNMODIFIED reference modules run on a host without GPU, DGL or ogb.
 
-Used only by tests/golden/make_golden.py (which needs /root/reference and therefore only runs in the build
-container; its outputs are the committed fixtures).  Two things are stood in for:
+Used only by tests/golden/make_golden.py (which needs a PipeGCN checkout;
+its outputs are the committed fixtures).  Two things are stood in for:
 
 1. CUDA: the reference needs a GPU even on its gloo path (`torch.cuda.Stream()`, `device='cuda'` buffers,
-   `.cuda()`, pinned host memory: /root/reference/helper/feature_buffer.py:72-75,84,98,109-112;
-   /root/reference/helper/reducer.py:19-21; /root/reference/train.py:74-81,300).  Streams and events carry
+   `.cuda()`, pinned host memory: PipeGCN/helper/feature_buffer.py:72-75,84,98,109-112;
+   PipeGCN/helper/reducer.py:19-21; PipeGCN/train.py:74-81,300).  Streams and events carry
    no values, so they become no-ops and every 'cuda' tensor lives on the host: the arithmetic the reference
    performs is unchanged.
 2. DGL (absent, unpinned fork): only the graph CONTAINER the reference's set-up helpers and layer use --
@@ -111,7 +111,7 @@ class FakeGraph:
         self.ndata, self.edata = _Data(), _Data()
         self.nodes = _NodeView(self)
 
-    # container API used by /root/reference/train.py and module/layer.py
+    # container API used by PipeGCN/train.py and module/layer.py
     def edges(self):
         return self.u.clone(), self.v.clone()
 

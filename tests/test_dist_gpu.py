@@ -1,4 +1,4 @@
-"""Real multi-GPU parity where the driver sees it: one process per GPU under torchrun -- CUDA IPC heaps, in-kernel
+"""Real multi-GPU parity: one process per GPU under torchrun -- CUDA IPC heaps, in-kernel
 NVLink stores, NCCL all-reduce, eager and CUDA-graph replay -- against the CPU oracle (tools/dist_parity.py).
 Skipped when fewer than two GPUs are visible; `bench.py --gpus N` runs the same check before timing."""
 import os

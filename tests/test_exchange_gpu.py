@@ -1,7 +1,7 @@
 """GPU parity of the halo exchange alone (no GEMM in the loop): `Buffer.update` and its backward replayed on
 the oracle's own per-epoch inputs must reproduce the oracle's concatenated features and hooked gradients
 BIT FOR BIT in fp32 -- same values, same EMA rounding (two roundings, no FMA), same peer order of the
-boundary add -- in all four modes of /root/reference/helper/feature_buffer.py."""
+boundary add -- in all four modes of PipeGCN/helper/feature_buffer.py."""
 import pytest
 import torch
 

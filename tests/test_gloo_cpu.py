@@ -1,7 +1,7 @@
 """world_size-2 gloo tests on the host: the N>1 logic that does not need a GPU.
 
 * the oracle over a real gloo process group (one process per partition, tagged isend/recv like
-  /root/reference/helper/feature_buffer.py:173,179) equals the oracle over the in-process thread fabric;
+  PipeGCN/helper/feature_buffer.py:173,179) equals the oracle over the in-process thread fabric;
 * `Reducer` (pack -> /n_train -> all-reduce -> unpack) across two processes reproduces the reduced gradients the
   reference's reducer produced (golden fixture);
 * `DistWorld.publish/collect` exchanges the per-rank buffer tables.

@@ -1,5 +1,5 @@
 """The oracle and the layout builder against the golden fixtures, i.e. against outputs of the UNMODIFIED
-reference code (tests/golden/make_golden.py ran /root/reference's Buffer, GraphSAGE, Reducer and set-up helpers
+reference code (tests/golden/make_golden.py ran PipeGCN's Buffer, GraphSAGE, Reducer and set-up helpers
 over gloo on the host).  This is what pins the oracle: fp32, same inputs, same initial weights."""
 from pathlib import Path
 

@@ -1,4 +1,4 @@
-"""Host-side logic of round 2 that needs no GPU: the chunk plan of the aggregate kernels, the on-disk partition cache,
+"""Host-side logic that needs no GPU: the chunk plan of the aggregate kernels, the on-disk partition cache,
 evaluation bookkeeping and result-file naming."""
 import argparse
 

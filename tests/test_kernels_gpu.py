@@ -118,7 +118,7 @@ def test_row_div():
 @pytest.mark.parametrize("m,n,k0,k1", [(1000, 256, 256, 256), (4097, 256, 602, 0), (300, 41, 256, 256),
                                        (128, 16, 20, 20), (77, 128, 100, 100), (5000, 64, 64, 0)])
 def test_linear_tcgen05(dtype, tol, m, n, k0, k1):
-    """pg_linear (tcgen05/TMEM/TMA) vs fp64 matmul of the same (rounded) inputs; bf16: rel 1e-2 (bf16 output
+    """pg_linear (wgmma/TMA) vs fp64 matmul of the same (rounded) inputs; bf16: rel 1e-2 (bf16 output
     rounding), fp32 through the 3xTF32 product: rel 2e-5."""
     from pipegcn_b200 import ops
     from pipegcn_b200.graph import alloc_rows
@@ -195,6 +195,16 @@ def test_layer_norm_relu_matches_torch(dtype, n, d, relu, stage):
     gamma = (torch.rand(d, device=DEV) + 0.5).requires_grad_(True)
     beta = torch.randn(d, device=DEV).requires_grad_(True)
     go = torch.randn(n, d, device=DEV).to(dtype)
+    if relu:
+        # a pre-activation within rounding of zero has no defined ReLU mask (two correct implementations may disagree on
+        # its sign, and the whole row's gradient with it): such rows get the data of a row without one.  Seen on an H100
+        # with (n, d, dtype) = (70001, 256, fp32), torch.manual_seed(256): row 34146 held a pre-activation of 1.03e-8 in
+        # torch's fp32 LayerNorm and -8.3e-9 in fp64; the kernel masked it, torch did not, and all 256 gradients of
+        # that row differed (the device generator's output depends on the GPU, so other GPUs draw other rows)
+        pre = torch.nn.functional.layer_norm(y.detach().float(), (d,), gamma.detach(), beta.detach(), 1e-5)
+        tie = (pre.abs() < 1e-6).any(1)
+        assert int(tie.sum()) <= 1 + n // 1000
+        y[tie] = y[(~tie).nonzero()[0, 0]].clone()
     yq = y.detach().clone().requires_grad_(True)
     assert ops.ln_relu_supported(yq)
     _C.check(_C.lib.pg_set_option(b"ln_stage", stage))
@@ -377,8 +387,8 @@ def test_chunked_kernel_equals_row_kernel(dtype, d):
 @pytest.mark.parametrize("m,n,k", [(5000, 256, 256), (70000, 256, 256), (3000, 64, 256), (2500, 41, 602), (1, 16, 8),
                                    (63, 128, 100), (12345, 200, 1204)])
 def test_wgrad_matches_torch(dtype, m, n, k):
-    """pg_wgrad (MN-major tcgen05, split-K over the rows) == g^T @ x in fp64: bf16 exact products with fp32
-    accumulation (rel. 1e-5 of the output scale), fp32 through the 3xTF32 product (rel. 3e-5)."""
+    """pg_wgrad (MN-major wgmma, split-K over the rows) == g^T @ x in fp64: bf16 exact products with fp32
+    accumulation (rel. 1e-5 of the output scale), fp32 through six products of bf16 terms (rel. 3e-5)."""
     from pipegcn_b200 import ops
     from pipegcn_b200.graph import alloc_rows
     gen = torch.Generator().manual_seed(m + n + k)
@@ -388,15 +398,6 @@ def test_wgrad_matches_torch(dtype, m, n, k):
     x.copy_(torch.randn(m, k, generator=gen).to(dtype))
     out = ops.wgrad(g, x)
     assert out.shape == (n, k) and out.dtype == torch.float32
-    if dtype == torch.float32:          # both fp32 evaluations: MN-major tf32 (3 passes) and bf16 x 3 (6 passes)
-        other = "bf16x3" if ops.WGRAD_FP32 == "3xtf32" else "3xtf32"
-        saved, ops.WGRAD_FP32 = ops.WGRAD_FP32, other
-        try:
-            out2 = ops.wgrad(g, x)
-        finally:
-            ops.WGRAD_FP32 = saved
-        ref2 = g.double().cpu().t() @ x.double().cpu()
-        assert (out2.double().cpu() - ref2).abs().max().item() <= 3e-5 * max(ref2.abs().max().item(), 1.0) + 1e-6, other
     ref = g.double().cpu().t() @ x.double().cpu()
     err = (out.double().cpu() - ref).abs().max().item()
     assert err <= 3e-5 * max(ref.abs().max().item(), 1.0) + 1e-6, (err, ref.abs().max().item())

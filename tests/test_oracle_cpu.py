@@ -107,7 +107,7 @@ def test_ops_refuse_cpu_tensors():
 
 
 def test_command_line_matches_reference_flags():
-    """Same flags, aliases and defaults as /root/reference/helper/parser.py (fixture tests/golden/ref_parser.json),
+    """Same flags, aliases and defaults as PipeGCN/helper/parser.py (fixture tests/golden/ref_parser.json),
     except `--backend` (nccl instead of gloo: the only implemented transport) and the added `--dtype` and `--no-partition-cache`."""
     import json
     from pipegcn_b200.helper.parser import create_parser

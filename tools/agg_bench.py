@@ -7,7 +7,7 @@ at most 16 vectors through the row-per-group kernel instead of the chunked sub-w
 CUDA-event timed, checked against cuSPARSE (fp32 SpMM); one JSON line per variant.
 
     python tools/agg_bench.py [shape=rmat-1m] [P=1] [dtype=bf16] [d=n_feat] [--once] [--variants 1,2h4,...]
-`--once`: a single launch per case after warm-up (what `ncu -k regex:agg` profiles).
+`--once`: a single launch per case after warm-up (for a profiler run).
 """
 import json
 import sys
@@ -16,11 +16,13 @@ from pathlib import Path
 sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
 import torch
 
+from bench import peaks
 from pipegcn_b200 import _C, ops
 from pipegcn_b200.graph import PartGraph, alloc_rows
 from pipegcn_b200.partition import PartitionPlan
 from pipegcn_b200.synthetic import make_graph, random_partition
 
+HBM_PEAK, PEAK_SOURCE = peaks()      # the denominator bench.py uses
 argv = [a for a in sys.argv[1:] if not a.startswith("--")]
 once = "--once" in sys.argv
 variants = ["1", "2n4s", "2h4s", "2n4", "2h4"]
@@ -90,7 +92,8 @@ for var in variants:
     bb = ops.aggregate_bytes(graph.bwd, gy, False)
     es = x.element_size()
     print(json.dumps(dict(info, variant=var, ok=bool(err_f <= tol and err_b <= tol), err_fwd=err_f, err_bwd=err_b,
-                          fwd_ms=tf, bwd_ms=tb, fwd_frac_of_6572=bf / tf / 1e6 / 6572.2, bwd_frac_of_6572=bb / tb / 1e6 / 6572.2,
+                          fwd_ms=tf, bwd_ms=tb, fwd_frac_of_hbm_peak=bf / tf / 1e6 / HBM_PEAK, bwd_frac_of_hbm_peak=bb / tb / 1e6 / HBM_PEAK,
+                          hbm_peak_gbs=HBM_PEAK, hbm_peak_source=PEAK_SOURCE,
                           fwd_gather_tbs=lay.nnz * d * es / tf / 1e9, bwd_gather_tbs=lay.nnz * d * es / tb / 1e9)), flush=True)
 _C.lib.pg_set_option(b"agg_impl", 2)
 _C.lib.pg_set_option(b"agg_l2_hint", 0)

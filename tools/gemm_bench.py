@@ -49,7 +49,7 @@ def main():
             ts = sorted(ev[i].elapsed_time(ev[i + 1]) for i in range(a.iters))
             med = ts[len(ts) // 2]
             nbytes = m * (sum(k_list) + n) * es
-            print(json.dumps(dict(kernel="linear_tcgen05", k=k_list, n=n, rows=m, dtype=a.dtype, gemm_epi_slabs=slabs,
+            print(json.dumps(dict(kernel="linear_wgmma", k=k_list, n=n, rows=m, dtype=a.dtype, gemm_epi_slabs=slabs,
                                   ms=round(med, 4), ms_best=round(ts[0], 4), gbs=round(nbytes / med / 1e6, 1))), flush=True)
     _C.lib.pg_set_option(b"gemm_epi_slabs", 2)
 

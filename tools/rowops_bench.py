@@ -3,7 +3,7 @@
     python tools/rowops_bench.py [--rows 1048576] [--d 256] [--dtype bf16] [--iters 20]
 
 Prints one JSON line per (kernel, ln_stage): milliseconds per launch (CUDA events, L2 flushed between launches by
-the working set itself: every tensor is larger than the 126 MB L2 at the default size) and the HBM GB/s of the
+the working set itself: every tensor is larger than the 50 MB L2 at the default size) and the HBM GB/s of the
 algorithmic bytes (tensors read once + written once).
 """
 import argparse
