@@ -199,6 +199,17 @@ int pg_ce_fwd(const void* z, int64_t ld, const int64_t* labels, int32_t n_rows, 
 int pg_ce_bwd(const void* z, int64_t ld, const int64_t* labels, const float* lse, const float* upstream,
               int32_t n_rows, int32_t n_total, int32_t c, int dtype, void* g, int64_t ldg, float* colsum,
               float* partial, void* stream);
+/*
+ * Accuracy counts of the evaluation (calc_acc, train.py:11-17) on the device.  For every row r < n_rows:
+ * p = argmax of the c logits z[r, 0:c] (fp32 or bf16, compared in fp32; torch.argmax's order: NaN is the maximum,
+ * the first maximal index wins); pred[r] = p when pred != NULL; for every bit k < n_tags set in tag[r] (bit k: row r
+ * belongs to mask k), counts[2k + 1] += 1 and counts[2k] += (p == labels[r]).  counts ([2 * n_tags] int64: correct,
+ * total per mask) is overwritten; labels, tag and counts may be NULL when n_tags == 0 (labels and tag also when
+ * n_rows == 0).  n_tags <= 8; any ld >= c.
+ * Integer atomics: the result is deterministic.
+ */
+int pg_eval_count(const void* logits, int64_t ld, int32_t n_rows, int32_t c, int dtype, const int64_t* labels,
+                  const uint8_t* tag, int32_t n_tags, int32_t* pred, int64_t* counts, void* stream);
 
 /* ------------------------------------------------------------------------------------------
  * Halo exchange (feature_buffer.py:165-194).  One descriptor per message of a launch; the

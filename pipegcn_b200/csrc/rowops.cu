@@ -722,12 +722,101 @@ dropout_kernel(const T* __restrict__ x, int64_t ldx, T* __restrict__ out, int64_
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------
+// Accuracy counts of the evaluation (calc_acc, PipeGCN/train.py:11-17) without moving the logits off the device: a row
+// is held by G = 2^k lanes that read its c logits with strided scalar loads (any ld, any alignment), reduce them to
+// torch.argmax's answer, and add the row to the (correct, total) counters of every mask in its tag.  The argmax order
+// is torch's: NaN beats every number, the lower index wins among equal values (and among NaNs), so the result does
+// not depend on how the lanes split the row.  Counters are integers: per-CTA shared-memory sums, one global atomic
+// per counter and CTA -- deterministic.
+constexpr int kMaxTags = 8;
+
+__device__ __forceinline__ bool argmax_better(float a, int ia, float b, int ib) {
+  const bool na = a != a, nb = b != b;
+  if (na || nb) return na && (!nb || ia < ib);
+  return a > b || (a == b && ia < ib);
+}
+
+template <typename T, int G>
+__global__ void __launch_bounds__(kRowThreads)
+eval_count_kernel(const T* __restrict__ z, int64_t ld, int n_rows, int c, const int64_t* __restrict__ labels,
+                  const uint8_t* __restrict__ tag, int n_tags, int32_t* __restrict__ pred,
+                  unsigned long long* __restrict__ counts) {
+  constexpr int RPW = 32 / G;
+  __shared__ unsigned int sc[2 * kMaxTags];
+  for (int i = threadIdx.x; i < 2 * kMaxTags; i += kRowThreads) sc[i] = 0u;
+  __syncthreads();
+  const int lane = threadIdx.x & 31, lane_g = lane % G, sub = lane / G;
+  const int warp = (blockIdx.x * kRowThreads + threadIdx.x) >> 5;
+  const int warps = (gridDim.x * kRowThreads) >> 5;
+  for (int row0 = warp * RPW; row0 < n_rows; row0 += warps * RPW) {
+    const int row = row0 + sub;
+    const bool valid = row < n_rows;
+    const T* zp = z + static_cast<int64_t>(valid ? row : n_rows - 1) * ld;
+    float best = -INFINITY;
+    int bi = c;                                                 // "no element yet": loses every comparison
+    for (int k = lane_g; k < c; k += G) {
+      const float v = static_cast<float>(zp[k]);
+      if (bi == c || argmax_better(v, k, best, bi)) { best = v; bi = k; }
+    }
+#pragma unroll
+    for (int o = G / 2; o > 0; o >>= 1) {
+      const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+      const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+      if (oi < c && (bi == c || argmax_better(ov, oi, best, bi))) { best = ov; bi = oi; }
+    }
+    if (lane_g == 0 && valid) {
+      if (pred) pred[row] = bi;
+      if (n_tags > 0) {
+        const unsigned int t = tag[row];
+        const unsigned int hit = labels[row] == static_cast<int64_t>(bi) ? 1u : 0u;
+        for (int k = 0; k < n_tags; ++k)
+          if (t & (1u << k)) {
+            if (hit) atomicAdd(&sc[2 * k], 1u);
+            atomicAdd(&sc[2 * k + 1], 1u);
+          }
+      }
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < 2 * n_tags && sc[threadIdx.x]) atomicAdd(counts + threadIdx.x, static_cast<unsigned long long>(sc[threadIdx.x]));
+}
+
 static int row_grid(int n_rows) {
   const int need = (n_rows + (kRowThreads / 32) - 1) / (kRowThreads / 32);
   return need < sm_count() * 8 ? (need > 0 ? need : 1) : sm_count() * 8;
 }
 
 }  // namespace pg
+
+extern "C" int pg_eval_count(const void* logits, int64_t ld, int32_t n_rows, int32_t c, int dtype, const int64_t* labels,
+                             const uint8_t* tag, int32_t n_tags, int32_t* pred, int64_t* counts, void* stream) {
+  using namespace pg;
+  PG_REQUIRE(c > 0 && ld >= c && n_rows >= 0 && (dtype == PG_F32 || dtype == PG_BF16), "pg_eval_count: bad shape or dtype");
+  PG_REQUIRE(n_tags >= 0 && n_tags <= kMaxTags, "pg_eval_count: n_tags=%d must be in [0, %d]", n_tags, kMaxTags);
+  PG_REQUIRE(n_tags == 0 || (counts && ((labels && tag) || n_rows == 0)),
+             "pg_eval_count: labels, tag and counts are needed for n_tags > 0");
+  PG_REQUIRE(n_rows == 0 || logits, "pg_eval_count: null logits");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (n_tags > 0) PG_CHECK_CUDA(cudaMemsetAsync(counts, 0, 2 * sizeof(int64_t) * n_tags, st));
+  if (n_rows == 0 || (n_tags == 0 && pred == nullptr)) return PG_OK;
+  // lanes per row: enough for about four logits each, at most a warp
+  int g = 1;
+  while (g < 32 && g * 4 < c) g <<= 1;
+  const int rpw = 32 / g;
+  const int64_t need = (static_cast<int64_t>(n_rows) + rpw * (kRowThreads / 32) - 1) / (rpw * (kRowThreads / 32));
+  const int grid = static_cast<int>(need < sm_count() * 8 ? need : sm_count() * 8);
+  unsigned long long* cnt = reinterpret_cast<unsigned long long*>(counts);
+#define PG_EVC(T_, G_) eval_count_kernel<T_, G_><<<grid, kRowThreads, 0, st>>>(static_cast<const T_*>(logits), ld, n_rows, c, labels, tag, n_tags, pred, cnt)
+#define PG_EVC_T(T_) do { \
+    if (g == 1) PG_EVC(T_, 1); else if (g == 2) PG_EVC(T_, 2); else if (g == 4) PG_EVC(T_, 4); \
+    else if (g == 8) PG_EVC(T_, 8); else if (g == 16) PG_EVC(T_, 16); else PG_EVC(T_, 32); } while (0)
+  if (dtype == PG_F32) PG_EVC_T(float); else PG_EVC_T(__nv_bfloat16);
+#undef PG_EVC_T
+#undef PG_EVC
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
 
 extern "C" int pg_row_grid(int32_t n_rows) { return pg::row_grid(n_rows); }
 

@@ -156,11 +156,14 @@ def build_rank_layout(spec: dict, rank: int, n_parts: int, device, world=None, s
         return out
 
     inner_gid = permute_rows(inner_orig)
+    train_in = permute_rows(tm)
     layout = PartitionLayout(
         rank=r, size=P, num_in=n_in, num_all=num_all, indptr=indptr, indices=indices, t_indptr=t_indptr,
         t_indices=t_indices, in_deg=in_deg, boundary=boundary, recv_shape=recv_shape, feat=permute_rows(feat_o),
-        label=permute_rows(label_o), train_mask=permute_rows(tm), inner_gid=inner_gid,
-        halo_gid=halo_gid, n_train_global=n_train_global)
+        label=permute_rows(label_o), train_mask=train_in, inner_gid=inner_gid,
+        halo_gid=halo_gid, n_train_global=n_train_global,
+        # GlobalGraph.val_mask / test_mask: the non-training nodes split by id parity
+        val_mask=~train_in & (inner_gid % 2 == 0), test_mask=~train_in & (inner_gid % 2 == 1))
     nnz = torch.tensor([float(layout.nnz)], dtype=torch.float64, device=dev)
     if world is not None and getattr(world, "size", 1) > 1 and not getattr(world, "is_local", False):
         world.all_reduce_sum_(nnz)

@@ -7,6 +7,7 @@ and the adjacency survive.
 """
 from __future__ import annotations
 
+import copy
 import ctypes as C
 import os
 from typing import Optional
@@ -147,6 +148,17 @@ class PartGraph:
     def from_layout(cls, lay, device="cuda", seg_len=None) -> "PartGraph":
         return cls(lay.num_in, lay.num_all, lay.indptr, lay.indices, lay.t_indptr, lay.t_indices, lay.in_deg,
                    device=device, seg_len=seg_len)
+
+    def scratch_view(self) -> "PartGraph":
+        """The same graph (shared index arrays) with scratch space of its own.  A user that runs between replays of
+        CUDA graphs captured on this graph (the partitioned evaluation, whose eval branch aggregates wider rows than
+        the training step) must not grow the scratch those graphs hold: growing frees the captured address."""
+        view = copy.copy(self)
+        for name in ("fwd", "bwd"):
+            plan = copy.copy(getattr(self, name))
+            plan._scratch = None
+            setattr(view, name, plan)
+        return view
 
     def deg_as_float(self, in_deg) -> torch.Tensor:
         """fp32 view of the `in_deg` argument of GraphSAGELayer.forward (cached for the graph's own tensor)."""

@@ -574,3 +574,183 @@ class Buffer(object):
         """Join the side stream (end of training / before reading buffers on the host)."""
         if self._comm_stream is not None:
             torch.cuda.current_stream().wait_stream(self._comm_stream)
+
+
+class EvalExchange:
+    """Forward-only, synchronous halo exchange of the partitioned evaluation, on a symmetric heap of its own.
+
+    Evaluation never writes the training `Buffer`: with --enable-pipeline the version the next epoch reads already
+    holds halo rows the peers have pushed, and overwriting them would silently change training.  Rows are exact: the
+    current eval-mode activations, no EMA, no dropout, no staleness.
+
+    Heap: flags [2][P] (uint32, word [b][j] = the last value peer j published into buffer b), then two row buffers
+    [num_all, ld] with ld = the padded widest graph-layer input.  Graph layer l reads buffer l % 2; the norm / ReLU
+    epilogue of layer l writes the inner rows of buffer (l + 1) % 2; a push sends this rank's boundary rows of buffer
+    l % 2 into the peers' halo rows of their buffer l % 2 and publishes seq * L + l + 1 (`seq` counts the eval calls).
+
+    Two buffers are enough.  Peer j pushes its layer l + 2 rows into my buffer l % 2 only after its wait on my layer
+    l + 1 flag, and my layer l + 1 push is stream-ordered after my layer-l aggregate, the last read of those halo rows.
+    My own inner rows of buffer l % 2 are rewritten by my layer l + 1 epilogue, stream-ordered after my layer-l push
+    (their only remote consumer: pushes write the peer's memory, nobody reads mine).  Across eval calls something
+    collective has to separate the last read of a call from the first push of the next, which waits on nothing:
+    `RankEngine.evaluate` sums its accuracy counts with an all-reduce, `RankEngine.predict` ends with a one-element
+    all-reduce, and `LocalTrainer` joins every rank's stream into the current stream at the end of a call and starts
+    the next call's streams after it.
+    """
+
+    def __init__(self, world, num_in, num_all, boundary, recv_shape, widths, n_layers, dtype,
+                 key='pipegcn.eval', timeout_ms=20000):
+        w = world
+        rank, size, dev = w.rank, w.size, w.device
+        self._world, self._key = w, key
+        self._num_in, self._num_all = int(num_in), int(num_all)
+        self._L = max(int(n_layers), 1)
+        self._dtype = dtype
+        self._es = torch.empty(0, dtype=dtype).element_size()
+        self._ld = _round_up(max(list(widths) + [1]), 8)
+        self._peers = [j for j in range(size) if j != rank]
+        self._pl = [None] * size
+        tot = self._num_in
+        for j in self._peers:
+            self._pl[j] = tot
+            tot += int(recv_shape[j])
+        assert tot == self._num_all, f"recv shapes {recv_shape} do not add up to num_all={num_all}"
+        self._bidx = {j: boundary[j].to(device=dev, dtype=torch.int32).contiguous() for j in self._peers}
+        # heap = flags + 2 * num_all * ld * s: independent of the number of layers
+        self.flag_bytes = _round_up(4 * 2 * size, _ALIGN)
+        buf_bytes = self._num_all * self._ld * self._es
+        self._buf_off = [self.flag_bytes, self.flag_bytes + buf_bytes]
+        self.heap_bytes = self.flag_bytes + 2 * buf_bytes
+        self._heap = Heap(self.heap_bytes, dev)
+        self._flags = self._heap.view(0, (2, size), torch.int32)
+        self._buf = [self._heap.view(o, (self._num_all, self._ld), dtype) for o in self._buf_off]
+        self._counters = torch.zeros(2 * size, dtype=torch.int32, device=dev)
+        self._status = torch.zeros(1, dtype=torch.int32, device=dev)
+        self.timeout_ms = int(timeout_ms)
+        self.seq = 0
+        self._connected = False
+        w.publish(key, {'heap': w.heap_token(self._heap), 'buf_off': list(self._buf_off), 'pl': list(self._pl),
+                        'ld': self._ld, 'es': self._es})
+
+    def _connect(self):
+        w = self._world
+        rank, size, dev = w.rank, w.size, w.device
+        tables = w.collect(self._key)
+        self._tables = tables                   # the peers' heaps this rank maps: what `release` unmaps
+        ld, es = self._ld, self._es
+        self._msgs, self._wait = [None, None], [None, None]
+        for b in (0, 1):
+            msgs = []
+            for j in self._peers:
+                t = tables[j]
+                if t['ld'] != ld or t['es'] != es:
+                    raise RuntimeError(f"rank {j} set up its eval exchange with another width / dtype")
+                base = w.map_peer(t['heap'])
+                dst = base + t['buf_off'][b] + t['pl'][rank] * ld * es
+                flag = base + 4 * (b * size + rank)
+                counter = self._counters.data_ptr() + 4 * (b * size + j)
+                msgs.append(_C.pg_msg(self._bidx[j].data_ptr(), 0, int(self._bidx[j].numel()), 0, dst, ld, None, 0,
+                                      flag, counter, int(t['pl'][rank])))
+            self._msgs[b] = _MsgSet(msgs, dev) if msgs else None
+            ptrs = [self._heap.ptr + 4 * (b * size + j) for j in self._peers]
+            self._wait[b] = torch.tensor(ptrs, dtype=torch.int64, device=dev) if ptrs else None
+        self._connected = True
+
+    def begin(self):
+        """Start an eval call (every rank, in the same order)."""
+        if not self._connected:
+            self._connect()
+        self.seq += 1
+
+    def rows(self, layer, d):
+        """[num_all, d]: the input of graph layer `layer`, inner rows then halo rows."""
+        return self._buf[layer % 2][:, :d]
+
+    def inner(self, layer, d):
+        return self._buf[layer % 2][:self._num_in, :d]
+
+    def halo(self, layer, d):
+        return self._buf[layer % 2][self._num_in:, :d]
+
+    def _value(self, layer):
+        return (self.seq * self._L + layer + 1) & 0xffffffff
+
+    def push(self, layer, d):
+        """Send this rank's boundary rows of layer `layer`'s input to every peer and publish the flag (zero-row
+        messages too: every peer waits for every other)."""
+        ms = self._msgs[layer % 2]
+        if ms is None:
+            return
+        src = self.inner(layer, d)
+        _C.count()
+        _C.check(_C.lib.pg_halo_push(ms.ptr, ms.n_msgs, ms.n_ctas, src.data_ptr(), src.stride(0), d,
+                                     _C.dtype_code(self._dtype), 0.0, 1.0, self._value(layer), None,
+                                     _C.stream_ptr()), "pg_halo_push")
+
+    def wait(self, layer):
+        """Block the stream until every peer's layer-`layer` rows have arrived (bounded: a timeout is reported by
+        `check_status`, it does not hang)."""
+        ptrs = self._wait[layer % 2]
+        if ptrs is None:
+            return
+        _C.count()
+        _C.check(_C.lib.pg_halo_wait(ptrs.data_ptr(), ptrs.numel(), self._value(layer), None, self.timeout_ms,
+                                     self._status.data_ptr(), None, _C.stream_ptr()), "pg_halo_wait")
+
+    def check_status(self):
+        """Raises if a flag wait timed out since the last check (host sync)."""
+        if int(self._status.item()) != 0:
+            self._status.zero_()
+            raise _C.PgError(f"eval halo exchange: a peer's flag did not arrive within {self.timeout_ms} ms "
+                             f"(PG_ERR_TIMEOUT); rank {self._world.rank} eval call {self.seq} received flags "
+                             f"[buffer][source rank] = {self._flags.tolist()}")
+
+    def release(self):
+        """Give the heap back (collective over the world, like `Buffer.release`)."""
+        w = self._world
+        if self._connected:
+            for j, t in enumerate(self._tables):
+                if j != w.rank:
+                    w.unmap_peer(t['heap'])
+        w.barrier()
+        self._heap.free()
+        self._buf = None
+        self._connected = False
+
+
+class OneShotExchange:
+    """One exchange of the halo rows of a static [N_in, d] tensor (the raw input features) through a non-pipelined
+    `Buffer`: the first half of --use-pp's precompute (PipeGCN/train.py:169-189) and the layer-0 halo rows of an
+    evaluation layout.  `push`, then `wait` (with several LocalWorld ranks in one process every rank pushes before any
+    rank waits), then `release` once every rank has waited (collective for a DistWorld)."""
+
+    def __init__(self, world, lay, d, dtype, backend, key, timeout_ms=None):
+        from .timer.comm_timer import CommTimer
+        self._d = int(d)
+        self._buf = Buffer(world)
+        self._buf.timer = CommTimer()
+        if timeout_ms is not None:
+            self._buf.timeout_ms = int(timeout_ms)
+        self._buf.init_buffer(lay.num_in, lay.num_all, lay.boundary, lay.recv_shape, [self._d], backend=backend,
+                              pipeline=False, dtype=dtype, world=world, key=key)
+        self.pushed = False
+
+    def push(self, feat):
+        """Copy `feat` into the inner rows and send its boundary rows to every peer."""
+        b = self._buf
+        b._connect()
+        feat = feat if feat.stride(1) == 1 else feat.contiguous()
+        b._push(b._self_msgs[(0, 0)], feat, self._d, 0)
+        b._push(b._fwd_msgs[(0, 0)], feat, self._d, 1)
+        self.pushed = True
+
+    def wait(self) -> torch.Tensor:
+        """Block the stream until the peers' rows have arrived; [num_all, d]: inner rows, then halo rows."""
+        self._buf._wait_flags(0, 0, 1, 'forward_0')
+        return self._buf._f_buf[(0, 0)][:, :self._d]
+
+    def check_status(self):
+        self._buf.check_status()
+
+    def release(self):
+        self._buf.release()

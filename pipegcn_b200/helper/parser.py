@@ -5,6 +5,12 @@ defaults to `nccl` (the reference implements gloo only; this engine implements t
 NVLink/NCCL path only), `--dataset` also accepts `synthetic:<shape>` (shapes in
 pipegcn_b200/synthetic.py), `--model` accepts `gcn` as an alias of `graphsage`, and
 `--dtype {fp32,bf16}` selects the activation storage type.
+
+`--eval-partitioned` (off by default; not in the reference) makes `--eval` partition-parallel: every rank evaluates
+its own inner rows over an exact halo exchange and the accuracy counts are summed across ranks, instead of rank 0
+evaluating the whole graph, which it would have to hold a second time.  The printed lines, the result file and the
+checkpoint keep their formats.  When the flag is absent the namespace has no `eval_partitioned` attribute (read it
+with getattr(args, 'eval_partitioned', False)), so the parsed flags stay the reference's.
 """
 import argparse
 
@@ -59,6 +65,9 @@ def build_parser():
     parser.add_argument('--no-partition-cache', action='store_false', dest='partition_cache',
                         help="do not read/write partitions/<graph_name>/part.pt")
     parser.set_defaults(partition_cache=True)
+    parser.add_argument('--eval-partitioned', '--eval_partitioned', action='store_true', default=argparse.SUPPRESS,
+                        help="with --eval: every rank evaluates its own nodes (exact halo exchange) instead of rank 0 "
+                             "evaluating the whole graph")
     return parser
 
 

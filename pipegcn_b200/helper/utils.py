@@ -21,8 +21,8 @@ import warnings
 
 import torch
 
-from ..partition import PartitionPlan, get_layer_size  # noqa: F401  (re-export)
-from ..synthetic import SHAPES, make_graph, random_partition, train_subgraph
+from ..partition import PartitionPlan, build_eval_layout, extend_partition, get_layer_size  # noqa: F401  (re-export)
+from ..synthetic import SHAPES, GlobalGraph, make_graph, random_partition, train_subgraph
 
 _ALIAS = {'reddit': 'reddit-shaped', 'ogbn-products': 'products-shaped'}
 
@@ -96,9 +96,35 @@ def graph_partition(g, args, rank=0):
     return blob['part'].to(torch.int64).to(g.src.device)
 
 
-def load_partition(args, rank, device=None, return_graph=False):
+class InductiveEvalLayouts:
+    """This rank's layouts of the two --inductive evaluation graphs of the reference (`evaluate_induc`): validation on
+    the subgraph of the training and validation nodes, test on the whole graph.  Both are partitioned by
+    `extend_partition` of the training assignment.  The global graph waits on the host; each layout is built on
+    `device` when it is asked for (the test layout at the end of training, after the validation one is freed)."""
+
+    def __init__(self, g_full, train_part, n_parts: int, rank: int, device):
+        self.device, self.P, self.rank = torch.device(device), int(n_parts), int(rank)
+        self.part = extend_partition(g_full.train_mask, train_part, self.P).cpu()
+        self.g = GlobalGraph(g_full.n_nodes, g_full.src.cpu(), g_full.dst.cpu(), g_full.feat.cpu(), g_full.label.cpu(),
+                             g_full.train_mask.cpu())
+
+    def _build(self, keep_val: bool):
+        g = GlobalGraph(self.g.n_nodes, self.g.src.to(self.device), self.g.dst.to(self.device), self.g.feat.to(self.device),
+                        self.g.label.to(self.device), self.g.train_mask.to(self.device))
+        keep = (g.train_mask | g.val_mask) if keep_val else None
+        return build_eval_layout(g, keep, self.part.to(self.device), self.P, self.rank)
+
+    def val_layout(self):
+        return self._build(True)
+
+    def test_layout(self):
+        return self._build(False)
+
+
+def load_partition(args, rank, device=None, return_graph=False, return_eval_layouts=False):
     """This rank's `PartitionLayout` (utils.py:99-129 + the set-up half of train.run).  With `return_graph` the
-    (transductive) global graph is returned too -- rank 0 evaluates on it (train.py:250-256)."""
+    (transductive) global graph is returned too -- rank 0 evaluates on it (train.py:250-256).  With
+    `return_eval_layouts` (--inductive --eval-partitioned) an `InductiveEvalLayouts` is returned too."""
     device = device if device is not None else (f'cuda:{torch.cuda.current_device()}' if torch.cuda.is_available() else 'cpu')
     g_full, n_feat, n_class = load_data(args.dataset, device=device)
     args.n_feat, args.n_class = n_feat, n_class
@@ -106,4 +132,8 @@ def load_partition(args, rank, device=None, return_graph=False):
     args.n_train = int(g.train_mask.sum().item())
     part = graph_partition(g, args, rank)
     layout = PartitionPlan(g, part, args.n_partitions).build(rank)
+    if return_eval_layouts:
+        if not getattr(args, 'inductive', False):
+            raise ValueError("return_eval_layouts: the transductive evaluation uses the training layout")
+        return layout, InductiveEvalLayouts(g_full, part, args.n_partitions, rank, device)
     return (layout, g_full) if return_graph else layout

@@ -51,7 +51,9 @@ class GraphSAGELayer(nn.Module):
                                   self.linear2.weight, self.linear2.bias, drop_bwd)
         assert in_deg is None
         ah = ops.sage_aggregate(feat, graph, graph.row_degrees())
+        # a partition's graph (partitioned evaluation): feat holds [inner | halo] rows, the outputs are the inner rows
+        x = feat[:graph.num_in] if feat.shape[0] != graph.num_in else feat
         if self.use_pp:
-            return ops.linear(torch.cat((feat, ah), dim=1), self.linear.weight, self.linear.bias)
-        return ops.sage_linear(feat, ah, self.linear1.weight, self.linear1.bias,
+            return ops.linear(torch.cat((x, ah), dim=1), self.linear.weight, self.linear.bias)
+        return ops.sage_linear(x, ah, self.linear1.weight, self.linear1.bias,
                                self.linear2.weight, self.linear2.bias)

@@ -118,5 +118,36 @@ class GraphSAGE(GNNBase):
                 h = self._norm_act(i, h, dest, fuse_drop=ops.FUSED_DROPOUT and p > 0 and dest is not None)
         return h
 
+    def forward_partitioned(self, g, xch, pp_feat=None, push0=False):
+        """Eval-mode forward of the inner rows of one partition (partitioned evaluation), as a generator that yields
+        after every halo push: with several ranks driven by one host thread every rank pushes before any rank waits.
+        `xch` is an `EvalExchange` whose buffer 0 holds the layer-0 input: the inner rows, and the halo rows too
+        unless `push0` (then they are exchanged like every later layer's); every norm / ReLU epilogue writes the next
+        graph layer's inner rows straight into the exchange buffer.  `pp_feat`: the --use-pp layer-0 input
+        cat(feat, neighbour mean) of the inner rows.  Returns the logits [N_in, C]."""
+        from .. import ops
+        assert not self.training
+        h = None
+        for i, layer in enumerate(self.layers):
+            if i < self.n_graph_layers:
+                if i == 0 and self.use_pp:
+                    h = ops.linear(pp_feat, layer.linear.weight, layer.linear.bias)
+                else:
+                    d = layer.in_feats
+                    if i > 0 or push0:
+                        xch.push(i, d)
+                        yield i
+                        xch.wait(i)
+                    h = layer(g, xch.rows(i, d), None)
+            else:
+                h = ops.linear(h, layer.weight, layer.bias)
+            if i < self.n_layers - 1:
+                dest = xch.inner(i + 1, h.shape[1]) if i + 1 < self.n_graph_layers else None
+                out = self._norm_act(i, h, dest)
+                if dest is not None and out.data_ptr() != dest.data_ptr():
+                    dest.copy_(out)
+                h = out
+        return h
+
 
 GCN = GraphSAGE

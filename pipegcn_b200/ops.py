@@ -638,6 +638,30 @@ def cross_entropy_sum(logits, labels, n_train):
     return CrossEntropySum.apply(logits, labels, int(n_train))
 
 
+def eval_count(logits: torch.Tensor, labels: torch.Tensor = None, tag: torch.Tensor = None, n_tags: int = 0,
+               want_pred: bool = False):
+    """(counts, pred): counts [n_tags, 2] int64 = (correct, total) of every mask k (rows whose `tag` has bit k), with
+    torch.argmax(logits, 1) as the prediction; pred [N] int32 (or None).  One kernel, the logits stay on the device."""
+    if n_tags and labels.dim() != 1:
+        # as calc_acc: the multi-label (yelp) F1 evaluation is not implemented
+        raise NotImplementedError("multi-label (yelp) evaluation is out of scope")
+    if logits.dim() != 2 or (logits.shape[1] > 1 and logits.stride(1) != 1) or not logits.is_cuda:
+        raise _C.PgError(f"eval_count: expected row-major CUDA logits, got {tuple(logits.shape)} {logits.stride()}")
+    n, c = logits.shape
+    dev = logits.device
+    counts = torch.empty(max(n_tags, 1), 2, dtype=torch.int64, device=dev)
+    pred = torch.empty(n, dtype=torch.int32, device=dev) if want_pred else None
+    if n_tags:
+        labels, tag = labels.contiguous(), tag.contiguous()
+        assert labels.dtype == torch.int64 and tag.dtype == torch.uint8 and labels.numel() == n and tag.numel() == n
+    _C.count()
+    _C.check(_C.lib.pg_eval_count(logits.data_ptr(), logits.stride(0), n, c, _C.dtype_code(logits.dtype),
+                                  labels.data_ptr() if n_tags else None, tag.data_ptr() if n_tags else None,
+                                  int(n_tags), pred.data_ptr() if pred is not None else None,
+                                  counts.data_ptr() if n_tags else None, _C.stream_ptr()), "pg_eval_count")
+    return counts[:n_tags], pred
+
+
 class Dropout(torch.autograd.Function):
     """Dropout whose mask is regenerated from (seed, element index) in the backward (csrc/rowops.cu)."""
 

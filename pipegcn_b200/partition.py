@@ -50,6 +50,10 @@ class PartitionLayout:
     halo_gid: torch.Tensor           # [H] original global id of every halo row
     n_train_global: int = 0
     extra: dict = field(default_factory=dict)
+    # [N_in] bool, same row order as `label`: the evaluation masks of the inner rows (GlobalGraph.val_mask /
+    # test_mask through inner_gid); None when the builder did not provide them
+    val_mask: Optional[torch.Tensor] = None
+    test_mask: Optional[torch.Tensor] = None
 
     @property
     def nnz(self) -> int:
@@ -169,13 +173,39 @@ class PartitionPlan:
             indptr=indptr, indices=indices, t_indptr=t_indptr, t_indices=t_indices,
             in_deg=self.in_deg[inner_gid], boundary=boundary, recv_shape=recv_shape,
             feat=g.feat[inner_gid], label=g.label[inner_gid], train_mask=g.train_mask[inner_gid],
-            inner_gid=inner_gid, halo_gid=halo_gid, n_train_global=self.n_train_global)
+            inner_gid=inner_gid, halo_gid=halo_gid, n_train_global=self.n_train_global,
+            val_mask=g.val_mask[inner_gid], test_mask=g.test_mask[inner_gid])
 
 
 def build_layouts(g: GlobalGraph, part: torch.Tensor, n_parts: int, ranks=None) -> List[PartitionLayout]:
     plan = PartitionPlan(g, part, n_parts)
     ranks = range(n_parts) if ranks is None else ranks
     return [plan.build(r) for r in ranks]
+
+
+def extend_partition(train_mask: torch.Tensor, train_part: torch.Tensor, n_parts: int, seed: int = 2) -> torch.Tensor:
+    """Node -> partition of the whole graph for the --inductive evaluation graphs: the training nodes keep the part
+    of the training partition (`train_part`, in ascending id order of the training nodes), every other node gets a
+    seeded uniform draw -- the same on every rank."""
+    from .synthetic import random_partition
+    part = random_partition(int(train_mask.numel()), n_parts, seed=seed, device=train_mask.device)
+    part[train_mask] = train_part.to(part.device).to(part.dtype)
+    return part
+
+
+def build_eval_layout(g: GlobalGraph, keep: Optional[torch.Tensor], part: torch.Tensor, n_parts: int,
+                      rank: int) -> PartitionLayout:
+    """Rank `rank`'s layout of the subgraph of `g` induced by `keep` (None: all of g) under the node -> partition map
+    `part` of g.  Ids (inner_gid, halo_gid) are those of the subgraph; val_mask / test_mask follow g's rule."""
+    from .synthetic import induced_subgraph
+    if keep is None:
+        sub, ids = g, None
+    else:
+        sub, ids = induced_subgraph(g, keep)
+    lay = PartitionPlan(sub, part if ids is None else part[ids], n_parts).build(rank)
+    gid = lay.inner_gid if ids is None else ids[lay.inner_gid]
+    lay.val_mask, lay.test_mask = g.val_mask[gid], g.test_mask[gid]
+    return lay
 
 
 def get_layer_size(n_feat: int, n_hidden: int, n_class: int, n_layers: int) -> List[int]:

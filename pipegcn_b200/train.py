@@ -10,11 +10,17 @@ checkpointing (train.py:20-61,377-400) run on the GPU with the same kernels (pip
 
 `RankEngine` is one rank; `LocalTrainer` steps several simulated ranks of a
 `LocalWorld` in lock-step on one GPU (each on its own stream).
+
+With `--eval --eval-partitioned` evaluation is collective: every rank evaluates its own inner rows
+(`RankEngine.predict` / `evaluate`, `LocalTrainer.predict` / `evaluate`) over an exact halo exchange of its own heap
+(`helper.feature_buffer.EvalExchange`), and no rank needs the global graph.
 """
 from __future__ import annotations
 
+import contextlib
 import os
 import time
+from types import SimpleNamespace
 from typing import List, Optional
 
 import numpy as np
@@ -23,7 +29,7 @@ import torch.nn.functional as F
 
 from .graph import PartGraph
 from .helper import context as ctx
-from .helper.feature_buffer import Buffer
+from .helper.feature_buffer import Buffer, OneShotExchange
 from .helper.reducer import Reducer
 from .helper.timer.comm_timer import CommTimer
 from .module.model import GraphSAGE
@@ -35,6 +41,34 @@ def create_model(layer_size, args, buffer=None, dtype=torch.float32):
         return GraphSAGE(layer_size, F.relu, args.use_pp, norm=args.norm, dropout=args.dropout,
                          n_linear=args.n_linear, train_size=args.n_train, buffer=buffer, dtype=dtype)
     raise NotImplementedError(args.model)
+
+
+def pp_input(graph, feat, rows):
+    """--use-pp layer-0 input of the inner rows: cat(feat, neighbour mean) (second half of `precompute`,
+    PipeGCN/train.py:169-189); `rows` [num_all, d] holds the raw features of the inner and the halo rows."""
+    from . import ops
+    from .graph import alloc_rows
+    d = feat.shape[1]
+    mean = ops.aggregate(graph.fwd, rows, row_div=graph.in_deg_f)
+    both = alloc_rows(graph.num_in, 2 * d, feat.dtype, feat.device)
+    both[:, :d].copy_(feat)
+    both[:, d:].copy_(mean)
+    return both
+
+
+@contextlib.contextmanager
+def _eval_mode(models):
+    """Every model in eval mode for the duration, each restored to its own mode afterwards (set once around the
+    whole, possibly lock-stepped, forward: the ranks of a LocalWorld may share one model)."""
+    uniq = list({id(m): m for m in models}.values())
+    modes = [m.training for m in uniq]
+    for m in uniq:
+        m.eval()
+    try:
+        yield
+    finally:
+        for m, was in zip(uniq, modes):
+            m.train(was)
 
 
 def reduce_hook(reducer, param, name, n_train):
@@ -104,45 +138,30 @@ class RankEngine:
         self.epoch = 0
         self.last_logits = None
         self.keep_logits = False
+        # what the partitioned evaluation of the training layout needs (index spaces, labels and masks of the inner
+        # rows); its exchange heap is allocated at the first evaluation
+        self._own_eval = SimpleNamespace(num_in=layout.num_in, num_all=layout.num_all, boundary=layout.boundary,
+                                         recv_shape=layout.recv_shape, label=layout.label,
+                                         val_mask=layout.val_mask, test_mask=layout.test_mask, feat=None)
+        self._evals = {}
 
     # ------------------------------------------------------------------ --use-pp (train.py:169-189)
     def pp_begin(self, layout):
         """One-shot exchange of the raw boundary features through the push kernel (first half of `precompute`)."""
-        from .graph import alloc_rows
-        pp = Buffer(self.world)
-        pp.timer = CommTimer()
-        pp.init_buffer(layout.num_in, layout.num_all, layout.boundary, layout.recv_shape, [self.args.n_feat],
-                       backend=self.args.backend, pipeline=False, dtype=self.dtype, world=self.world,
-                       key='pipegcn.buffer.pp')
-        self._pp = pp
-        self._pp_started = False
+        self._pp = OneShotExchange(self.world, layout, self.args.n_feat, self.dtype, self.args.backend,
+                                   key='pipegcn.buffer.pp')
 
     def _pp_push(self):
-        pp = self._pp
-        pp._connect()
-        d = self.args.n_feat
-        feat = self.feat if self.feat.stride(1) == 1 else self.feat.contiguous()
-        pp._push(pp._self_msgs[(0, 0)], feat, d, 0)
-        pp._push(pp._fwd_msgs[(0, 0)], feat, d, 1)
-        self._pp_started = True
+        self._pp.push(self.feat)
 
     def pp_end(self):
         """Wait for the peers' rows, neighbour mean, feat <- cat(feat, mean) (second half of `precompute`).  With
         several LocalWorld ranks in one process every rank must have pushed before any rank waits
         (`LocalTrainer` calls `_pp_push` on all engines first)."""
-        from . import ops
-        from .graph import alloc_rows
         pp = self._pp
-        if not self._pp_started:
+        if not pp.pushed:
             self._pp_push()
-        pp._wait_flags(0, 0, 1, 'forward_0')
-        d = self.args.n_feat
-        merged = pp._f_buf[(0, 0)][:, :d]
-        mean = ops.aggregate(self.graph.fwd, merged, row_div=self.graph.in_deg_f)
-        both = alloc_rows(self.graph.num_in, 2 * d, self.dtype, self.device)
-        both[:, :d].copy_(self.feat)
-        both[:, d:].copy_(mean)
-        self.feat = both
+        self.feat = pp_input(self.graph, self.feat, pp.wait())
         torch.cuda.synchronize()
         pp.check_status()
         self._pp_done = pp                 # peers may still be reading its heap: freed by `release_pp`
@@ -282,6 +301,187 @@ class RankEngine:
             p.grad = gr
         return loss
 
+    # ------------------------------------------------------------------ partitioned evaluation (--eval-partitioned)
+    # Every rank evaluates its own inner rows over an exact, synchronous halo exchange of the eval-mode activations
+    # (`EvalExchange`, a heap of its own).  The collective steps are generators that yield after every halo push: a
+    # DistWorld rank runs them to the end (`_drain`), `LocalTrainer` steps all ranks of a LocalWorld in lock-step so
+    # that every rank has pushed before any rank waits.  Callers run them under torch.no_grad().
+    def _eval_open_steps(self, eval_layout=None):
+        """Set up the partitioned evaluation of `eval_layout` (None: the training layout, transductive).  Collective."""
+        from .helper.feature_buffer import EvalExchange
+        args, dev = self.args, self.device
+        own = eval_layout is None
+        lay = self._own_eval if own else eval_layout
+        if lay.val_mask is None or lay.test_mask is None:
+            raise ValueError("partitioned evaluation needs the layout's val_mask / test_mask")
+        n_graph = args.n_layers - args.n_linear
+        widths = self.layer_size[(1 if args.use_pp else 0):n_graph]
+        tag = lay.val_mask.to(dev).to(torch.uint8) | (lay.test_mask.to(dev).to(torch.uint8) << 1)
+        st = SimpleNamespace(label=lay.label.to(dev), tag=tag, pp_feat=None, x0=None, feat=None, push0=False,
+                             n_rows=lay.num_in, layout=eval_layout)
+        if own:
+            st.graph = self.graph.scratch_view()           # captured training epochs keep their scratch address
+            # the eval branch divides by the row lengths of the CSR: a partition holds every in-edge of its inner rows,
+            # so these are the global in-degrees the training path divides by
+            if not torch.equal(self.graph.row_degrees(), self.graph.in_deg_f):
+                raise RuntimeError("partition layout: the CSR row lengths differ from the global in-degrees")
+            key = 'pipegcn.eval'
+        else:
+            st.graph = PartGraph.from_layout(eval_layout, device=dev)
+            # one key per evaluation layout (every rank opens them in the same order): several may be alive at once
+            self._n_eval_layouts = getattr(self, '_n_eval_layouts', 0) + 1
+            key = 'pipegcn.eval.layout%d' % self._n_eval_layouts
+        st.xch = EvalExchange(self.world, lay.num_in, lay.num_all, lay.boundary, lay.recv_shape, widths, n_graph,
+                              self.dtype, key=key, timeout_ms=self.buffer.timeout_ms)
+        self.last_eval_exchange = st.xch
+        yield 'publish'
+        if own:
+            if args.use_pp:
+                st.pp_feat = self.feat                     # cat(feat, neighbour mean), computed at set-up
+            elif self.buffer._static0_ready and self.buffer._x0 is not None:
+                # the raw halo rows of the static layer-0 shortcut (not the c_t-scaled copy update(0, .) returns);
+                # a view: `set_features` refreshes them
+                st.x0 = self.buffer._x0[:lay.num_all - lay.num_in, :args.n_feat]
+            else:
+                # no kept copy of the raw halo rows: every evaluation exchanges the current features' halo rows
+                st.push0 = self.world.size > 1
+            return st
+        # an evaluation layout: its features are those of the graph it was built from, static for the run
+        feat = eval_layout.feat.to(dev).to(self.dtype)
+        if self.world.size == 1:
+            rows = feat
+        else:
+            one = OneShotExchange(self.world, lay, args.n_feat, self.dtype, args.backend, key=key + '.raw',
+                                  timeout_ms=self.buffer.timeout_ms)
+            yield 'publish'
+            one.push(feat)
+            yield 'push'
+            rows = one.wait()
+        if args.use_pp:
+            st.pp_feat = pp_input(st.graph, feat, rows)    # recomputed over this layout's graph
+        else:
+            st.feat = feat
+            st.x0 = rows[lay.num_in:].clone()
+        if self.world.size > 1:
+            yield 'copied'                                 # every rank has its rows: the one-shot heap may go
+            torch.cuda.synchronize()
+            one.check_status()
+            one.release()
+        return st
+
+    def _feat0(self):
+        """The current layer-0 input features of the inner rows (they live in the training buffer unless --use-pp)."""
+        fb = self.buffer
+        if fb._ready and (0, 0) in fb._f_off:
+            return fb._f_buf[(0, 0)][:fb._num_in, :self.args.n_feat]
+        return self.feat
+
+    def _predict_steps(self, st, model):
+        """One rank's eval forward (generator); `model` is in eval mode for the whole call (`_eval_mode`)."""
+        xch = st.xch
+        xch.begin()
+        if not self.args.use_pp:
+            d = self.args.n_feat
+            xch.inner(0, d).copy_(st.feat if st.feat is not None else self._feat0())
+            n_halo = xch.halo(0, d).shape[0]
+            if st.x0 is not None and n_halo:
+                xch.halo(0, d).copy_(st.x0[:n_halo])
+        logits = yield from model.forward_partitioned(st.graph, xch, st.pp_feat, push0=st.push0)
+        return logits
+
+    @staticmethod
+    def _eval_key(eval_layout):
+        return None if eval_layout is None else id(eval_layout)
+
+    def _count(self, eval_layout, logits) -> torch.Tensor:
+        """[2, 2] int64 (correct, total) of this rank's validation and test rows (pg_eval_count)."""
+        from . import ops
+        st = self._evals[self._eval_key(eval_layout)]
+        counts, _ = ops.eval_count(logits, st.label, st.tag, 2)
+        return counts
+
+    def _predict(self, eval_layout, model):
+        if getattr(self.world, 'is_local', False) and self.world.size > 1:
+            raise RuntimeError("the ranks of a LocalWorld evaluate together: use LocalTrainer.predict / evaluate")
+        model = self.model if model is None else model
+        k = self._eval_key(eval_layout)
+        with torch.no_grad(), _eval_mode([model]):
+            if k not in self._evals:
+                self._evals[k] = _drain(self._eval_open_steps(eval_layout))
+            st = self._evals[k]
+            logits = _drain(self._predict_steps(st, model))
+        st.xch.check_status()
+        return logits
+
+    def predict(self, eval_layout=None, model=None) -> torch.Tensor:
+        """Eval-mode logits [N_in, C] of this rank's inner rows of `eval_layout` (None: the training layout), over an
+        exact halo exchange with the peers (collective: every rank calls it; the ranks of a LocalWorld go through
+        `LocalTrainer.predict`).  `model`: another model of the same shape (default: this rank's replica); it keeps
+        its train / eval mode."""
+        logits = self._predict(eval_layout, model)
+        if self.world.size > 1:
+            # the exchange's two buffers are reused by the next call: its first push into a peer's buffers must not
+            # overtake that peer's last read of this call (`evaluate` gets the same separation from its count sum)
+            self.world.all_reduce_sum_(torch.zeros(1, device=self.device))
+        return logits
+
+    def evaluate(self, eval_layout=None, model=None):
+        """(validation accuracy, test accuracy) over the inner rows of every rank: per-rank counts summed across the
+        world with `all_reduce_sum_` -- what `calc_acc` returns on the whole graph (nan for an empty mask).
+        Collective."""
+        counts = self._count(eval_layout, self._predict(eval_layout, model))
+        if self.world.size > 1:
+            self.world.all_reduce_sum_(counts)
+        return accuracies(counts)
+
+    def release_eval(self, eval_layout=None):
+        """Free the eval exchange heap of `eval_layout` (collective)."""
+        st = self._evals.pop(None if eval_layout is None else id(eval_layout), None)
+        if st is not None:
+            st.xch.release()
+
+    @property
+    def eval_heap_bytes(self) -> int:
+        return sum(st.xch.heap_bytes for st in self._evals.values())
+
+
+def _drain(gen):
+    """Run a collective step generator of one rank to the end; its return value."""
+    try:
+        while True:
+            next(gen)
+    except StopIteration as stop:
+        return stop.value
+
+
+def _lockstep(gens, streams):
+    """Step the generators of all LocalWorld ranks round by round, each on its rank's stream: every rank reaches
+    its next yield (after its halo push) before any rank goes on to its wait."""
+    cur = torch.cuda.current_stream()
+    for s in streams:
+        s.wait_stream(cur)
+    out = [None] * len(gens)
+    live = list(range(len(gens)))
+    while live:
+        nxt = []
+        for i in live:
+            with torch.cuda.stream(streams[i]):
+                try:
+                    next(gens[i])
+                    nxt.append(i)
+                except StopIteration as stop:
+                    out[i] = stop.value
+        live = nxt
+    for s in streams:
+        cur.wait_stream(s)
+    return out
+
+
+def accuracies(counts: torch.Tensor):
+    """[k, 2] (correct, total) -> k accuracies (calc_acc: nan for an empty mask)."""
+    c = counts.cpu().tolist()
+    return tuple(float(a) / b if b else float('nan') for a, b in c)
+
 
 class LocalTrainer:
     """Lock-step driver of all ranks of a LocalWorld on one GPU (one stream per rank)."""
@@ -361,18 +561,68 @@ class LocalTrainer:
             e.buffer.check_status()
         return losses
 
+    # ---- partitioned evaluation, all ranks in lock-step (each rank pushes a layer before any rank waits on it)
+    def predict(self, eval_layouts=None, model=None) -> List[torch.Tensor]:
+        """Eval-mode logits of every rank's inner rows (`RankEngine.predict`); `eval_layouts`: one layout per rank, or
+        None for the training layouts; `model`: one model all ranks evaluate (default: each rank's replica), which
+        keeps its train / eval mode.  Consecutive calls are separated by the host: a call's streams join the current
+        stream at its end, and the next call's streams start after it."""
+        lays = eval_layouts if eval_layouts is not None else [None] * len(self.engines)
+        models = [model] * len(self.engines) if model is not None else [e.model for e in self.engines]
+        with torch.no_grad(), _eval_mode(models):
+            missing = [i for i, (e, l) in enumerate(zip(self.engines, lays)) if e._eval_key(l) not in e._evals]
+            if missing:
+                assert len(missing) == len(self.engines), "every rank sets up its eval exchange at the same time"
+                states = _lockstep([e._eval_open_steps(l) for e, l in zip(self.engines, lays)], self.streams)
+                for e, l, st in zip(self.engines, lays, states):
+                    e._evals[e._eval_key(l)] = st
+            logits = _lockstep([e._predict_steps(e._evals[e._eval_key(l)], m)
+                                for e, l, m in zip(self.engines, lays, models)], self.streams)
+        for e, l in zip(self.engines, lays):
+            e._evals[e._eval_key(l)].xch.check_status()
+        return logits
 
-def run(layout: PartitionLayout, args, world=None, eval_graph=None):
+    def evaluate(self, eval_layouts=None, model=None):
+        """(validation accuracy, test accuracy) over all ranks: per-rank device counts, summed on the host."""
+        lays = eval_layouts if eval_layouts is not None else [None] * len(self.engines)
+        logits = self.predict(eval_layouts, model)
+        total = sum(e._count(l, z).cpu() for e, l, z in zip(self.engines, lays, logits))
+        return accuracies(total)
+
+    def release_eval(self, eval_layouts=None):
+        lays = eval_layouts if eval_layouts is not None else [None] * len(self.engines)
+        torch.cuda.synchronize()
+        for e, l in zip(self.engines, lays):
+            e.release_eval(l)
+
+
+def run(layout: PartitionLayout, args, world=None, eval_graph=None, eval_layouts=None):
     """One rank's training loop with the reference's log line, evaluation and checkpoint (train.py:341-400).
-    `eval_graph`: the global graph rank 0 evaluates on every `log_every` epochs when `args.eval` is set."""
+    `eval_graph`: the global graph rank 0 evaluates on every `log_every` epochs when `args.eval` is set.
+    With `args.eval_partitioned` every rank evaluates its own inner rows instead (no global graph anywhere); for
+    --inductive `eval_layouts` (helper.utils.InductiveEvalLayouts) builds the validation and test layouts."""
     if world is None:
         from .world import default_world
         world = default_world()
     rank = world.rank
     engine = RankEngine(layout, args, world, buffer=ctx.buffer, reducer=ctx.reducer)
     timer = engine.buffer.timer
-    do_eval = bool(getattr(args, 'eval', False)) and rank == 0
-    eval_set = best = result_file_name = None
+    part_eval = bool(getattr(args, 'eval', False)) and bool(getattr(args, 'eval_partitioned', False))
+    do_eval = bool(getattr(args, 'eval', False)) and rank == 0 and not part_eval
+    inductive = bool(getattr(args, 'inductive', False))
+    eval_set = best = result_file_name = val_layout = None
+    if part_eval:
+        from .evaluate import BestModel, result_file
+        if inductive:
+            if eval_layouts is None:
+                raise ValueError("run(..., eval_layouts=None) with --inductive --eval-partitioned: pass "
+                                 "load_partition(..., return_eval_layouts=True)[1]")
+            val_layout = eval_layouts.val_layout()
+        best = BestModel()                       # every rank: the replicas are identical, so are their choices
+        if rank == 0:
+            os.makedirs('checkpoint/', exist_ok=True)
+            os.makedirs('results/', exist_ok=True)
+            result_file_name = result_file(args)
     if do_eval:
         if eval_graph is None:
             raise ValueError("run(..., eval_graph=None) with args.eval set: rank 0 needs the global graph "
@@ -415,6 +665,17 @@ def run(layout: PartitionLayout, args, world=None, eval_graph=None):
             else:
                 val_acc = evaluate_induc(name, engine.model, eval_set.val, 'val', result_file_name)
             best.offer(val_acc, engine.model)
+        if part_eval and (epoch + 1) % args.log_every == 0:               # collective: every rank evaluates
+            from .evaluate import _emit
+            name = 'Epoch %05d' % epoch
+            val_acc, test_acc = engine.evaluate(val_layout)
+            if rank == 0:
+                if not inductive:
+                    _emit("{:s} | Validation Accuracy {:.2%} | Test Accuracy {:.2%}".format(name, val_acc, test_acc),
+                          result_file_name)
+                else:
+                    _emit("{:s} | Accuracy {:.2%}".format(name, val_acc), result_file_name)
+            best.offer(val_acc, engine.model)
     engine.buffer.synchronize()
     if do_eval and best.state is not None:                                # train.py:392-400
         path = best.save(args)
@@ -424,6 +685,26 @@ def run(layout: PartitionLayout, args, world=None, eval_graph=None):
         final.load_state_dict(best.state)
         engine.test_acc = evaluate_induc('Test Result', final, eval_set.test, 'test')
         engine.best_val_acc, engine.checkpoint_path = best.acc, path
+    if part_eval and best.state is not None:
+        from .evaluate import _emit
+        path = best.save(args) if rank == 0 else None
+        if rank == 0:
+            print('model saved')
+            print("Validation accuracy {:.2%}".format(best.acc))
+        final = create_model(engine.layer_size, args, buffer=engine.buffer, dtype=engine.dtype).to(engine.device)
+        final.load_state_dict(best.state)
+        test_layout = val_layout
+        if inductive:                            # the test graph (all nodes) is built once the val heap is gone
+            engine.release_eval(val_layout)
+            val_layout = None
+            test_layout = eval_layouts.test_layout()
+        engine.test_acc = engine.evaluate(test_layout, model=final)[1]
+        if rank == 0:
+            _emit("{:s} | Accuracy {:.2%}".format('Test Result', engine.test_acc), None)
+        engine.release_eval(test_layout)
+        engine.best_val_acc, engine.checkpoint_path = best.acc, path
+    if part_eval:
+        engine.release_eval(val_layout)
     return engine
 
 
@@ -450,11 +731,18 @@ def init_processes(rank, size, args):
     dist.init_process_group('nccl', rank=rank, world_size=size, device_id=torch.device('cuda', rank))
     check_parser(args)
     from .helper.utils import load_partition
-    want_graph = bool(getattr(args, 'eval', False)) and rank == 0
-    out = load_partition(args, rank, return_graph=want_graph)
-    layout, g_full = out if want_graph else (out, None)
+    part_eval = bool(getattr(args, 'eval', False)) and bool(getattr(args, 'eval_partitioned', False))
+    want_graph = bool(getattr(args, 'eval', False)) and rank == 0 and not part_eval
+    want_layouts = part_eval and bool(getattr(args, 'inductive', False))
+    g_full = eval_layouts = None
+    if want_graph:
+        layout, g_full = load_partition(args, rank, return_graph=True)
+    elif want_layouts:
+        layout, eval_layouts = load_partition(args, rank, return_eval_layouts=True)
+    else:
+        layout = load_partition(args, rank)
     try:
-        return run(layout, args, eval_graph=g_full)
+        return run(layout, args, eval_graph=g_full, eval_layouts=eval_layouts)
     finally:
         torch.cuda.synchronize()
         dist.barrier()
