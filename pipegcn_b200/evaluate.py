@@ -1,8 +1,8 @@
 """Accuracy evaluation and checkpointing around the hot path.
 
-Counterparts of PipeGCN/train.py: `calc_acc` (:11-17), `evaluate_induc`
-(:20-39), `evaluate_trans` (:42-61) and the best-model bookkeeping of `run`
-(:377-400).  The reference deep-copies the model, moves it to the CPU and evaluates on
+Counterparts of PipeGCN/train.py: `calc_acc` (:11-17), the accuracies of
+`evaluate_induc` (:20-39) and `evaluate_trans` (:42-61) and the best-model bookkeeping of `run`
+(:377-400); `train.run` prints and writes them.  The reference deep-copies the model, moves it to the CPU and evaluates on
 the whole DGL graph from a worker thread; here the SAME sm_90a kernels evaluate the
 homogeneous full graph on the GPU (the eval branch of GraphSAGELayer, layer.py:52-62),
 on the training stream, from the live weights.
@@ -77,22 +77,11 @@ def _emit(buf: str, result_file_name: Optional[str]):
     print(buf)
 
 
-def evaluate_trans(name, model, part, result_file_name=None) -> float:
-    """train.py:42-61: validation and test accuracy on the full graph; returns the validation accuracy."""
+def accuracies(model, part, masks) -> tuple:
+    """The accuracies of `model` over the rows of each mask in `masks` (keys of `part`), from one forward: what
+    `evaluate_trans` (train.py:42-61, validation and test) and `evaluate_induc` (train.py:20-39, one mask) print."""
     logits = _logits(model, part)
-    val_acc = calc_acc(logits[part["val_mask"]], part["label"][part["val_mask"]])
-    test_acc = calc_acc(logits[part["test_mask"]], part["label"][part["test_mask"]])
-    _emit("{:s} | Validation Accuracy {:.2%} | Test Accuracy {:.2%}".format(name, val_acc, test_acc), result_file_name)
-    return val_acc
-
-
-def evaluate_induc(name, model, part, mode, result_file_name=None) -> float:
-    """train.py:20-39; mode: 'val' or 'test'."""
-    logits = _logits(model, part)
-    mask = part[mode + "_mask"]
-    acc = calc_acc(logits[mask], part["label"][mask])
-    _emit("{:s} | Accuracy {:.2%}".format(name, acc), result_file_name)
-    return acc
+    return tuple(calc_acc(logits[part[m]], part["label"][part[m]]) for m in masks)
 
 
 def result_file(args) -> str:

@@ -57,6 +57,101 @@ class _MsgSet:
         self.ptr = self.dev.data_ptr()
 
 
+class _Exchange:
+    """The protocol every halo exchange here shares: the row map of the [num_all] space, the per-peer boundary index,
+    a symmetric heap whose flag words come first (word [row][j] = the last value peer j published for flag row `row`),
+    the peers' mappings, and the push / flag-wait launches with their timeout status."""
+
+    def _init_rows(self, world, num_in, num_all, boundary, recv_shape, dtype):
+        self._world = world
+        rank, size, dev = world.rank, world.size, world.device
+        self._num_in, self._num_all = int(num_in), int(num_all)
+        self._dtype, self._es = dtype, torch.empty(0, dtype=dtype).element_size()
+        self._recv_shape = list(recv_shape)
+        self._peers = [j for j in range(size) if j != rank]
+        # rows [pl[j], pl[j] + recv_shape[j]) of the [num_all] space hold peer j's halo (feature_buffer.py:33-43)
+        self._pl, self._bidx = [None] * size, [None] * size
+        tot = self._num_in
+        for j in self._peers:
+            self._pl[j] = tot
+            tot += int(recv_shape[j])
+            self._bidx[j] = boundary[j].to(device=dev, dtype=torch.int32).contiguous()
+        assert tot == self._num_all, f"recv shapes {recv_shape} do not add up to num_all={num_all}"
+        self._status = torch.zeros(1, dtype=torch.int32, device=dev)
+        self._mapped = []
+        self._connected = False
+
+    def _publish(self, key, nbytes, table, flag_shape):
+        """Allocate the heap (flags of `flag_shape` first) and publish its token with `table` under `key`."""
+        w = self._world
+        self._key = key
+        self._heap = Heap(nbytes, w.device)
+        self._flags = self._heap.view(0, flag_shape, torch.int32)
+        w.publish(key, dict(heap=w.heap_token(self._heap), **table))
+
+    def _map_peers(self):
+        """Every rank's table and the base address of each peer's heap (needs every rank's table)."""
+        w = self._world
+        tables = w.collect(self._key)
+        self._mapped = [tables[j]['heap'] for j in self._peers]
+        base = {j: w.map_peer(t) for j, t in zip(self._peers, self._mapped)}
+        self._connected = True
+        return tables, base
+
+    def _flag_ptr(self, base, row):          # word [row][this rank] of the flags of the peer heap at `base`
+        return base + 4 * (row * self._world.size + self._world.rank)
+
+    def _wait_ptrs(self, row):
+        """Device array of this rank's flag words [row][j] for every peer j (None without peers)."""
+        size = self._world.size
+        ptrs = [self._heap.ptr + 4 * (row * size + j) for j in self._peers]
+        return torch.tensor(ptrs, dtype=torch.int64, device=self._world.device) if ptrs else None
+
+    def _msg_set(self, msgs):
+        return _MsgSet(msgs, self._world.device) if msgs else None
+
+    def _halo_push(self, ms: Optional[_MsgSet], src, d, value, value_dev=None, momentum=0.0, drop=None):
+        """Send the rows of `src` the messages name, publish `value` (+ *value_dev) in their flag words.  `drop`: the
+        RECEIVER's dropout key, applied to the rows as they are stored into its buffer."""
+        if ms is None:
+            return
+        _C.count()
+        if drop is not None and drop.p > 0:
+            _C.check(_C.lib.pg_halo_push_drop(ms.ptr, ms.n_msgs, ms.n_ctas, src.data_ptr(), src.stride(0), d,
+                                              _C.dtype_code(src.dtype), momentum, 1 - momentum,
+                                              value, value_dev, C.byref(drop.c()), _C.stream_ptr()), "pg_halo_push_drop")
+            return
+        _C.check(_C.lib.pg_halo_push(ms.ptr, ms.n_msgs, ms.n_ctas, src.data_ptr(), src.stride(0), d,
+                                     _C.dtype_code(src.dtype), momentum, 1 - momentum,
+                                     value, value_dev, _C.stream_ptr()), "pg_halo_push")
+
+    def _halo_wait(self, ptrs, value, value_dev=None, wait_ns=None):
+        """Block the stream until the flag words `ptrs` hold `value` (+ *value_dev), for at most `timeout_ms` (a
+        timeout is reported by `check_status`); the kernel adds its blocked time to the device int64 `wait_ns`."""
+        if ptrs is None:
+            return
+        _C.count()
+        _C.check(_C.lib.pg_halo_wait(ptrs.data_ptr(), ptrs.numel(), value, value_dev, self.timeout_ms,
+                                     self._status.data_ptr(), wait_ns, _C.stream_ptr()), "pg_halo_wait")
+
+    def check_status(self):
+        """Raises if a flag wait timed out since the last check (host sync)."""
+        if int(self._status.item()) != 0:
+            self._status.zero_()
+            raise _C.PgError(self._timeout_text())
+
+    def release(self):
+        """Give the symmetric heap back: close the peers' mappings, wait for every rank (they close theirs of this
+        heap), free.  Collective over the world; the exchange is unusable afterwards."""
+        w = self._world
+        for t in self._mapped:
+            w.unmap_peer(t)
+        self._mapped = []
+        w.barrier()
+        self._heap.free()
+        self._connected = False
+
+
 class _HaloUpdate(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feat, buf, layer, push_src, drop):
@@ -68,14 +163,12 @@ class _HaloUpdate(torch.autograd.Function):
         return ctx.buf._backward(ctx.layer, ctx.epoch, grad), None, None, None, None
 
 
-class Buffer(object):
+class Buffer(_Exchange):
 
     def __init__(self, world=None):
-        super().__init__()
         self._world = world
         self._epoch = 0
         self._ready = False
-        self._connected = False
         self._pipeline = False
         self.timeout_ms = 20000
         self.timer = comm_timer
@@ -94,22 +187,16 @@ class Buffer(object):
         if self._world is None:
             self._world = default_world()
         w = self._world
-        rank, size = w.rank, w.size
-        dev = w.device
-        self._num_in, self._num_all = int(num_in), int(num_all)
-        self._boundary = boundary
+        size, dev = w.size, w.device
+        self._init_rows(w, num_in, num_all, boundary, f_recv_shape, dtype)
         self._n_layers = len(layer_size)
         self._layer_size = list(layer_size)
         self._pipeline = bool(pipeline)
         self._epoch = 0
-        self._recv_shape = list(f_recv_shape)
         self._corr_feat, self._corr_grad = bool(corr_feat), bool(corr_grad)
         self._corr_momentum = float(corr_momentum)
         self._use_pp = bool(use_pp)
-        self._dtype = dtype
-        self._es = torch.empty(0, dtype=dtype).element_size()
         self._nver = 2 if pipeline else 1
-        self._peers = [j for j in range(size) if j != rank]
         L = self._n_layers
         # static-layer-0 shortcut (SURVEY.md §8f-2): the input features never change, so their halo rows are
         # exchanged ONCE (`static0_begin/_end`) into `x0`; what `update(0, .)` returns at epoch t is c_t * x0 with
@@ -120,34 +207,16 @@ class Buffer(object):
         self._static0_ready = False
         self._l0_one = set()
 
-        # rows [pl[j], pr[j]) of the [num_all] space hold peer j's halo (feature_buffer.py:33-43)
-        self._pl, self._pr = [None] * size, [None] * size
-        tot = self._num_in
-        for j in range(size):
-            if j == rank:
-                continue
-            self._pl[j] = tot
-            tot += int(f_recv_shape[j])
-            self._pr[j] = tot
-        assert tot == self._num_all, f"recv shapes {f_recv_shape} do not add up to num_all={num_all}"
-
         # concatenated boundary space: rows [boff[j], boff[j]+B_j) of b_recv belong to peer j
-        self._bidx = [None] * size
         self._boff = [0] * size
         btot = 0
-        for j in range(size):
-            if j == rank:
-                continue
+        for j in self._peers:
             self._boff[j] = btot
-            self._bidx[j] = boundary[j].to(device=dev, dtype=torch.int32).contiguous()
             btot += int(boundary[j].numel())
-        self._btot = btot
 
-        # ---- carve the symmetric heap
+        # ---- carve the symmetric heap: flags [L][2][P] (row l * 2 + direction), then the row blocks
         self._ld = [_round_up(d, 8) for d in layer_size]
-        off = 0
-        self._flag_off = off
-        off = _round_up(off + 4 * L * 2 * size, _ALIGN)
+        off = _round_up(4 * L * 2 * size, _ALIGN)
         self._f_off, self._b_off = {}, {}
         for l in range(L):
             if l == 0 and use_pp:
@@ -162,10 +231,12 @@ class Buffer(object):
         if self._static0:
             self._x0_off = off
             off = _round_up(off + max(self._num_all - self._num_in, 1) * self._ld[0] * self._es, _ALIGN)
-        self._heap = Heap(max(off, _ALIGN), dev)
+        self._publish(key, max(off, _ALIGN), {
+            'f_off': dict(self._f_off), 'b_off': dict(self._b_off), 'pl': list(self._pl), 'boff': list(self._boff),
+            'ld': list(self._ld), 'nver': self._nver, 'es': self._es, 'x0_off': self._x0_off, 'num_in': self._num_in,
+        }, (L, 2, size))
         self._x0 = None if self._x0_off is None else self._heap.view(
             self._x0_off, (max(self._num_all - self._num_in, 1), self._ld[0]), dtype)
-        self._flags = self._heap.view(self._flag_off, (L, 2, size), torch.int32)
         self._f_buf = {k: self._heap.view(o, (self._num_all, self._ld[k[0]]), dtype) for k, o in self._f_off.items()}
         self._b_recv = {k: self._heap.view(o, (max(btot, 1), self._ld[k[0]]), dtype) for k, o in self._b_off.items()}
 
@@ -197,30 +268,20 @@ class Buffer(object):
             self._urow = self._uptr = self._usrc = None
 
         self._counters = torch.zeros(max(1, (4 * L * self._nver + 1) * size), dtype=torch.int32, device=dev)
-        self._status = torch.zeros(1, dtype=torch.int32, device=dev)
         # nanoseconds the compute stream spent blocked in flag waits, accumulated by the wait kernel itself
         # (comm_timer.py:17-27's exposed-comm metric where host events cannot be used: CUDA-graph replays)
         self._wait_ns = torch.zeros(1, dtype=torch.int64, device=dev)
-        self._epoch_dev = torch.zeros(1, dtype=torch.int32, device=dev)    # == self._epoch, readable by kernels
+        self.epoch_dev = torch.zeros(1, dtype=torch.int32, device=dev)    # == self._epoch, readable by kernels
         self._comm_stream = torch.cuda.Stream(device=dev) if dev.type == 'cuda' else None
         self._push_done = {}
         self._comm_forked = False
         self._keep = []
-
-        self._key = key
-        w.publish(key, {
-            'heap': w.heap_token(self._heap), 'f_off': dict(self._f_off), 'b_off': dict(self._b_off),
-            'flag_off': self._flag_off, 'pl': list(self._pl), 'boff': list(self._boff), 'ld': list(self._ld),
-            'n_layers': L, 'nver': self._nver, 'es': self._es, 'x0_off': self._x0_off, 'num_in': self._num_in,
-        })
-        self._ready, self._connected = True, False
+        self._ready = True
 
     def _connect(self):
         """Map the peers' heaps and build the message descriptors (needs every rank's table)."""
-        w = self._world
-        rank, size, dev = w.rank, w.size, w.device
-        tables = w.collect(self._key)
-        base = {j: w.map_peer(tables[j]['heap']) for j in range(size)}
+        rank = self._world.rank
+        tables, base = self._map_peers()
         L, es = self._n_layers, self._es
         for j in self._peers:
             t = tables[j]
@@ -231,23 +292,19 @@ class Buffer(object):
         def counter_ptr():
             return self._counters.data_ptr() + 4 * next(cnt)
 
-        def flag_ptr(j, l, direction):
-            # word (l, direction, source=rank) of rank j's flag array
-            return base[j] + tables[j]['flag_off'] + 4 * ((l * 2 + direction) * size + rank)
-
         self._self_msgs, self._fwd_msgs, self._bwd_msgs = {}, {}, {}
         for (l, v) in self._f_off:
             ld = self._ld[l]
             m = _C.pg_msg(None, 0, self._num_in, 0, self._f_buf[(l, v)].data_ptr(), ld, None, 0, None, None, 0)
-            self._self_msgs[(l, v)] = _MsgSet([m], dev)
+            self._self_msgs[(l, v)] = self._msg_set([m])
             msgs = []
             for j in self._peers:
                 dst = base[j] + tables[j]['f_off'][(l, v)] + tables[j]['pl'][rank] * ld * es
                 ema = self._f_ema[l][j] if self._f_ema[l] is not None else None
                 msgs.append(_C.pg_msg(self._bidx[j].data_ptr(), 0, int(self._bidx[j].numel()), 0, dst, ld,
                                       ema.data_ptr() if ema is not None else None, ld,
-                                      flag_ptr(j, l, 0), counter_ptr(), int(tables[j]['pl'][rank])))
-            self._fwd_msgs[(l, v)] = _MsgSet(msgs, dev) if msgs else None
+                                      self._flag_ptr(base[j], l * 2), counter_ptr(), int(tables[j]['pl'][rank])))
+            self._fwd_msgs[(l, v)] = self._msg_set(msgs)
         for (l, v) in self._b_off:
             ld = self._ld[l]
             msgs = []
@@ -256,8 +313,8 @@ class Buffer(object):
                 ema = self._b_ema[l][j] if self._b_ema[l] is not None else None
                 msgs.append(_C.pg_msg(None, self._pl[j], int(self._recv_shape[j]), 0, dst, ld,
                                       ema.data_ptr() if ema is not None else None, ld,
-                                      flag_ptr(j, l, 1), counter_ptr(), int(tables[j]['boff'][rank])))
-            self._bwd_msgs[(l, v)] = _MsgSet(msgs, dev) if msgs else None
+                                      self._flag_ptr(base[j], l * 2 + 1), counter_ptr(), int(tables[j]['boff'][rank])))
+            self._bwd_msgs[(l, v)] = self._msg_set(msgs)
         self._x0_msgs = None
         if self._static0:
             ld = self._ld[0]
@@ -269,16 +326,11 @@ class Buffer(object):
                 # the backward flag word of layer 0 is free (layer 0 has no gradient exchange): it carries the
                 # generation of the one-shot push
                 msgs.append(_C.pg_msg(self._bidx[j].data_ptr(), 0, int(self._bidx[j].numel()), 0, dst, ld,
-                                      None, 0, flag_ptr(j, 0, 1), counter_ptr(),
+                                      None, 0, self._flag_ptr(base[j], 1), counter_ptr(),
                                       int(tables[j]['pl'][rank] - tables[j]['num_in'])))
-            self._x0_msgs = _MsgSet(msgs, dev) if msgs else None
+            self._x0_msgs = self._msg_set(msgs)
         # device arrays of the flag words this rank waits on, per (layer, direction)
-        self._wait = {}
-        for l in range(L):
-            for direction in (0, 1):
-                ptrs = [self._heap.ptr + self._flag_off + 4 * ((l * 2 + direction) * size + j) for j in self._peers]
-                self._wait[(l, direction)] = torch.tensor(ptrs, dtype=torch.int64, device=dev) if ptrs else None
-        self._connected = True
+        self._wait = {(l, direction): self._wait_ptrs(l * 2 + direction) for l in range(L) for direction in (0, 1)}
 
     # ------------------------------------------------------------------ zero-copy producer interface
     def _use_version(self) -> int:
@@ -292,12 +344,29 @@ class Buffer(object):
             return None
         v = self._use_version()
         ev = self._push_done.get((layer, v))
-        if ev is not None:                       # the side-stream push of two epochs ago read these rows
+        # the side-stream push of two epochs ago read these rows (an eager epoch's event: not inside a capture)
+        if ev is not None and not self.graph_mode:
             torch.cuda.current_stream().wait_event(ev)
         return self._f_buf[(layer, v)][:self._num_in, :self._layer_size[layer]]
 
     def has_peers(self) -> bool:
         return bool(self._ready and self._peers)
+
+    @property
+    def static0_ready(self) -> bool:                # True once `static0_end` has run
+        return self._static0_ready
+
+    def input_rows(self):
+        """[N_in, d_0] inner rows of layer 0, version 0 (the input features), or None with --use-pp."""
+        if not self._ready or (0, 0) not in self._f_off:
+            return None
+        return self._f_buf[(0, 0)][:self._num_in, :self._layer_size[0]]
+
+    def static_halo(self):
+        """[num_all - N_in, d_0] raw halo rows of the static layer-0 store once exchanged, else None."""
+        if not self._static0_ready or self._x0 is None:
+            return None
+        return self._x0[:self._num_all - self._num_in, :self._layer_size[0]]
 
     def clean_view(self, layer):
         """[N_in, d] buffer for the CLEAN (not dropped-out) rows of layer `layer` in this epoch's version: with the
@@ -333,14 +402,14 @@ class Buffer(object):
             torch.cuda.current_stream().wait_stream(self._comm_stream)
         self._comm_forked = False
         self._epoch += 1
-        self._epoch_dev.add_(1)
+        self.epoch_dev.add_(1)
         self._keep.clear()
 
     def _val(self, offset: int):
         """(value, value_dev) of a flag publish / wait for epoch + offset: a host constant when running eagerly,
         an offset to the device-side epoch counter when the epoch is captured into a CUDA graph."""
         if self.graph_mode:
-            return offset & 0xffffffff, self._epoch_dev.data_ptr()
+            return offset & 0xffffffff, self.epoch_dev.data_ptr()
         return (self._epoch + offset) & 0xffffffff, None
 
     def take_wait_ns(self) -> int:
@@ -349,45 +418,26 @@ class Buffer(object):
         self._wait_ns.zero_()
         return ns
 
-    def check_status(self):
-        """Raises if a flag wait timed out since the last check (host sync)."""
-        if int(self._status.item()) != 0:
-            self._status.zero_()
-            raise _C.PgError("halo exchange: a peer's flag did not arrive within "
-                             f"{self.timeout_ms} ms (PG_ERR_TIMEOUT); rank {self._world.rank} epoch {self._epoch} "
-                             f"pipeline={self._pipeline} static0={self._static0_ready} received flags "
-                             f"[layer][fwd,bwd][source rank] = {self._flags.tolist()}")
+    def _timeout_text(self):
+        return ("halo exchange: a peer's flag did not arrive within "
+                f"{self.timeout_ms} ms (PG_ERR_TIMEOUT); rank {self._world.rank} epoch {self._epoch} "
+                f"pipeline={self._pipeline} static0={self._static0_ready} received flags "
+                f"[layer][fwd,bwd][source rank] = {self._flags.tolist()}")
 
     # ------------------------------------------------------------------ kernels
     def _push(self, ms: Optional[_MsgSet], src: torch.Tensor, d: int, offset: int, drop=None):
-        """`offset`: the flag carries epoch + offset (1 for a message of this epoch).  `drop`: the RECEIVER's dropout
-        key, applied to the rows as they are stored into its buffer."""
-        if ms is None:
-            return
-        value, value_dev = self._val(offset)
-        _C.count()
-        if drop is not None and drop.p > 0:
-            _C.check(_C.lib.pg_halo_push_drop(ms.ptr, ms.n_msgs, ms.n_ctas, src.data_ptr(), src.stride(0), d,
-                                              _C.dtype_code(src.dtype), self._corr_momentum, 1 - self._corr_momentum,
-                                              value, value_dev, C.byref(drop.c()), _C.stream_ptr()), "pg_halo_push_drop")
-            return
-        _C.check(_C.lib.pg_halo_push(ms.ptr, ms.n_msgs, ms.n_ctas, src.data_ptr(), src.stride(0), d,
-                                     _C.dtype_code(src.dtype), self._corr_momentum, 1 - self._corr_momentum,
-                                     value, value_dev, _C.stream_ptr()), "pg_halo_push")
+        """`offset`: the flag carries epoch + offset (1 for a message of this epoch)."""
+        self._halo_push(ms, src, d, *self._val(offset), self._corr_momentum, drop)
 
     def _wait_flags(self, layer: int, direction: int, offset: int, name: str):
         ptrs = self._wait[(layer, direction)]
         if ptrs is None:
             return
-        value, value_dev = self._val(offset)
         timed = not self.graph_mode                   # timing events cannot be queried inside a captured graph
         if timed:
             e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
             e0.record()
-        _C.count()
-        _C.check(_C.lib.pg_halo_wait(ptrs.data_ptr(), ptrs.numel(), value, value_dev, self.timeout_ms,
-                                     self._status.data_ptr(), self._wait_ns.data_ptr(), _C.stream_ptr()),
-                 "pg_halo_wait")
+        self._halo_wait(ptrs, *self._val(offset), self._wait_ns.data_ptr())
         if timed:
             e1.record()
             self.timer.add_events(name, e0, e1)
@@ -415,21 +465,12 @@ class Buffer(object):
         if feat.stride(1) != 1:
             feat = feat.contiguous()
         self._static0_gen += 1
-        ms = self._x0_msgs
-        if ms is not None:
-            _C.count()
-            _C.check(_C.lib.pg_halo_push(ms.ptr, ms.n_msgs, ms.n_ctas, feat.data_ptr(), feat.stride(0),
-                                         self._layer_size[0], _C.dtype_code(feat.dtype), 0.0, 1.0,
-                                         self._static0_gen, None, _C.stream_ptr()), "pg_halo_push")
+        self._halo_push(self._x0_msgs, feat, self._layer_size[0], self._static0_gen)
 
     def static0_end(self):
         if not self._static0:
             return
-        ptrs = self._wait[(0, 1)]
-        if ptrs is not None:
-            _C.count()
-            _C.check(_C.lib.pg_halo_wait(ptrs.data_ptr(), ptrs.numel(), self._static0_gen, None, self.timeout_ms,
-                                         self._status.data_ptr(), None, _C.stream_ptr()), "pg_halo_wait")
+        self._halo_wait(self._wait[(0, 1)], self._static0_gen)
         self._static0_ready = True
         self._l0_one.clear()
         if self.graph_mode and not self._corr_feat:
@@ -460,7 +501,7 @@ class Buffer(object):
         off = 0 if self._pipeline else 1
         if self._corr_feat:
             if self.graph_mode:
-                self._scale_x0(v, off, self._epoch_dev.data_ptr())
+                self._scale_x0(v, off, self.epoch_dev.data_ptr())
             else:
                 self._scale_x0(v, self._epoch + off, None)
         elif v not in self._l0_one and self._epoch + off > 0:
@@ -559,16 +600,8 @@ class Buffer(object):
                                         int(self._urow.numel()), _C.stream_ptr()), "pg_boundary_add")
 
     def release(self):
-        """Give the symmetric heap back: close the peers' mappings, wait for every rank (they close theirs of this
-        heap), free.  Collective over the world; the buffer is unusable afterwards."""
-        w = self._world
-        if self._connected:
-            for j, t in enumerate(w.collect(self._key)):
-                if j != w.rank:
-                    w.unmap_peer(t['heap'])
-        w.barrier()
-        self._heap.free()
-        self._ready = self._connected = False
+        super().release()
+        self._ready = False
 
     def synchronize(self):
         """Join the side stream (end of training / before reading buffers on the host)."""
@@ -576,7 +609,7 @@ class Buffer(object):
             torch.cuda.current_stream().wait_stream(self._comm_stream)
 
 
-class EvalExchange:
+class EvalExchange(_Exchange):
     """Forward-only, synchronous halo exchange of the partitioned evaluation, on a symmetric heap of its own.
 
     Evaluation never writes the training `Buffer`: with --enable-pipeline the version the next epoch reads already
@@ -600,44 +633,25 @@ class EvalExchange:
 
     def __init__(self, world, num_in, num_all, boundary, recv_shape, widths, n_layers, dtype,
                  key='pipegcn.eval', timeout_ms=20000):
-        w = world
-        rank, size, dev = w.rank, w.size, w.device
-        self._world, self._key = w, key
-        self._num_in, self._num_all = int(num_in), int(num_all)
+        self._init_rows(world, num_in, num_all, boundary, recv_shape, dtype)
         self._L = max(int(n_layers), 1)
-        self._dtype = dtype
-        self._es = torch.empty(0, dtype=dtype).element_size()
         self._ld = _round_up(max(list(widths) + [1]), 8)
-        self._peers = [j for j in range(size) if j != rank]
-        self._pl = [None] * size
-        tot = self._num_in
-        for j in self._peers:
-            self._pl[j] = tot
-            tot += int(recv_shape[j])
-        assert tot == self._num_all, f"recv shapes {recv_shape} do not add up to num_all={num_all}"
-        self._bidx = {j: boundary[j].to(device=dev, dtype=torch.int32).contiguous() for j in self._peers}
+        size = world.size
         # heap = flags + 2 * num_all * ld * s: independent of the number of layers
         self.flag_bytes = _round_up(4 * 2 * size, _ALIGN)
         buf_bytes = self._num_all * self._ld * self._es
         self._buf_off = [self.flag_bytes, self.flag_bytes + buf_bytes]
         self.heap_bytes = self.flag_bytes + 2 * buf_bytes
-        self._heap = Heap(self.heap_bytes, dev)
-        self._flags = self._heap.view(0, (2, size), torch.int32)
+        self._publish(key, self.heap_bytes, {'buf_off': list(self._buf_off), 'pl': list(self._pl), 'ld': self._ld,
+                                             'es': self._es}, (2, size))
         self._buf = [self._heap.view(o, (self._num_all, self._ld), dtype) for o in self._buf_off]
-        self._counters = torch.zeros(2 * size, dtype=torch.int32, device=dev)
-        self._status = torch.zeros(1, dtype=torch.int32, device=dev)
+        self._counters = torch.zeros(2 * size, dtype=torch.int32, device=world.device)
         self.timeout_ms = int(timeout_ms)
         self.seq = 0
-        self._connected = False
-        w.publish(key, {'heap': w.heap_token(self._heap), 'buf_off': list(self._buf_off), 'pl': list(self._pl),
-                        'ld': self._ld, 'es': self._es})
 
     def _connect(self):
-        w = self._world
-        rank, size, dev = w.rank, w.size, w.device
-        tables = w.collect(self._key)
-        self._tables = tables                   # the peers' heaps this rank maps: what `release` unmaps
-        ld, es = self._ld, self._es
+        rank, size, ld, es = self._world.rank, self._world.size, self._ld, self._es
+        tables, base = self._map_peers()
         self._msgs, self._wait = [None, None], [None, None]
         for b in (0, 1):
             msgs = []
@@ -645,16 +659,12 @@ class EvalExchange:
                 t = tables[j]
                 if t['ld'] != ld or t['es'] != es:
                     raise RuntimeError(f"rank {j} set up its eval exchange with another width / dtype")
-                base = w.map_peer(t['heap'])
-                dst = base + t['buf_off'][b] + t['pl'][rank] * ld * es
-                flag = base + 4 * (b * size + rank)
+                dst = base[j] + t['buf_off'][b] + t['pl'][rank] * ld * es
                 counter = self._counters.data_ptr() + 4 * (b * size + j)
                 msgs.append(_C.pg_msg(self._bidx[j].data_ptr(), 0, int(self._bidx[j].numel()), 0, dst, ld, None, 0,
-                                      flag, counter, int(t['pl'][rank])))
-            self._msgs[b] = _MsgSet(msgs, dev) if msgs else None
-            ptrs = [self._heap.ptr + 4 * (b * size + j) for j in self._peers]
-            self._wait[b] = torch.tensor(ptrs, dtype=torch.int64, device=dev) if ptrs else None
-        self._connected = True
+                                      self._flag_ptr(base[j], b), counter, int(t['pl'][rank])))
+            self._msgs[b] = self._msg_set(msgs)
+            self._wait[b] = self._wait_ptrs(b)
 
     def begin(self):
         """Start an eval call (every rank, in the same order)."""
@@ -678,79 +688,67 @@ class EvalExchange:
     def push(self, layer, d):
         """Send this rank's boundary rows of layer `layer`'s input to every peer and publish the flag (zero-row
         messages too: every peer waits for every other)."""
-        ms = self._msgs[layer % 2]
-        if ms is None:
-            return
-        src = self.inner(layer, d)
-        _C.count()
-        _C.check(_C.lib.pg_halo_push(ms.ptr, ms.n_msgs, ms.n_ctas, src.data_ptr(), src.stride(0), d,
-                                     _C.dtype_code(self._dtype), 0.0, 1.0, self._value(layer), None,
-                                     _C.stream_ptr()), "pg_halo_push")
+        self._halo_push(self._msgs[layer % 2], self.inner(layer, d), d, self._value(layer))
 
     def wait(self, layer):
         """Block the stream until every peer's layer-`layer` rows have arrived (bounded: a timeout is reported by
         `check_status`, it does not hang)."""
-        ptrs = self._wait[layer % 2]
-        if ptrs is None:
-            return
-        _C.count()
-        _C.check(_C.lib.pg_halo_wait(ptrs.data_ptr(), ptrs.numel(), self._value(layer), None, self.timeout_ms,
-                                     self._status.data_ptr(), None, _C.stream_ptr()), "pg_halo_wait")
+        self._halo_wait(self._wait[layer % 2], self._value(layer))
 
-    def check_status(self):
-        """Raises if a flag wait timed out since the last check (host sync)."""
-        if int(self._status.item()) != 0:
-            self._status.zero_()
-            raise _C.PgError(f"eval halo exchange: a peer's flag did not arrive within {self.timeout_ms} ms "
-                             f"(PG_ERR_TIMEOUT); rank {self._world.rank} eval call {self.seq} received flags "
-                             f"[buffer][source rank] = {self._flags.tolist()}")
+    def _timeout_text(self):
+        return (f"eval halo exchange: a peer's flag did not arrive within {self.timeout_ms} ms "
+                f"(PG_ERR_TIMEOUT); rank {self._world.rank} eval call {self.seq} received flags "
+                f"[buffer][source rank] = {self._flags.tolist()}")
 
     def release(self):
-        """Give the heap back (collective over the world, like `Buffer.release`)."""
-        w = self._world
-        if self._connected:
-            for j, t in enumerate(self._tables):
-                if j != w.rank:
-                    w.unmap_peer(t['heap'])
-        w.barrier()
-        self._heap.free()
+        super().release()
         self._buf = None
-        self._connected = False
 
 
-class OneShotExchange:
-    """One exchange of the halo rows of a static [N_in, d] tensor (the raw input features) through a non-pipelined
-    `Buffer`: the first half of --use-pp's precompute (PipeGCN/train.py:169-189) and the layer-0 halo rows of an
-    evaluation layout.  `push`, then `wait` (with several LocalWorld ranks in one process every rank pushes before any
-    rank waits), then `release` once every rank has waited (collective for a DistWorld)."""
+class OneShotExchange(_Exchange):
+    """One exchange of the halo rows of a static [N_in, d] tensor (the raw input features): the first half of
+    --use-pp's precompute (PipeGCN/train.py:169-189) and the layer-0 halo rows of an evaluation layout.  `push`, then
+    `wait` (every rank pushes before any rank waits), then `release` once every rank has waited.  Heap: flags [1][2][P],
+    then rows [num_all, round_up(d, 8)] -- the layout of a one-layer, non-pipelined `Buffer`."""
 
-    def __init__(self, world, lay, d, dtype, backend, key, timeout_ms=None):
-        from .timer.comm_timer import CommTimer
-        self._d = int(d)
-        self._buf = Buffer(world)
-        self._buf.timer = CommTimer()
-        if timeout_ms is not None:
-            self._buf.timeout_ms = int(timeout_ms)
-        self._buf.init_buffer(lay.num_in, lay.num_all, lay.boundary, lay.recv_shape, [self._d], backend=backend,
-                              pipeline=False, dtype=dtype, world=world, key=key)
-        self.pushed = False
+    def __init__(self, world, lay, d, dtype, key, timeout_ms=20000):
+        self._init_rows(world, lay.num_in, lay.num_all, lay.boundary, lay.recv_shape, dtype)
+        self.timeout_ms = int(timeout_ms)
+        self._d, self._ld = int(d), _round_up(int(d), 8)
+        size = world.size
+        row_off = _round_up(4 * 2 * size, _ALIGN)
+        self._publish(key, _round_up(row_off + self._num_all * self._ld * self._es, _ALIGN),
+                      {'row_off': row_off, 'pl': list(self._pl)}, (1, 2, size))
+        self._rows = self._heap.view(row_off, (self._num_all, self._ld), dtype)
+        self._counters = torch.zeros(size, dtype=torch.int32, device=world.device)
+
+    def _connect(self):
+        rank, ld, es = self._world.rank, self._ld, self._es
+        tables, base = self._map_peers()
+        self._self_msgs = self._msg_set([_C.pg_msg(None, 0, self._num_in, 0, self._rows.data_ptr(), ld, None, 0,
+                                                   None, None, 0)])
+        msgs = []
+        for k, j in enumerate(self._peers):
+            t = tables[j]
+            dst = base[j] + t['row_off'] + t['pl'][rank] * ld * es
+            msgs.append(_C.pg_msg(self._bidx[j].data_ptr(), 0, int(self._bidx[j].numel()), 0, dst, ld, None, 0,
+                                  self._flag_ptr(base[j], 0), self._counters.data_ptr() + 4 * k, int(t['pl'][rank])))
+        self._msgs = self._msg_set(msgs)
+        self._wait = self._wait_ptrs(0)
 
     def push(self, feat):
         """Copy `feat` into the inner rows and send its boundary rows to every peer."""
-        b = self._buf
-        b._connect()
+        if not self._connected:
+            self._connect()
         feat = feat if feat.stride(1) == 1 else feat.contiguous()
-        b._push(b._self_msgs[(0, 0)], feat, self._d, 0)
-        b._push(b._fwd_msgs[(0, 0)], feat, self._d, 1)
-        self.pushed = True
+        self._halo_push(self._self_msgs, feat, self._d, 0)
+        self._halo_push(self._msgs, feat, self._d, 1)
 
     def wait(self) -> torch.Tensor:
         """Block the stream until the peers' rows have arrived; [num_all, d]: inner rows, then halo rows."""
-        self._buf._wait_flags(0, 0, 1, 'forward_0')
-        return self._buf._f_buf[(0, 0)][:, :self._d]
+        self._halo_wait(self._wait, 1)
+        return self._rows[:, :self._d]
 
-    def check_status(self):
-        self._buf.check_status()
-
-    def release(self):
-        self._buf.release()
+    def _timeout_text(self):
+        return (f"one-shot halo exchange '{self._key}': a peer's flag did not arrive within {self.timeout_ms} ms "
+                f"(PG_ERR_TIMEOUT); rank {self._world.rank} received flags [source rank] = {self._flags[0, 0].tolist()}")

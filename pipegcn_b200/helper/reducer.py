@@ -18,7 +18,7 @@ class Reducer(object):
         self._params = []
         self._pending = {}
         self._n_train = None
-        self._flat = None
+        self.flat = None
 
     def init(self, model, world=None):
         if world is not None:
@@ -29,7 +29,7 @@ class Reducer(object):
         self._params = [(n, p) for n, p in model.named_parameters()]
         total = sum(p.numel() for _, p in self._params)
         dev = self._params[0][1].device if self._params else 'cpu'
-        self._flat = torch.zeros(total, dtype=torch.float32, device=dev)
+        self.flat = torch.zeros(total, dtype=torch.float32, device=dev)
         self._pending = {}
 
     def reduce(self, param, name, data, n_train):
@@ -43,7 +43,7 @@ class Reducer(object):
             return
         self.pack()
         if self._world.size > 1:
-            self._world.all_reduce_sum_(self._flat)
+            self._world.all_reduce_sum_(self.flat)
         self.unpack()
 
     def pack(self):
@@ -56,11 +56,11 @@ class Reducer(object):
             grads.append(g)
         views, off = [], 0
         for g in grads:
-            views.append(self._flat[off: off + g.numel()].view_as(g))
+            views.append(self.flat[off: off + g.numel()].view_as(g))
             off += g.numel()
         torch._foreach_copy_(views, grads)
         if self._n_train is not None:
-            self._flat.div_(self._n_train)
+            self.flat.div_(self._n_train)
         self._views = views
 
     def unpack(self):

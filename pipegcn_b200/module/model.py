@@ -65,7 +65,7 @@ class GraphSAGE(GNNBase):
     def _drop_spec(self, i):
         """Dropout key of graph layer i in this epoch (same on every rank; the step is the buffer's device-side epoch)."""
         from .. import ops
-        return ops.DropSpec(self.dropout.p, ops.layer_seed(i), getattr(self._buffer(), '_epoch_dev', None), 0)
+        return ops.DropSpec(self.dropout.p, ops.layer_seed(i), getattr(self._buffer(), 'epoch_dev', None), 0)
 
     def _norm_act(self, i, h, dest=None, fuse_drop=False):
         if self.use_norm:

@@ -29,7 +29,7 @@ import torch.nn.functional as F
 
 from .graph import PartGraph
 from .helper import context as ctx
-from .helper.feature_buffer import Buffer, OneShotExchange
+from .helper.feature_buffer import Buffer, EvalExchange, OneShotExchange
 from .helper.reducer import Reducer
 from .helper.timer.comm_timer import CommTimer
 from .module.model import GraphSAGE
@@ -103,17 +103,12 @@ class RankEngine:
                                 dtype=self.dtype, world=world,
                                 static_layer0=bool(getattr(args, 'static_layer0', True)))
         self.feat = layout.feat.to(dev).to(self.dtype)
-        self._pp = None
-        if args.use_pp:
-            self.pp_begin(layout)
-            if not getattr(world, 'is_local', False) or world.size == 1:
-                self.pp_end()
-                self.release_pp()
-        else:
-            # the static input features live in the exchange buffer of layer 0 (all versions): update(0, .) copies nothing
-            self.buffer.load_inner(0, self.feat)
-            if not getattr(world, 'is_local', False) or world.size == 1:
-                self.static0()          # LocalWorld ranks: `LocalTrainer` runs the two phases over all ranks
+        # the collective set-up; its first step (allocate and publish this rank's heaps) runs here.  The ranks of a
+        # LocalWorld run the rest together (`LocalTrainer`), every other rank runs it now
+        self.setup_steps = self._setup_steps(layout)
+        next(self.setup_steps)
+        if not self._local_peers():
+            _lockstep([self.setup_steps])
         tm = layout.train_mask.to(dev)
         self.part_train = int(tm.sum().item())
         prefix = bool(tm[:self.part_train].all().item()) if self.part_train else True
@@ -145,44 +140,27 @@ class RankEngine:
                                          val_mask=layout.val_mask, test_mask=layout.test_mask, feat=None)
         self._evals = {}
 
-    # ------------------------------------------------------------------ --use-pp (train.py:169-189)
-    def pp_begin(self, layout):
-        """One-shot exchange of the raw boundary features through the push kernel (first half of `precompute`)."""
-        self._pp = OneShotExchange(self.world, layout, self.args.n_feat, self.dtype, self.args.backend,
-                                   key='pipegcn.buffer.pp')
+    def _local_peers(self) -> bool:
+        """True for a rank of a LocalWorld with peers: its collective steps need the other ranks' steps in between."""
+        return getattr(self.world, 'is_local', False) and self.world.size > 1
 
-    def _pp_push(self):
-        self._pp.push(self.feat)
-
-    def pp_end(self):
-        """Wait for the peers' rows, neighbour mean, feat <- cat(feat, mean) (second half of `precompute`).  With
-        several LocalWorld ranks in one process every rank must have pushed before any rank waits
-        (`LocalTrainer` calls `_pp_push` on all engines first)."""
-        pp = self._pp
-        if not pp.pushed:
-            self._pp_push()
-        self.feat = pp_input(self.graph, self.feat, pp.wait())
-        torch.cuda.synchronize()
-        pp.check_status()
-        self._pp_done = pp                 # peers may still be reading its heap: freed by `release_pp`
-        self._pp = None
-
-    def release_pp(self):
-        """Free the one-shot --use-pp exchange heap (collective for a DistWorld: every rank calls it after its
-        `pp_end`; for LocalWorld ranks call it once every rank has finished `pp_end`)."""
-        pp = getattr(self, '_pp_done', None)
-        if pp is not None:
-            pp.release()
-            self._pp_done = None
-
-    def static0(self, phase=None):
-        """One-shot exchange of the static layer-0 halo rows (SURVEY.md §8f-2); `phase` 'begin' / 'end' / both."""
+    def _setup_steps(self, layout):
+        """Collective set-up (generator): the --use-pp precompute (train.py:169-189), cat(feat, neighbour mean) over
+        the raw features' halo rows, or else the one-shot exchange of the static layer-0 halo rows (SURVEY.md §8f-2)."""
         if self.args.use_pp:
+            self.feat = yield from _raw_halo_steps(self.world, layout, self.feat, self.args.n_feat, 'pipegcn.buffer.pp',
+                                                   self.buffer.timeout_ms,
+                                                   lambda rows: pp_input(self.graph, self.feat, rows))
             return
-        if phase in (None, 'begin'):
-            self.buffer.static0_begin(self.buffer._f_buf[(0, 0)][:self.buffer._num_in, :self.args.n_feat])
-        if phase in (None, 'end'):
-            self.buffer.static0_end()
+        # the static input features live in the exchange buffer of layer 0 (all versions): update(0, .) copies nothing
+        self.buffer.load_inner(0, self.feat)
+        yield 'publish'
+        yield from self._static0_steps()
+
+    def _static0_steps(self):
+        self.buffer.static0_begin(self.buffer.input_rows())
+        yield 'push'
+        self.buffer.static0_end()
 
     def forward_backward(self, keep_logits=False):
         """train.py:343-355; returns the summed loss (device tensor, no host sync)."""
@@ -205,9 +183,14 @@ class RankEngine:
     def set_features(self, feat):
         """New input features for the coming epoch (host or device tensor, [N_in, n_feat])."""
         if self.buffer.inner_view(0) is not None:
+            static0 = self.buffer.static0_ready          # new features: their halo rows have to be exchanged again
+            if static0 and self._local_peers():
+                raise RuntimeError("set_features on one rank of a LocalWorld cannot re-exchange the static layer-0 "
+                                   "halo rows (its peers would have to push at the same time): set static_layer0=False")
             # layer 0 lives in the exchange buffer, one copy per version (epoch parity): refresh all of them
             self.buffer.load_inner(0, feat.to(self.device, non_blocking=True) if not feat.is_cuda else feat)
-            self.static0()          # new features: their halo rows have to be exchanged again
+            if static0:
+                _lockstep([self._static0_steps()])
             return
         # --use-pp: `self.feat` is cat(feat, neighbour mean) (train.py:169-189); the raw half is refreshed, the mean is
         # set-up work of the reference (precompute runs once, train.py:287-288) and is not recomputed per step
@@ -270,13 +253,12 @@ class RankEngine:
         """Capture one whole epoch (forward, loss, backward with both halo exchanges, gradient all-reduce, Adam
         step) into a CUDA graph -- two graphs with --enable-pipeline, one per epoch parity, because the exchange
         buffers alternate.  Everything that changes from epoch to epoch is read from the device: the epoch counter
-        behind the flag values (`Buffer._epoch_dev`) and the dropout step.  Call after >= 3 eager epochs."""
+        behind the flag values (`Buffer.epoch_dev`) and the dropout step.  Call after >= 3 eager epochs."""
         from . import ops
         assert self.epoch >= 3, "run a few eager epochs first (allocator, lazy handles, steady-state control flow)"
         assert self.use_graph, "create the engine with args.cuda_graph=True (capturable optimizer)"
         self.buffer.graph_mode = True
-        self.buffer._push_done.clear()
-        ops.STEP_DEV = self.buffer._epoch_dev
+        ops.STEP_DEV = self.buffer.epoch_dev
         torch.cuda.synchronize()
         graphs = []
         pool = None
@@ -303,12 +285,11 @@ class RankEngine:
 
     # ------------------------------------------------------------------ partitioned evaluation (--eval-partitioned)
     # Every rank evaluates its own inner rows over an exact, synchronous halo exchange of the eval-mode activations
-    # (`EvalExchange`, a heap of its own).  The collective steps are generators that yield after every halo push: a
-    # DistWorld rank runs them to the end (`_drain`), `LocalTrainer` steps all ranks of a LocalWorld in lock-step so
-    # that every rank has pushed before any rank waits.  Callers run them under torch.no_grad().
+    # (`EvalExchange`, a heap of its own).  The collective steps are generators that yield after every halo push,
+    # driven by `_lockstep` (all ranks of a LocalWorld together, so that every rank has pushed before any rank waits).
+    # Callers run them under torch.no_grad().
     def _eval_open_steps(self, eval_layout=None):
         """Set up the partitioned evaluation of `eval_layout` (None: the training layout, transductive).  Collective."""
-        from .helper.feature_buffer import EvalExchange
         args, dev = self.args, self.device
         own = eval_layout is None
         lay = self._own_eval if own else eval_layout
@@ -338,43 +319,24 @@ class RankEngine:
         if own:
             if args.use_pp:
                 st.pp_feat = self.feat                     # cat(feat, neighbour mean), computed at set-up
-            elif self.buffer._static0_ready and self.buffer._x0 is not None:
-                # the raw halo rows of the static layer-0 shortcut (not the c_t-scaled copy update(0, .) returns);
-                # a view: `set_features` refreshes them
-                st.x0 = self.buffer._x0[:lay.num_all - lay.num_in, :args.n_feat]
             else:
-                # no kept copy of the raw halo rows: every evaluation exchanges the current features' halo rows
-                st.push0 = self.world.size > 1
+                # the raw halo rows of the static layer-0 shortcut (not the c_t-scaled copy update(0, .) returns);
+                # a view: `set_features` refreshes them.  Without that store every evaluation exchanges the current
+                # features' halo rows
+                st.x0 = self.buffer.static_halo()
+                st.push0 = st.x0 is None and self.world.size > 1
             return st
         # an evaluation layout: its features are those of the graph it was built from, static for the run
         feat = eval_layout.feat.to(dev).to(self.dtype)
-        if self.world.size == 1:
-            rows = feat
-        else:
-            one = OneShotExchange(self.world, lay, args.n_feat, self.dtype, args.backend, key=key + '.raw',
-                                  timeout_ms=self.buffer.timeout_ms)
-            yield 'publish'
-            one.push(feat)
-            yield 'push'
-            rows = one.wait()
-        if args.use_pp:
-            st.pp_feat = pp_input(st.graph, feat, rows)    # recomputed over this layout's graph
-        else:
-            st.feat = feat
-            st.x0 = rows[lay.num_in:].clone()
-        if self.world.size > 1:
-            yield 'copied'                                 # every rank has its rows: the one-shot heap may go
-            torch.cuda.synchronize()
-            one.check_status()
-            one.release()
-        return st
 
-    def _feat0(self):
-        """The current layer-0 input features of the inner rows (they live in the training buffer unless --use-pp)."""
-        fb = self.buffer
-        if fb._ready and (0, 0) in fb._f_off:
-            return fb._f_buf[(0, 0)][:fb._num_in, :self.args.n_feat]
-        return self.feat
+        def use(rows):
+            if args.use_pp:
+                st.pp_feat = pp_input(st.graph, feat, rows)    # recomputed over this layout's graph
+            else:
+                st.feat = feat
+                st.x0 = rows[lay.num_in:].clone()
+        yield from _raw_halo_steps(self.world, lay, feat, args.n_feat, key + '.raw', self.buffer.timeout_ms, use)
+        return st
 
     def _predict_steps(self, st, model):
         """One rank's eval forward (generator); `model` is in eval mode for the whole call (`_eval_mode`)."""
@@ -382,7 +344,7 @@ class RankEngine:
         xch.begin()
         if not self.args.use_pp:
             d = self.args.n_feat
-            xch.inner(0, d).copy_(st.feat if st.feat is not None else self._feat0())
+            xch.inner(0, d).copy_(st.feat if st.feat is not None else self.buffer.input_rows())
             n_halo = xch.halo(0, d).shape[0]
             if st.x0 is not None and n_halo:
                 xch.halo(0, d).copy_(st.x0[:n_halo])
@@ -401,17 +363,9 @@ class RankEngine:
         return counts
 
     def _predict(self, eval_layout, model):
-        if getattr(self.world, 'is_local', False) and self.world.size > 1:
+        if self._local_peers():
             raise RuntimeError("the ranks of a LocalWorld evaluate together: use LocalTrainer.predict / evaluate")
-        model = self.model if model is None else model
-        k = self._eval_key(eval_layout)
-        with torch.no_grad(), _eval_mode([model]):
-            if k not in self._evals:
-                self._evals[k] = _drain(self._eval_open_steps(eval_layout))
-            st = self._evals[k]
-            logits = _drain(self._predict_steps(st, model))
-        st.xch.check_status()
-        return logits
+        return _predict([self], [eval_layout], [self.model if model is None else model])[0]
 
     def predict(self, eval_layout=None, model=None) -> torch.Tensor:
         """Eval-mode logits [N_in, C] of this rank's inner rows of `eval_layout` (None: the training layout), over an
@@ -436,7 +390,7 @@ class RankEngine:
 
     def release_eval(self, eval_layout=None):
         """Free the eval exchange heap of `eval_layout` (collective)."""
-        st = self._evals.pop(None if eval_layout is None else id(eval_layout), None)
+        st = self._evals.pop(self._eval_key(eval_layout), None)
         if st is not None:
             st.xch.release()
 
@@ -445,36 +399,60 @@ class RankEngine:
         return sum(st.xch.heap_bytes for st in self._evals.values())
 
 
-def _drain(gen):
-    """Run a collective step generator of one rank to the end; its return value."""
-    try:
-        while True:
-            next(gen)
-    except StopIteration as stop:
-        return stop.value
+def _raw_halo_steps(world, lay, feat, d, key, timeout_ms, use):
+    """One-shot exchange of the raw features' halo rows (generator): publish, push, wait, hand the [num_all, d] rows
+    (inner, then halo) to `use`, then -- once every rank has used its rows -- free the heap.  Returns `use`'s result."""
+    one = OneShotExchange(world, lay, d, feat.dtype, key, timeout_ms)
+    yield 'publish'
+    one.push(feat)
+    yield 'push'
+    out = use(one.wait())
+    yield 'copied'                                     # every rank has its rows: the one-shot heap may go
+    torch.cuda.synchronize()
+    one.check_status()
+    one.release()
+    return out
 
 
-def _lockstep(gens, streams):
-    """Step the generators of all LocalWorld ranks round by round, each on its rank's stream: every rank reaches
-    its next yield (after its halo push) before any rank goes on to its wait."""
+def _lockstep(gens, streams=None):
+    """Step the collective step generators of one or more ranks round by round (each on its rank's stream, or all on
+    the current stream when `streams` is None): every rank reaches its next yield (after its halo push) before any
+    rank goes on to its wait.  Their return values."""
     cur = torch.cuda.current_stream()
-    for s in streams:
+    for s in streams or ():
         s.wait_stream(cur)
     out = [None] * len(gens)
     live = list(range(len(gens)))
     while live:
         nxt = []
         for i in live:
-            with torch.cuda.stream(streams[i]):
+            with torch.cuda.stream(streams[i] if streams else None):
                 try:
                     next(gens[i])
                     nxt.append(i)
                 except StopIteration as stop:
                     out[i] = stop.value
         live = nxt
-    for s in streams:
+    for s in streams or ():
         cur.wait_stream(s)
     return out
+
+
+def _predict(engines, lays, models, streams=None):
+    """Eval-mode logits of every engine's inner rows of its layout (None: the training layout) under its model: sets
+    up the evaluation states it is missing, runs the forward steps in lock-step, checks the exchanges."""
+    with torch.no_grad(), _eval_mode(models):
+        missing = [i for i, (e, l) in enumerate(zip(engines, lays)) if e._eval_key(l) not in e._evals]
+        if missing:
+            assert len(missing) == len(engines), "every rank sets up its eval exchange at the same time"
+            states = _lockstep([e._eval_open_steps(l) for e, l in zip(engines, lays)], streams)
+            for e, l, st in zip(engines, lays, states):
+                e._evals[e._eval_key(l)] = st
+        logits = _lockstep([e._predict_steps(e._evals[e._eval_key(l)], m) for e, l, m in zip(engines, lays, models)],
+                           streams)
+    for e, l in zip(engines, lays):
+        e._evals[e._eval_key(l)].xch.check_status()
+    return logits
 
 
 def accuracies(counts: torch.Tensor):
@@ -493,20 +471,8 @@ class LocalTrainer:
         self.world = local_world
         self.engines = [RankEngine(l, args, local_world.view(r), init_state=init_state, seg_len=seg_len)
                         for r, l in enumerate(layouts)]
-        if args.use_pp and len(layouts) > 1:          # all ranks push before any rank waits (one host thread)
-            for e, s in zip(self.engines, self.streams):
-                with torch.cuda.stream(s):
-                    e._pp_push()
-            for e, s in zip(self.engines, self.streams):
-                with torch.cuda.stream(s):
-                    e.pp_end()
-            for e in self.engines:
-                e.release_pp()
-        if not args.use_pp and len(layouts) > 1:      # static layer-0 halo: all ranks push before any rank waits
-            for ph in ('begin', 'end'):
-                for e, s in zip(self.engines, self.streams):
-                    with torch.cuda.stream(s):
-                        e.static0(ph)
+        if len(layouts) > 1:
+            _lockstep([e.setup_steps for e in self.engines], self.streams)
             torch.cuda.synchronize()
         for e in self.engines:
             e.buffer.timeout_ms = 5000
@@ -530,7 +496,7 @@ class LocalTrainer:
             dry.run_epoch()
         torch.cuda.synchronize()
         for e in dry.engines:
-            e.buffer._heap.free()
+            e.buffer.release()
         torch.cuda.set_rng_state(rng, local_world.device)
         del dry
 
@@ -549,11 +515,11 @@ class LocalTrainer:
                 e.reducer.pack()
         for s in self.streams:
             cur.wait_stream(s)
-        total = self.engines[0].reducer._flat.clone()
+        total = self.engines[0].reducer.flat.clone()
         for e in self.engines[1:]:
-            total += e.reducer._flat
+            total += e.reducer.flat
         for e in self.engines:
-            e.reducer._flat.copy_(total)
+            e.reducer.flat.copy_(total)
             e.reducer.unpack()
             e.optimizer.step()
             e.epoch += 1
@@ -569,18 +535,7 @@ class LocalTrainer:
         stream at its end, and the next call's streams start after it."""
         lays = eval_layouts if eval_layouts is not None else [None] * len(self.engines)
         models = [model] * len(self.engines) if model is not None else [e.model for e in self.engines]
-        with torch.no_grad(), _eval_mode(models):
-            missing = [i for i, (e, l) in enumerate(zip(self.engines, lays)) if e._eval_key(l) not in e._evals]
-            if missing:
-                assert len(missing) == len(self.engines), "every rank sets up its eval exchange at the same time"
-                states = _lockstep([e._eval_open_steps(l) for e, l in zip(self.engines, lays)], self.streams)
-                for e, l, st in zip(self.engines, lays, states):
-                    e._evals[e._eval_key(l)] = st
-            logits = _lockstep([e._predict_steps(e._evals[e._eval_key(l)], m)
-                                for e, l, m in zip(self.engines, lays, models)], self.streams)
-        for e, l in zip(self.engines, lays):
-            e._evals[e._eval_key(l)].xch.check_status()
-        return logits
+        return _predict(self.engines, lays, models, self.streams)
 
     def evaluate(self, eval_layouts=None, model=None):
         """(validation accuracy, test accuracy) over all ranks: per-rank device counts, summed on the host."""
@@ -608,31 +563,49 @@ def run(layout: PartitionLayout, args, world=None, eval_graph=None, eval_layouts
     engine = RankEngine(layout, args, world, buffer=ctx.buffer, reducer=ctx.reducer)
     timer = engine.buffer.timer
     part_eval = bool(getattr(args, 'eval', False)) and bool(getattr(args, 'eval_partitioned', False))
-    do_eval = bool(getattr(args, 'eval', False)) and rank == 0 and not part_eval
+    do_eval = bool(getattr(args, 'eval', False)) and (rank == 0 or part_eval)
     inductive = bool(getattr(args, 'inductive', False))
-    eval_set = best = result_file_name = val_layout = None
+    best = result_file_name = val_layout = None
     if part_eval:
-        from .evaluate import BestModel, result_file
         if inductive:
             if eval_layouts is None:
                 raise ValueError("run(..., eval_layouts=None) with --inductive --eval-partitioned: pass "
                                  "load_partition(..., return_eval_layouts=True)[1]")
             val_layout = eval_layouts.val_layout()
-        best = BestModel()                       # every rank: the replicas are identical, so are their choices
-        if rank == 0:
-            os.makedirs('checkpoint/', exist_ok=True)
-            os.makedirs('results/', exist_ok=True)
-            result_file_name = result_file(args)
-    if do_eval:
+
+        def val_accs():                          # collective: every rank evaluates
+            return engine.evaluate(val_layout)
+
+        def test_acc(model):
+            nonlocal val_layout
+            test_layout = val_layout
+            if inductive:                        # the test graph (all nodes) is built once the val heap is gone
+                engine.release_eval(val_layout)
+                val_layout = None
+                test_layout = eval_layouts.test_layout()
+            acc = engine.evaluate(test_layout, model=model)[1]
+            engine.release_eval(test_layout)
+            return acc
+    elif do_eval:
         if eval_graph is None:
             raise ValueError("run(..., eval_graph=None) with args.eval set: rank 0 needs the global graph "
                              "(load_partition(..., return_graph=True)) or pass --no-eval")
-        from .evaluate import BestModel, EvalSet, evaluate_induc, evaluate_trans, result_file
-        eval_set = EvalSet(eval_graph, engine.device, inductive=getattr(args, 'inductive', False), dtype=engine.dtype)
-        best = BestModel()
-        os.makedirs('checkpoint/', exist_ok=True)                         # train.py:258-260
-        os.makedirs('results/', exist_ok=True)
-        result_file_name = result_file(args)
+        from .evaluate import EvalSet, accuracies as full_graph_accuracies
+        eval_set = EvalSet(eval_graph, engine.device, inductive=inductive, dtype=engine.dtype)
+
+        def val_accs():
+            masks = ('val_mask',) if inductive else ('val_mask', 'test_mask')
+            return full_graph_accuracies(engine.model, eval_set.val, masks)
+
+        def test_acc(model):
+            return full_graph_accuracies(model, eval_set.test, ('test_mask',))[0]
+    if do_eval:
+        from .evaluate import BestModel, _emit, result_file
+        best = BestModel()                       # every rank that evaluates: the replicas make the same choices
+        if rank == 0:
+            os.makedirs('checkpoint/', exist_ok=True)                     # train.py:258-260
+            os.makedirs('results/', exist_ok=True)
+            result_file_name = result_file(args)
     del eval_graph
     train_dur, comm_dur, reduce_dur = [], [], []
     for epoch in range(args.n_epochs):
@@ -660,48 +633,25 @@ def run(layout: PartitionLayout, args, world=None, eval_graph=None, eval_layouts
         engine.buffer.check_status()
         if do_eval and (epoch + 1) % args.log_every == 0:                 # train.py:377-390
             name = 'Epoch %05d' % epoch
-            if not eval_set.inductive:
-                val_acc = evaluate_trans(name, engine.model, eval_set.val, result_file_name)
-            else:
-                val_acc = evaluate_induc(name, engine.model, eval_set.val, 'val', result_file_name)
-            best.offer(val_acc, engine.model)
-        if part_eval and (epoch + 1) % args.log_every == 0:               # collective: every rank evaluates
-            from .evaluate import _emit
-            name = 'Epoch %05d' % epoch
-            val_acc, test_acc = engine.evaluate(val_layout)
+            accs = val_accs()
             if rank == 0:
                 if not inductive:
-                    _emit("{:s} | Validation Accuracy {:.2%} | Test Accuracy {:.2%}".format(name, val_acc, test_acc),
+                    _emit("{:s} | Validation Accuracy {:.2%} | Test Accuracy {:.2%}".format(name, *accs[:2]),
                           result_file_name)
                 else:
-                    _emit("{:s} | Accuracy {:.2%}".format(name, val_acc), result_file_name)
-            best.offer(val_acc, engine.model)
+                    _emit("{:s} | Accuracy {:.2%}".format(name, accs[0]), result_file_name)
+            best.offer(accs[0], engine.model)
     engine.buffer.synchronize()
     if do_eval and best.state is not None:                                # train.py:392-400
-        path = best.save(args)
-        print('model saved')
-        print("Validation accuracy {:.2%}".format(best.acc))
-        final = create_model(engine.layer_size, args, buffer=engine.buffer, dtype=engine.dtype).to(engine.device)
-        final.load_state_dict(best.state)
-        engine.test_acc = evaluate_induc('Test Result', final, eval_set.test, 'test')
-        engine.best_val_acc, engine.checkpoint_path = best.acc, path
-    if part_eval and best.state is not None:
-        from .evaluate import _emit
         path = best.save(args) if rank == 0 else None
         if rank == 0:
             print('model saved')
             print("Validation accuracy {:.2%}".format(best.acc))
         final = create_model(engine.layer_size, args, buffer=engine.buffer, dtype=engine.dtype).to(engine.device)
         final.load_state_dict(best.state)
-        test_layout = val_layout
-        if inductive:                            # the test graph (all nodes) is built once the val heap is gone
-            engine.release_eval(val_layout)
-            val_layout = None
-            test_layout = eval_layouts.test_layout()
-        engine.test_acc = engine.evaluate(test_layout, model=final)[1]
+        engine.test_acc = test_acc(final)
         if rank == 0:
             _emit("{:s} | Accuracy {:.2%}".format('Test Result', engine.test_acc), None)
-        engine.release_eval(test_layout)
         engine.best_val_acc, engine.checkpoint_path = best.acc, path
     if part_eval:
         engine.release_eval(val_layout)

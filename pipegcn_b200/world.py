@@ -106,7 +106,7 @@ class LocalRank:
         pass
 
     def all_reduce_sum_(self, tensor):
-        raise RuntimeError("LocalWorld ranks reduce through LocalReducerGroup, not a collective")
+        raise RuntimeError("LocalWorld ranks reduce through LocalTrainer, not a collective")
 
 
 class DistWorld:

@@ -130,7 +130,7 @@ def test_engine_matches_reference_golden(name, static0):
                          use_pp=c.get("use_pp", False))
     eargs.static_layer0 = static0
     trainer = LocalTrainer(layouts, eargs, LocalWorld(P, "cuda"), init_state=fx["ranks"][0]["init_state"], seg_len=32)
-    assert all(e.buffer._static0_ready == (static0 and not c.get("use_pp", False)) for e in trainer.engines)
+    assert all(e.buffer.static0_ready == (static0 and not c.get("use_pp", False)) for e in trainer.engines)
     caps = [dict() for _ in range(P)]
     for r, eng in enumerate(trainer.engines):
         for i, layer in enumerate(eng.model.layers):
@@ -294,3 +294,22 @@ def test_keyed_dropout_statistics_and_row_offset():
     step.add_(1)
     assert not torch.equal(ops.dropout_rows(x, spec), y)
     assert torch.equal(ops.dropout_rows(x, spec.shifted(-1)), y)
+
+
+def test_set_features_on_one_local_rank_with_static_layer0_raises():
+    """One rank of a LocalWorld with P > 1 cannot re-exchange the static layer-0 halo rows on its own (its peers
+    would never push): `set_features` raises before launching anything instead of waiting for the flag timeout."""
+    from pipegcn_b200 import _C
+    from pipegcn_b200.train import LocalTrainer
+    from pipegcn_b200.world import LocalWorld
+    from tests.helpers import make_args, small_world
+    g, _, layouts, _ = small_world("tiny", 2)
+    _, eargs = make_args(g, 5)
+    trainer = LocalTrainer(layouts, eargs, LocalWorld(2, "cuda"))
+    eng = trainer.engines[0]
+    assert eng.buffer.static0_ready
+    launches = _C.LAUNCHES
+    with pytest.raises(RuntimeError, match="static_layer0=False"):
+        eng.set_features(layouts[0].feat.cuda())
+    assert _C.LAUNCHES == launches
+    eng.buffer.check_status()

@@ -19,7 +19,7 @@ for what in ("forward", "fwd_bwd", "fwd_bwd_next", "fwd_bwd_reduce", "full"):
     for _ in range(3):
         eng.run_epoch()
     eng.buffer.graph_mode = True
-    ops.STEP_DEV = eng.buffer._epoch_dev
+    ops.STEP_DEV = eng.buffer.epoch_dev
     torch.cuda.synchronize()
     gr = torch.cuda.CUDAGraph()
     eng.optimizer.zero_grad(set_to_none=True)
