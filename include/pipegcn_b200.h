@@ -276,6 +276,43 @@ int pg_boundary_add(void* grad, int64_t ld_grad, const void* recv, int64_t ld_re
                     const int32_t* urow, const int32_t* uptr, const int32_t* usrc, int32_t n_urow, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Boundary-node sampling (BNS-GCN, synchronous training): in epoch t rank r keeps halo row h (its row in r's `_U`
+ * space, h >= N_in) iff hash(seed, t, r, h) < thresh, thresh = round(p * 2^32); inner rows are always kept.  The
+ * hash is one function (csrc/common.cuh: bns_key / bns_keep), so the receiver, the pushing owner and the owner's
+ * boundary add draw the same sample from the key alone.  t = epoch (+ *epoch_dev when epoch_dev != NULL: the
+ * device epoch counter of a captured CUDA graph).
+ * ---------------------------------------------------------------------------------------- */
+typedef struct pg_bns {
+  uint64_t seed;
+  uint32_t thresh;
+  uint32_t epoch;
+  const uint32_t* epoch_dev;
+} pg_bns;
+
+/* mask[h - num_in] = keep(rank, h) for the halo rows h in [num_in, num_all) (bytes 0 / 1), and deg[v] = the number of
+ * kept sources of inner row v in the forward CSR (indptr [num_in + 1], indices = `_U` rows; the self loop counts):
+ * the sampled in-degree, as fp32.  One launch, one coalesced pass over the CSR. */
+int pg_bns_sample(const pg_bns* s, int32_t rank, const int32_t* indptr, const int32_t* indices, int32_t num_in,
+                  int32_t num_all, uint8_t* mask, float* deg, void* stream);
+/* pg_halo_push_drop (no EMA: the messages' ema must be NULL) that moves only the sampled rows: row i of message m is
+ * loaded and stored iff keep(keys[2m], keys[2m + 1] + i) -- keys[2m] the rank whose `_U` space the rows are keyed in,
+ * keys[2m + 1] the row of i = 0 there (the receiver and dst_row0 for a feature push, the pusher and src_row0 for a
+ * gradient push).  Flags are published as by pg_halo_push, also for messages whose sample is empty.  drop may be
+ * NULL. */
+int pg_halo_push_bns(const pg_msg* msgs, int32_t n_msgs, int32_t n_ctas, const int32_t* keys, const void* src,
+                     int64_t ld_src, int32_t d, int dtype, uint32_t value, const uint32_t* value_dev,
+                     const pg_drop* drop, const pg_bns* s, void* stream);
+/* pg_boundary_add over the kept slots only: slot k of recv is added iff keep(slot_keys[2k], slot_keys[2k + 1]) (the
+ * receiving peer and the row the slot fills in its `_U` space). */
+int pg_boundary_add_bns(void* grad, int64_t ld_grad, const void* recv, int64_t ld_recv, int32_t d, int dtype,
+                        const int32_t* urow, const int32_t* uptr, const int32_t* usrc, int32_t n_urow,
+                        const int32_t* slot_keys, const pg_bns* s, void* stream);
+/* dst[r, 0:d] = mask[r] ? src[r, 0:d] : 0 for r < n_rows; with src == NULL the kept rows of dst are left as they
+ * are (only the unkept rows are zeroed). */
+int pg_bns_mask_rows(const void* src, int64_t ld_src, void* dst, int64_t ld_dst, int32_t n_rows, int32_t d, int dtype,
+                     const uint8_t* mask, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Symmetric heap: device memory that peers map through CUDA IPC (host pointers out).
  * ---------------------------------------------------------------------------------------- */
 #define PG_IPC_HANDLE_BYTES 64

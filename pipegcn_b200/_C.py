@@ -42,6 +42,10 @@ class pg_drop(C.Structure):
     _fields_ = [("p", C.c_float), ("seed", C.c_uint64), ("step_dev", C.c_void_p), ("step_off", C.c_int32)]
 
 
+class pg_bns(C.Structure):
+    _fields_ = [("seed", C.c_uint64), ("thresh", C.c_uint32), ("epoch", C.c_uint32), ("epoch_dev", C.c_void_p)]
+
+
 def _load():
     if not _LIB_PATH.exists():
         raise PgError(f"{_LIB_PATH} is missing: build it with `python -m pipegcn_b200.build` "
@@ -82,6 +86,11 @@ def _load():
         "pg_halo_wait": (C.c_int, [vp, i32, u32, vp, i32, vp, vp, vp]),
         "pg_scale_rows": (C.c_int, [vp, i64, vp, i64, i32, i32, C.c_int, f32, C.c_int, i32, vp, vp]),
         "pg_boundary_add": (C.c_int, [vp, i64, vp, i64, i32, C.c_int, vp, vp, vp, i32, vp]),
+        "pg_bns_sample": (C.c_int, [C.POINTER(pg_bns), i32, vp, vp, i32, i32, vp, vp, vp]),
+        "pg_halo_push_bns": (C.c_int, [vp, i32, i32, vp, vp, i64, i32, C.c_int, u32, vp, C.POINTER(pg_drop),
+                                       C.POINTER(pg_bns), vp]),
+        "pg_boundary_add_bns": (C.c_int, [vp, i64, vp, i64, i32, C.c_int, vp, vp, vp, i32, vp, C.POINTER(pg_bns), vp]),
+        "pg_bns_mask_rows": (C.c_int, [vp, i64, vp, i64, i32, i32, C.c_int, vp, vp]),
         "pg_heap_alloc": (C.c_int, [C.c_size_t, C.POINTER(vp)]),
         "pg_heap_free": (C.c_int, [vp]),
         "pg_ipc_export": (C.c_int, [vp, C.c_char_p]),

@@ -198,6 +198,21 @@ __device__ __forceinline__ void drop_apply2(float2 (&f)[H], uint64_t i, uint32_t
     f[k].y = ((h >> 16) >= thresh16) ? m.y : 0.f;
   }
 }
+// ---- boundary-node sampling (pg_bns) ---------------------------------------------------------------------------------
+// Rank r keeps halo row h (its row in r's `_U` space) in epoch t iff mix32(mix32(h ^ k) + k) < thresh, with the key
+// k = bns_key(seed, t, r).  A pure function of (seed, t, r, h): the receiver, the sender and the boundary add draw
+// the same sample without exchanging it.  tests/test_boundary_sampling_cpu.py ports it to the host.
+__device__ __forceinline__ uint32_t bns_epoch(const pg_bns& s) {
+  return s.epoch + (s.epoch_dev != nullptr ? *s.epoch_dev : 0u);
+}
+__device__ __forceinline__ uint32_t bns_key(uint64_t seed, uint32_t t, uint32_t r) {
+  const uint32_t k = mix32(static_cast<uint32_t>(seed >> 32) + 0x632be5abU * (t + 1u));
+  return mix32((static_cast<uint32_t>(seed) ^ k) + 0x85ebca6bU * (r + 1u));
+}
+__device__ __forceinline__ bool bns_keep(uint32_t key, uint32_t h, uint32_t thresh) {
+  return mix32(mix32(h ^ key) + key) < thresh;
+}
+
 inline DropArg make_drop(const pg_drop* d) {
   DropArg a{0u, 1.f, 0u, 0u, nullptr, 0};
   if (d != nullptr && d->p > 0.f) {

@@ -152,6 +152,21 @@ class _Exchange:
         self._connected = False
 
 
+def check_sampling(sampling_rate, pipeline=False, corr_feat=False, corr_grad=False) -> float:
+    """The boundary-node sampling rate as a float; raises for a rate outside (0, 1] and for the combinations that are
+    not implemented (before anything is allocated)."""
+    p = float(sampling_rate)
+    if not 0.0 < p <= 1.0:
+        raise ValueError(f"--sampling-rate {sampling_rate}: expected 0 < p <= 1")
+    if p < 1.0:
+        other = [name for name, on in (('--enable-pipeline', pipeline), ('--feat-corr', corr_feat),
+                                       ('--grad-corr', corr_grad)) if on]
+        if other:
+            raise NotImplementedError(f"--sampling-rate {p} together with {' '.join(other)}: boundary-node sampling "
+                                      "is implemented for synchronous training without corrections only")
+    return p
+
+
 class _HaloUpdate(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feat, buf, layer, push_src, drop):
@@ -173,11 +188,16 @@ class Buffer(_Exchange):
         self.timeout_ms = 20000
         self.timer = comm_timer
         self.graph_mode = False      # True while an epoch is captured into / replayed from a CUDA graph
+        self._bns = False            # boundary-node sampling (init_buffer's sampling_rate < 1)
 
     # ------------------------------------------------------------------ set-up
     def init_buffer(self, num_in, num_all, boundary, f_recv_shape, layer_size, use_pp=False, backend='nccl',
                     pipeline=False, corr_feat=False, corr_grad=False, corr_momentum=0,
-                    dtype=torch.float32, world=None, key='pipegcn.buffer', static_layer0=False):
+                    dtype=torch.float32, world=None, key='pipegcn.buffer', static_layer0=False, sampling_rate=1.0,
+                    sampling_seed=0):
+        """`sampling_rate` p < 1: boundary-node sampling (synchronous, no corrections): every epoch this rank keeps a
+        random fraction p of its halo rows (`sample`), the peers push only those, the others read as zero rows."""
+        rate = check_sampling(sampling_rate, pipeline, corr_feat, corr_grad)
         if backend not in ('nccl', 'nvlink'):
             # the reference implements gloo only and raises for the rest (feature_buffer.py:204-205);
             # this engine implements the NVLink path only
@@ -273,6 +293,13 @@ class Buffer(_Exchange):
         self._wait_ns = torch.zeros(1, dtype=torch.int64, device=dev)
         self.epoch_dev = torch.zeros(1, dtype=torch.int32, device=dev)    # == self._epoch, readable by kernels
         self._comm_stream = torch.cuda.Stream(device=dev) if dev.type == 'cuda' else None
+        # boundary-node sampling: this epoch's keep mask of the halo rows and the sampled in-degree (`sample`)
+        self._bns = rate < 1.0 and bool(self._peers)
+        self._bns_rate, self._bns_seed = rate, int(sampling_seed)
+        self._bns_mask = self._bns_deg = None
+        if self._bns:
+            self._bns_mask = torch.zeros(max(self._num_all - self._num_in, 1), dtype=torch.uint8, device=dev)
+            self._bns_deg = torch.zeros(self._num_in, dtype=torch.float32, device=dev)
         self._push_done = {}
         self._comm_forked = False
         self._keep = []
@@ -329,8 +356,57 @@ class Buffer(_Exchange):
                                       None, 0, self._flag_ptr(base[j], 1), counter_ptr(),
                                       int(tables[j]['pl'][rank] - tables[j]['num_in'])))
             self._x0_msgs = self._msg_set(msgs)
+        if self._bns:
+            # sample keys (rank, `_U` row of row 0) per message: a feature push is keyed in the receiver's space, a
+            # gradient push in this rank's; slot k of b_recv by the peer that filled it and the row it filled there
+            self._bns_fwd_keys = self._keys([(j, tables[j]['pl'][rank]) for j in self._peers])
+            self._bns_bwd_keys = self._keys([(rank, self._pl[j]) for j in self._peers])
+            slots = [torch.stack([torch.full((n,), j, dtype=torch.int64), tables[j]['pl'][rank] + torch.arange(n)], 1)
+                     for j in self._peers for n in [int(self._bidx[j].numel())]]
+            self._bns_slot_keys = torch.cat(slots).to(device=self._world.device, dtype=torch.int32).contiguous()
         # device arrays of the flag words this rank waits on, per (layer, direction)
         self._wait = {(l, direction): self._wait_ptrs(l * 2 + direction) for l in range(L) for direction in (0, 1)}
+
+    def _keys(self, pairs):
+        return torch.tensor(pairs, dtype=torch.int32, device=self._world.device).reshape(-1, 2).contiguous()
+
+    # ------------------------------------------------------------------ boundary-node sampling
+    @property
+    def sampling(self) -> bool:
+        """True when epochs exchange a sample of the halo rows (rate < 1 and peers to exchange with)."""
+        return self._bns
+
+    def _bns_spec(self):
+        from ..ops import BnsSpec
+        if self.graph_mode:
+            return BnsSpec(self._bns_rate, self._bns_seed, 0, self.epoch_dev)
+        return BnsSpec(self._bns_rate, self._bns_seed, self._epoch)
+
+    def sample(self, plan):
+        """Draw this epoch's sample (one launch): the keep mask of this rank's halo rows and the sampled in-degree of
+        its inner rows over the forward CSR `plan`.  Returns the degree [N_in] fp32, the `in_deg` of this epoch."""
+        from ..ops import bns_sample
+        bns_sample(self._bns_spec(), self._world.rank, plan, self._num_in, self._num_all, self._bns_mask, self._bns_deg)
+        return self._bns_deg
+
+    def sample_mask(self):
+        """[num_all - N_in] bool copy of the current keep mask of the halo rows (None without sampling)."""
+        if not self._bns:
+            return None
+        return self._bns_mask[:self._num_all - self._num_in].bool()
+
+    def _push_bns(self, ms, keys, src, d, offset, drop=None):
+        if ms is None:
+            return
+        _C.count()
+        spec = self._bns_spec()
+        _C.check(_C.lib.pg_halo_push_bns(ms.ptr, ms.n_msgs, ms.n_ctas, keys.data_ptr(), src.data_ptr(), src.stride(0),
+                                         d, _C.dtype_code(src.dtype), *self._val(offset),
+                                         C.byref(drop.c()) if drop is not None and drop.p > 0 else None,
+                                         C.byref(spec.c()), _C.stream_ptr()), "pg_halo_push_bns")
+
+    def _halo_rows(self, layer, v):
+        return self._f_buf[(layer, v)][self._num_in:, :self._layer_size[layer]]
 
     # ------------------------------------------------------------------ zero-copy producer interface
     def _use_version(self) -> int:
@@ -499,7 +575,10 @@ class Buffer(_Exchange):
             self._push(self._self_msgs[(0, v)], feat, d, 0)
         # k = EMA updates the consumed message has seen: epoch t consumes message t-1 (pipelined) or t
         off = 0 if self._pipeline else 1
-        if self._corr_feat:
+        if self._bns:
+            from ..ops import bns_mask_rows          # this epoch's sample of x0: keep * x0, rebuilt every epoch
+            bns_mask_rows(self._bns_mask, self._halo_rows(0, v), self._x0[:self._num_all - self._num_in, :d])
+        elif self._corr_feat:
             if self.graph_mode:
                 self._scale_x0(v, off, self.epoch_dev.data_ptr())
             else:
@@ -534,7 +613,12 @@ class Buffer(_Exchange):
             v = 0
             if not aliased(v):
                 self._push(self._self_msgs[(layer, v)], feat, d, 0)
-            self._push(self._fwd_msgs[(layer, v)], src, d, 1, drop)          # consumed in this epoch: same step
+            if self._bns:
+                from ..ops import bns_mask_rows
+                self._push_bns(self._fwd_msgs[(layer, v)], self._bns_fwd_keys, src, d, 1, drop)
+                bns_mask_rows(self._bns_mask, self._halo_rows(layer, v))      # unkept halo rows read as zero
+            else:
+                self._push(self._fwd_msgs[(layer, v)], src, d, 1, drop)      # consumed in this epoch: same step
             self._wait_flags(layer, 0, 1, f'forward_{layer}')
         else:
             v_use, v_send = (t + 1) % 2, t % 2
@@ -569,7 +653,10 @@ class Buffer(_Exchange):
             grad = grad.contiguous()
         if not self._pipeline:
             v = 0
-            self._push(self._bwd_msgs[(layer, v)], grad, d, epoch - self._epoch + 1)
+            if self._bns:                             # gradients of the kept halo rows only
+                self._push_bns(self._bwd_msgs[(layer, v)], self._bns_bwd_keys, grad, d, epoch - self._epoch + 1)
+            else:
+                self._push(self._bwd_msgs[(layer, v)], grad, d, epoch - self._epoch + 1)
             self._wait_flags(layer, 1, epoch - self._epoch + 1, f'backward_{layer}')
             self._boundary_add(layer, v, grad)
         else:
@@ -594,6 +681,13 @@ class Buffer(_Exchange):
             return
         recv = self._b_recv[(layer, v)]
         _C.count()
+        if self._bns:                                 # the slots the receiving peers kept
+            _C.check(_C.lib.pg_boundary_add_bns(grad.data_ptr(), grad.stride(0), recv.data_ptr(), recv.stride(0),
+                                                self._layer_size[layer], _C.dtype_code(grad.dtype),
+                                                self._urow.data_ptr(), self._uptr.data_ptr(), self._usrc.data_ptr(),
+                                                int(self._urow.numel()), self._bns_slot_keys.data_ptr(),
+                                                C.byref(self._bns_spec().c()), _C.stream_ptr()), "pg_boundary_add_bns")
+            return
         _C.check(_C.lib.pg_boundary_add(grad.data_ptr(), grad.stride(0), recv.data_ptr(), recv.stride(0),
                                         self._layer_size[layer], _C.dtype_code(grad.dtype),
                                         self._urow.data_ptr(), self._uptr.data_ptr(), self._usrc.data_ptr(),

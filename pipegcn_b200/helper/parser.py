@@ -11,6 +11,11 @@ its own inner rows over an exact halo exchange and the accuracy counts are summe
 evaluating the whole graph, which it would have to hold a second time.  The printed lines, the result file and the
 checkpoint keep their formats.  When the flag is absent the namespace has no `eval_partitioned` attribute (read it
 with getattr(args, 'eval_partitioned', False)), so the parsed flags stay the reference's.
+
+`--sampling-rate p` (0 < p <= 1; not in the reference) turns on boundary-node sampling (BNS-GCN) in synchronous
+training: every epoch each partition keeps a random fraction p of its halo nodes and drops the rest from its graph for
+that epoch, so the halo exchange moves p times the bytes.  Evaluation always uses the full graph.  Like
+`--eval-partitioned` it has a suppressed default: read it with getattr(args, 'sampling_rate', 1.0).
 """
 import argparse
 
@@ -52,6 +57,16 @@ _FLAGS = [
 ]
 
 
+def _sampling_rate(text):
+    try:
+        p = float(text)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"invalid sampling rate '{text}'")
+    if not 0.0 < p <= 1.0:           # also refuses nan
+        raise argparse.ArgumentTypeError(f"sampling rate {text}: expected 0 < p <= 1")
+    return p
+
+
 def build_parser():
     parser = argparse.ArgumentParser(description='PipeGCN on H100')
     for flag, kw in _FLAGS:
@@ -68,6 +83,9 @@ def build_parser():
     parser.add_argument('--eval-partitioned', '--eval_partitioned', action='store_true', default=argparse.SUPPRESS,
                         help="with --eval: every rank evaluates its own nodes (exact halo exchange) instead of rank 0 "
                              "evaluating the whole graph")
+    parser.add_argument('--sampling-rate', '--sampling_rate', type=_sampling_rate, default=argparse.SUPPRESS,
+                        help="boundary-node sampling: the fraction of halo nodes every partition keeps per epoch "
+                             "(synchronous training; default 1 = all)")
     return parser
 
 

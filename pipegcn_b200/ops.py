@@ -42,6 +42,76 @@ def layer_seed(layer: int) -> int:
     return (torch.initial_seed() * 0x9E3779B97F4A7C15 + (layer + 1) * 0xD1B54A32D192ED03) & 0xFFFFFFFFFFFFFFFF
 
 
+class BnsSpec:
+    """Key of a boundary-node sample (include/pipegcn_b200.h: pg_bns): sampling rate p, 64-bit seed, and the epoch,
+    a host value or the device counter `epoch_dev` (CUDA-graph replay)."""
+
+    def __init__(self, p: float, seed: int, epoch: int = 0, epoch_dev: torch.Tensor = None):
+        self.p, self.seed = float(p), int(seed) & 0xFFFFFFFFFFFFFFFF
+        self.thresh = bns_threshold(p)
+        self.epoch, self.epoch_dev = int(epoch) & 0xFFFFFFFF, epoch_dev
+
+    def c(self):
+        return _C.pg_bns(self.seed, self.thresh, self.epoch,
+                         self.epoch_dev.data_ptr() if self.epoch_dev is not None else None)
+
+
+def bns_threshold(p: float) -> int:
+    """round(p * 2^32) as the uint32 bound of the keep test (hash < thresh); p < 1."""
+    if not 0.0 < p < 1.0:
+        raise ValueError(f"sampling rate {p}: the sampled path needs 0 < p < 1")
+    return min(int(round(p * 2.0 ** 32)), 0xFFFFFFFF)
+
+
+def bns_seed(seed: int) -> int:
+    """Seed of the boundary sample from the run's --seed (the same on every rank)."""
+    return (int(seed) * 0x9E3779B97F4A7C15 + 0xB5AD4ECEDA1CE2A9) & 0xFFFFFFFFFFFFFFFF
+
+
+def _mix32(x):
+    x = x & 0xFFFFFFFF
+    x ^= x >> 16
+    x = (x * 0x7FEB352D) & 0xFFFFFFFF
+    x ^= x >> 15
+    x = (x * 0x846CA68B) & 0xFFFFFFFF
+    x ^= x >> 16
+    return x
+
+
+def bns_keep_host(seed: int, epoch: int, rank: int, rows, thresh: int):
+    """Host port of csrc/common.cuh's bns_key / bns_keep: numpy bool array, True where rank `rank` keeps `_U` row
+    `rows` in epoch `epoch`."""
+    import numpy as np
+    seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+    k = _mix32(((seed >> 32) + 0x632BE5AB * ((epoch + 1) & 0xFFFFFFFF)) & 0xFFFFFFFF)
+    key = _mix32((((seed & 0xFFFFFFFF) ^ k) + 0x85EBCA6B * ((rank + 1) & 0xFFFFFFFF)) & 0xFFFFFFFF)
+    h = np.asarray(rows, dtype=np.uint64) & np.uint64(0xFFFFFFFF)
+    hv = _mix32((_mix32(h ^ np.uint64(key)) + np.uint64(key)) & np.uint64(0xFFFFFFFF))
+    return hv < np.uint64(thresh)
+
+
+def bns_sample(spec: BnsSpec, rank: int, plan: CsrPlan, num_in: int, num_all: int, mask: torch.Tensor,
+               deg: torch.Tensor):
+    """mask[:num_all - num_in] <- keep bytes of this rank's halo rows, deg[:num_in] <- sampled in-degrees (fp32)."""
+    assert mask.dtype == torch.uint8 and deg.dtype == torch.float32 and plan.n_rows == num_in
+    _C.count()
+    _C.check(_C.lib.pg_bns_sample(C.byref(spec.c()), int(rank), plan.indptr.data_ptr(), plan.indices.data_ptr(),
+                                  int(num_in), int(num_all), mask.data_ptr(), deg.data_ptr(), _C.stream_ptr()),
+             "pg_bns_sample")
+
+
+def bns_mask_rows(mask: torch.Tensor, dst: torch.Tensor, src: torch.Tensor = None):
+    """dst = mask ? src : 0 row by row; without `src` only the unkept rows of dst are zeroed."""
+    n, d = dst.shape
+    if n == 0:
+        return dst
+    _C.count()
+    _C.check(_C.lib.pg_bns_mask_rows(src.data_ptr() if src is not None else None, src.stride(0) if src is not None else 0,
+                                     dst.data_ptr(), dst.stride(0), n, d, _C.dtype_code(dst.dtype), mask.data_ptr(),
+                                     _C.stream_ptr()), "pg_bns_mask_rows")
+    return dst
+
+
 def _drop_ok(t: torch.Tensor) -> bool:
     """The mask is defined on 16-byte vectors of padded, aligned rows."""
     return t.dim() == 2 and t.is_cuda and t.stride(1) == 1 and (t.stride(0) * t.element_size()) % 16 == 0 \

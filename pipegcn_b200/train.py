@@ -29,11 +29,16 @@ import torch.nn.functional as F
 
 from .graph import PartGraph
 from .helper import context as ctx
-from .helper.feature_buffer import Buffer, EvalExchange, OneShotExchange
+from .helper.feature_buffer import Buffer, EvalExchange, OneShotExchange, check_sampling
 from .helper.reducer import Reducer
 from .helper.timer.comm_timer import CommTimer
 from .module.model import GraphSAGE
 from .partition import PartitionLayout, get_layer_size
+
+
+def _bns_seed(args):
+    from .ops import bns_seed
+    return bns_seed(getattr(args, 'seed', 0))
 
 
 def create_model(layer_size, args, buffer=None, dtype=torch.float32):
@@ -86,6 +91,8 @@ class RankEngine:
 
     def __init__(self, layout: PartitionLayout, args, world, buffer: Optional[Buffer] = None,
                  reducer: Optional[Reducer] = None, init_state=None, seg_len=None):
+        sampling_rate = check_sampling(getattr(args, 'sampling_rate', 1.0), args.enable_pipeline, args.feat_corr,
+                                       args.grad_corr)
         self.args, self.world, self.rank = args, world, world.rank
         dev = world.device
         self.device = dev
@@ -101,7 +108,8 @@ class RankEngine:
                                 backend=args.backend, pipeline=args.enable_pipeline, corr_feat=args.feat_corr,
                                 corr_grad=args.grad_corr, corr_momentum=args.corr_momentum,
                                 dtype=self.dtype, world=world,
-                                static_layer0=bool(getattr(args, 'static_layer0', True)))
+                                static_layer0=bool(getattr(args, 'static_layer0', True)),
+                                sampling_rate=sampling_rate, sampling_seed=_bns_seed(args))
         self.feat = layout.feat.to(dev).to(self.dtype)
         # the collective set-up; its first step (allocate and publish this rank's heaps) runs here.  The ranks of a
         # LocalWorld run the rest together (`LocalTrainer`), every other rank runs it now
@@ -165,8 +173,10 @@ class RankEngine:
     def forward_backward(self, keep_logits=False):
         """train.py:343-355; returns the summed loss (device tensor, no host sync)."""
         self.model.train()
+        # boundary-node sampling: this epoch's sample, and its in-degrees for every graph layer
+        in_deg = self.buffer.sample(self.graph.fwd) if self.buffer.sampling else self.in_deg
         feat = self.buffer.inner_view(0)
-        logits = self.model(self.graph, feat if feat is not None else self.feat, self.in_deg)
+        logits = self.model(self.graph, feat if feat is not None else self.feat, in_deg)
         if isinstance(self.train_sel, slice) and logits.dtype in (torch.float32, torch.bfloat16):
             from . import ops
             loss = ops.cross_entropy_sum(logits, self.labels, self.part_train)      # fused softmax-CE (sum)
@@ -487,10 +497,12 @@ class LocalTrainer:
         from .world import LocalWorld
         dry_args = copy.copy(args)
         dry_args.enable_pipeline = True
+        dry_args.sampling_rate = 1.0
         dry = LocalTrainer.__new__(LocalTrainer)
         dry.world = LocalWorld(local_world.size, local_world.device)
         dry.streams = self.streams
         dry.engines = [RankEngine(l, dry_args, dry.world.view(r), seg_len=seg_len) for r, l in enumerate(layouts)]
+        _lockstep([e.setup_steps for e in dry.engines], self.streams)     # --use-pp: the precompute
         rng = torch.cuda.get_rng_state(local_world.device)
         for _ in range(2):
             dry.run_epoch()
@@ -665,6 +677,7 @@ def check_parser(args):
 
 def init_processes(rank, size, args):
     """Initialise the distributed environment and train this rank (train.py:408-416)."""
+    check_sampling(getattr(args, 'sampling_rate', 1.0), args.enable_pipeline, args.feat_corr, args.grad_corr)
     os.environ['MASTER_ADDR'] = args.master_addr
     os.environ['MASTER_PORT'] = '%d' % args.port
     import torch.distributed as dist
