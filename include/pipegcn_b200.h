@@ -313,6 +313,47 @@ int pg_bns_mask_rows(const void* src, int64_t ld_src, void* dst, int64_t ld_dst,
                      const uint8_t* mask, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Graph attention (GAT, DGL GATConv with negative_slope 0.2, no attention dropout) over the `_U` rows
+ * [inner | halo] of one partition.  z [num_all, H * D] (fp32 or bf16, `dtype`) holds H heads of D columns per row;
+ * el [num_all, H] and er [N_in, H] are fp32 scores; for the in-edges u -> v of the forward CSR
+ *   e_uv = LeakyReLU(el[u] + er[v]),  a_uv = softmax over u of e_uv,  out[v] = sum_u a_uv z[u] + bias
+ * per head.  `keep` (uint8 [num_all - num_in], may be NULL) is the boundary-node sample of the halo rows: a halo row u
+ * with keep[u - num_in] == 0 is absent from every softmax and gets no gradient.  The plan must carry the chunk table
+ * (pg_csr::chunks); `scratch` is fp32 of n_seg * H * (D + 2) floats (may be NULL when n_seg == 0).  fp32 accumulation,
+ * no atomics, no per-edge storage, D <= 512; the results are the same bits from run to run.
+ * ---------------------------------------------------------------------------------------- */
+/* loads every attention kernel (call it before any halo wait can spin: a first launch may wait for the device) */
+int pg_gat_preload(void);
+/* el[r, k] = <z[r, k, :], attn_l[k, :]> for r < n_rows, er[r, k] = <z[r, k, :], attn_r[k, :]> for r < n_er */
+int pg_gat_scores(const void* z, int64_t ldz, int32_t n_rows, int32_t n_er, int32_t H, int32_t D, int dtype,
+                  const float* attn_l, const float* attn_r, float* el, float* er, void* stream);
+/* out[v] (activation dtype, bias fp32 [H * D] or NULL) and the softmax statistics m[v, k] (maximum) and s[v, k]
+ * (sum of exp(e - m)), fp32 [N_in, H], over the forward CSR g (rows = inner rows v) */
+int pg_gat_aggregate(const pg_csr* g, const void* z, int64_t ldz, int32_t H, int32_t D, int dtype, const float* el,
+                     const float* er, const float* bias, const uint8_t* keep, int32_t num_in, void* out, int64_t ldo,
+                     float* m, float* s, float* scratch, void* stream);
+/* backward over the forward CSR, grad = dL/d out:  dv[v, k] = <grad[v, k], out[v, k] - bias[k]>, evaluated as
+ * sum_u a_uv <grad[v, k], z[u, k]> (the products the second output uses, so that bf16 rounding of the stored output does
+ * not enter), and der[v, k] = sum_u a_uv (<grad[v, k], z[u, k]> - dv[v, k]) LeakyReLU'(el[u, k] + er[v, k]) */
+int pg_gat_bwd_dst(const pg_csr* g, const void* z, int64_t ldz, const void* grad, int64_t ldg, int32_t H, int32_t D,
+                   int dtype, const float* el, const float* er, const float* m, const float* s, const uint8_t* keep,
+                   int32_t num_in, float* der, float* dv, float* scratch, void* stream);
+/* backward over the CSC gt (rows = all `_U` rows u, columns = destinations v):
+ *   del[u, k] = sum_v a_uv (<grad[v, k], z[u, k]> - dv[v, k]) LeakyReLU'(el[u, k] + er[v, k])
+ *   dz[u, k] = sum_v a_uv grad[v, k] + del[u, k] attn_l[k] (+ der[u, k] attn_r[k] for u < num_in)
+ * dz in the activation dtype; unkept halo rows get dz = 0, del = 0 */
+int pg_gat_bwd_src(const pg_csr* gt, const void* z, int64_t ldz, const void* grad, int64_t ldg, int32_t H, int32_t D,
+                   int dtype, const float* el, const float* er, const float* m, const float* s, const float* dv,
+                   const float* der, const float* attn_l, const float* attn_r, const uint8_t* keep, int32_t num_in,
+                   void* dz, int64_t lddz, float* del, float* scratch, void* stream);
+/* out[k * D + c] = sum_r coef[r, k] x[r, k * D + c] (coef fp32 [n_rows, H], NULL: 1) in a fixed order: the gradients
+ * of attn_l / attn_r (coef = del / der) and column sums (H = 1).  partial: fp32 scratch of
+ * pg_gat_colsum_blocks(n_rows) * H * D floats */
+int pg_gat_colsum_blocks(int32_t n_rows);
+int pg_gat_colsum(const void* x, int64_t ldx, int32_t n_rows, int32_t H, int32_t D, int dtype, const float* coef,
+                  float* out, float* partial, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Symmetric heap: device memory that peers map through CUDA IPC (host pointers out).
  * ---------------------------------------------------------------------------------------- */
 #define PG_IPC_HANDLE_BYTES 64

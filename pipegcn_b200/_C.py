@@ -91,6 +91,16 @@ def _load():
                                        C.POINTER(pg_bns), vp]),
         "pg_boundary_add_bns": (C.c_int, [vp, i64, vp, i64, i32, C.c_int, vp, vp, vp, i32, vp, C.POINTER(pg_bns), vp]),
         "pg_bns_mask_rows": (C.c_int, [vp, i64, vp, i64, i32, i32, C.c_int, vp, vp]),
+        "pg_gat_preload": (C.c_int, []),
+        "pg_gat_scores": (C.c_int, [vp, i64, i32, i32, i32, i32, C.c_int, vp, vp, vp, vp, vp]),
+        "pg_gat_aggregate": (C.c_int, [C.POINTER(pg_csr), vp, i64, i32, i32, C.c_int, vp, vp, vp, vp, i32, vp, i64,
+                                       vp, vp, vp, vp]),
+        "pg_gat_bwd_dst": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, i32, i32, C.c_int, vp, vp, vp, vp, vp, i32,
+                                     vp, vp, vp, vp]),
+        "pg_gat_bwd_src": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, i32, i32, C.c_int, vp, vp, vp, vp, vp, vp,
+                                     vp, vp, vp, i32, vp, i64, vp, vp, vp]),
+        "pg_gat_colsum_blocks": (C.c_int, [i32]),
+        "pg_gat_colsum": (C.c_int, [vp, i64, i32, i32, i32, C.c_int, vp, vp, vp, vp]),
         "pg_heap_alloc": (C.c_int, [C.c_size_t, C.POINTER(vp)]),
         "pg_heap_free": (C.c_int, [vp]),
         "pg_ipc_export": (C.c_int, [vp, C.c_char_p]),

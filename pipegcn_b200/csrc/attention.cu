@@ -1,0 +1,683 @@
+// Graph attention (GAT, DGL GATConv semantics) on sm_90a: attention scores, the edge-softmax aggregate and its two
+// backward passes, and the fixed-order column reductions of the attention-vector gradients.
+//
+// One warp owns one (row, head) pair: lane l holds the columns l, l + 32, ... of the head's D columns, so every
+// per-head dot product is one warp butterfly (all lanes end with the same bits: IEEE addition commutes).  Edges are
+// taken 32 at a time: lane i scores edge i, the batch's maximum / sum are warp reductions, and the gathered rows are
+// then accumulated edge by edge in CSR order.  The rows are walked through the chunk table of the pg_csr plan (the
+// chunked aggregate's): long rows come as segments that write fp32 partials to `scratch`, and a fix-up merges each
+// long row's partials in segment order.  No atomics, no per-edge storage: every result is the same bits run to run.
+#include <algorithm>
+#include <math.h>
+#include <mutex>
+
+#include "common.cuh"
+
+namespace pg {
+namespace {
+
+constexpr int kGatWarps = 4;              // warps per CTA
+constexpr float kNegSlope = 0.2f;         // LeakyReLU negative slope of GATConv
+constexpr int32_t kColMask = 0x7fffffff;  // pidx bit 31 is the "hot row" hint
+
+__device__ __forceinline__ float warp_sum(float x) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) x += __shfl_xor_sync(0xffffffffu, x, o);
+  return x;
+}
+__device__ __forceinline__ float warp_max(float x) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, o));
+  return x;
+}
+
+__device__ __forceinline__ float ldf(const float* p) { return __ldg(p); }
+__device__ __forceinline__ float ldf(const __nv_bfloat16* p) { return __bfloat162float(__ldg(p)); }
+template <typename T> __device__ __forceinline__ T from_f(float x);
+template <> __device__ __forceinline__ float from_f<float>(float x) { return x; }
+template <> __device__ __forceinline__ __nv_bfloat16 from_f<__nv_bfloat16>(float x) { return __float2bfloat16_rn(x); }
+
+__device__ __forceinline__ bool is_kept(const uint8_t* keep, int32_t num_in, int32_t u) {
+  return keep == nullptr || u < num_in || keep[u - num_in] != 0;
+}
+
+// the plan's chunk table (include/pipegcn_b200.h: pg_csr::chunks)
+struct Walk {
+  const int4* chunks;
+  int32_t n_chunks;
+  const int32_t* pidx;
+  const int32_t* prow;
+  const int32_t* long_row;
+  const int32_t* long_seg_ptr;
+  const int32_t* seg_long;
+  int32_t n_long;
+};
+
+Walk make_walk(const pg_csr* g) {
+  return Walk{reinterpret_cast<const int4*>(g->chunks), g->n_chunks, g->pidx, g->prow, g->long_row, g->long_seg_ptr,
+              g->seg_long, g->n_long};
+}
+
+// Calls f(row, first entry, entries, slot) for every row (slot -1) or long-row segment (slot = its scratch slot) of
+// chunk c.
+template <typename F>
+__device__ __forceinline__ void walk_chunk(const Walk& w, int c, F&& f) {
+  const int4 ch = w.chunks[c];
+  const int kind = ch.w & 3, nr = ch.w >> 2;
+  if (kind == 2) {
+    f(w.long_row[w.seg_long[ch.z]], ch.x, ch.y, ch.z);
+  } else if (kind == 1) {
+    f(w.prow[ch.z], ch.x, ch.y, -1);
+  } else {
+    for (int j = 0; j < nr; ++j) f(w.prow[ch.z + j], ch.x + j * ch.y, ch.y, -1);
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------- scores
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32)
+gat_scores_kernel(const T* __restrict__ z, int64_t ldz, int32_t n_rows, int32_t n_er, int32_t H, int32_t D,
+                  const float* __restrict__ attn_l, const float* __restrict__ attn_r, float* __restrict__ el,
+                  float* __restrict__ er) {
+  const int lane = threadIdx.x & 31;
+  const int r = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (r >= n_rows) return;
+  const T* zr = z + static_cast<int64_t>(r) * ldz + static_cast<int64_t>(k) * D;
+  const bool want_r = r < n_er;
+  float sl = 0.f, sr = 0.f;
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int col = lane + 32 * j;
+    if (col < D) {
+      const float x = ldf(zr + col);
+      sl = fmaf(x, attn_l[k * D + col], sl);
+      if (want_r) sr = fmaf(x, attn_r[k * D + col], sr);
+    }
+  }
+  sl = warp_sum(sl);
+  if (want_r) sr = warp_sum(sr);
+  if (lane == 0) {
+    el[static_cast<int64_t>(r) * H + k] = sl;
+    if (want_r) er[static_cast<int64_t>(r) * H + k] = sr;
+  }
+}
+
+// ---------------------------------------------------------------------------------------------------- forward
+struct FwdArgs {
+  Walk w;
+  const void* z; int64_t ldz;
+  const float* el; const float* er; const float* bias;
+  const uint8_t* keep; int32_t num_in;
+  void* out; int64_t ldo;
+  float* m; float* s;
+  float* scratch;          // [n_seg][H][D + 2] = (m, s, acc[D]) of every long-row segment
+  int32_t H, D;
+};
+
+template <typename T, int NJ>
+__device__ __forceinline__ void fwd_store(const FwdArgs& a, int v, int k, int lane, float m, float s,
+                                          const float (&acc)[NJ]) {
+  T* o = static_cast<T*>(a.out) + static_cast<int64_t>(v) * a.ldo + static_cast<int64_t>(k) * a.D;
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int col = lane + 32 * j;
+    if (col < a.D) {
+      const float b = a.bias != nullptr ? a.bias[k * a.D + col] : 0.f;
+      o[col] = from_f<T>((s > 0.f ? __fdiv_rn(acc[j], s) : 0.f) + b);
+    }
+  }
+  if (lane == 0) {
+    a.m[static_cast<int64_t>(v) * a.H + k] = m;
+    a.s[static_cast<int64_t>(v) * a.H + k] = s;
+  }
+}
+
+// online softmax of one row (or segment) for head k: running max m, running sum s, rescaled accumulator
+template <typename T, int NJ>
+__device__ __forceinline__ void fwd_row(const FwdArgs& a, const Walk& w, int v, int e0, int n, int slot, int k,
+                                        int lane) {
+  const T* z = static_cast<const T*>(a.z);
+  const int H = a.H, D = a.D;
+  const float erv = a.er[static_cast<int64_t>(v) * H + k];
+  float m = -INFINITY, s = 0.f, acc[NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) acc[j] = 0.f;
+  for (int b = 0; b < n; b += 32) {
+    const int i = b + lane;
+    int u = 0;
+    float e = -INFINITY;
+    if (i < n) {
+      u = w.pidx[e0 + i] & kColMask;
+      if (is_kept(a.keep, a.num_in, u)) {
+        const float x = a.el[static_cast<int64_t>(u) * H + k] + erv;
+        e = x > 0.f ? x : x * kNegSlope;
+      }
+    }
+    const float bm = warp_max(e);
+    if (bm == -INFINITY) continue;           // no kept source in this batch
+    const float mn = fmaxf(m, bm);
+    const float sc = expf(m - mn);
+    const float p = e == -INFINITY ? 0.f : expf(e - mn);
+    s = fmaf(s, sc, warp_sum(p));
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) acc[j] *= sc;
+    const int cnt = min(32, n - b);
+    for (int t = 0; t < cnt; ++t) {
+      const float pt = __shfl_sync(0xffffffffu, p, t);
+      const int ut = __shfl_sync(0xffffffffu, u, t);
+      if (pt == 0.f) continue;               // warp-uniform: unkept sources are never read
+      const T* zr = z + static_cast<int64_t>(ut) * a.ldz + static_cast<int64_t>(k) * D;
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) {
+        const int col = lane + 32 * j;
+        if (col < D) acc[j] = fmaf(pt, ldf(zr + col), acc[j]);
+      }
+    }
+    m = mn;
+  }
+  if (slot < 0) {
+    fwd_store<T, NJ>(a, v, k, lane, m, s, acc);
+  } else {
+    float* p = a.scratch + (static_cast<int64_t>(slot) * H + k) * (D + 2);
+    if (lane == 0) { p[0] = m; p[1] = s; }
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int col = lane + 32 * j;
+      if (col < D) p[2 + col] = acc[j];
+    }
+  }
+}
+
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32) gat_fwd_kernel(FwdArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int c = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (c >= a.w.n_chunks) return;
+  walk_chunk(a.w, c, [&](int v, int e0, int n, int slot) { fwd_row<T, NJ>(a, a.w, v, e0, n, slot, k, lane); });
+}
+
+// merge the (m, s, acc) partials of every long row in segment order
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32) gat_fwd_fixup_kernel(FwdArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int li = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (li >= a.w.n_long) return;
+  const int H = a.H, D = a.D;
+  float m = -INFINITY, s = 0.f, acc[NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) acc[j] = 0.f;
+  for (int sg = a.w.long_seg_ptr[li]; sg < a.w.long_seg_ptr[li + 1]; ++sg) {
+    const float* p = a.scratch + (static_cast<int64_t>(sg) * H + k) * (D + 2);
+    const float mi = p[0];
+    if (mi == -INFINITY) continue;
+    const float mn = fmaxf(m, mi);
+    const float ca = expf(m - mn), cb = expf(mi - mn);
+    s = fmaf(s, ca, p[1] * cb);
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int col = lane + 32 * j;
+      if (col < D) acc[j] = fmaf(acc[j], ca, p[2 + col] * cb);
+    }
+    m = mn;
+  }
+  fwd_store<T, NJ>(a, a.w.long_row[li], k, lane, m, s, acc);
+}
+
+// ---------------------------------------------------------------------------------------------------- backward
+struct BwdArgs {
+  Walk w;
+  const void* z; int64_t ldz;
+  const void* g; int64_t ldg;
+  const float* el; const float* er; const float* m; const float* s;
+  const float* dv;                        // source pass: D[v, k] = <g[v, k], out[v, k] - bias[k]>
+  const float* der;                       // source pass: der of the inner rows
+  const float* attn_l; const float* attn_r;
+  const uint8_t* keep; int32_t num_in;
+  float* der_out; float* dv_out;          // destination pass
+  void* dz; int64_t lddz; float* del_out; // source pass
+  float* scratch;
+  int32_t H, D;
+};
+
+// softmax weight and LeakyReLU slope of edge u -> v for head k (0 for an unkept source or an empty softmax)
+__device__ __forceinline__ void edge_weight(const BwdArgs& a, int u, int v, int k, float& w, float& slope) {
+  const int64_t vk = static_cast<int64_t>(v) * a.H + k;
+  const float x = a.el[static_cast<int64_t>(u) * a.H + k] + a.er[vk];
+  const float e = x > 0.f ? x : x * kNegSlope;
+  const float s = a.s[vk];
+  w = s > 0.f ? __fdiv_rn(expf(e - a.m[vk]), s) : 0.f;
+  slope = x > 0.f ? 1.f : kNegSlope;
+}
+
+// der[v, k] = sum_u a_uv (<g_v, z_u> - D_v) LeakyReLU'(x_uv) over the forward CSR row v, with
+// D_v = <g_v, out_v - bias> = sum_u a_uv <g_v, z_u> taken from the same products as the first term (not from the stored
+// output: with bf16 storage its rounding would not cancel), in one pass: der = A - D_v B with A = sum a dot slope and
+// B = sum a slope.  A segment of a long row writes its partial (A, B, D) to scratch.
+template <typename T, int NJ>
+__device__ __forceinline__ void dst_row(const BwdArgs& a, const Walk& w, int v, int e0, int n, int slot, int k,
+                                        int lane) {
+  const T* z = static_cast<const T*>(a.z);
+  const int D = a.D;
+  const T* gv = static_cast<const T*>(a.g) + static_cast<int64_t>(v) * a.ldg + static_cast<int64_t>(k) * D;
+  float gr[NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int col = lane + 32 * j;
+    gr[j] = col < D ? ldf(gv + col) : 0.f;
+  }
+  float sa = 0.f, sb = 0.f, sd = 0.f;
+  for (int b = 0; b < n; b += 32) {
+    const int i = b + lane;
+    int u = 0;
+    float wt = 0.f, sl = 0.f;
+    if (i < n) {
+      u = w.pidx[e0 + i] & kColMask;
+      if (is_kept(a.keep, a.num_in, u)) edge_weight(a, u, v, k, wt, sl);
+    }
+    const int cnt = min(32, n - b);
+    for (int t = 0; t < cnt; ++t) {
+      const float at = __shfl_sync(0xffffffffu, wt, t);
+      const int ut = __shfl_sync(0xffffffffu, u, t);
+      const float st = __shfl_sync(0xffffffffu, sl, t);
+      if (at == 0.f) continue;
+      const T* zr = z + static_cast<int64_t>(ut) * a.ldz + static_cast<int64_t>(k) * D;
+      float dp = 0.f;
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) {
+        const int col = lane + 32 * j;
+        if (col < D) dp = fmaf(gr[j], ldf(zr + col), dp);
+      }
+      const float ad = at * warp_sum(dp);
+      sd += ad;
+      sa = fmaf(ad, st, sa);
+      sb = fmaf(at, st, sb);
+    }
+  }
+  if (lane == 0) {
+    const int64_t vk = static_cast<int64_t>(v) * a.H + k;
+    if (slot < 0) {
+      a.der_out[vk] = fmaf(-sd, sb, sa);
+      a.dv_out[vk] = sd;
+    } else {
+      float* p = a.scratch + (static_cast<int64_t>(slot) * a.H + k) * 3;
+      p[0] = sa; p[1] = sb; p[2] = sd;
+    }
+  }
+}
+
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32) gat_bwd_dst_kernel(BwdArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int c = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (c >= a.w.n_chunks) return;
+  walk_chunk(a.w, c, [&](int v, int e0, int n, int slot) { dst_row<T, NJ>(a, a.w, v, e0, n, slot, k, lane); });
+}
+
+__global__ void gat_bwd_dst_fixup_kernel(BwdArgs a) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= a.w.n_long * a.H) return;
+  const int li = i / a.H, k = i % a.H;
+  float sa = 0.f, sb = 0.f, sd = 0.f;
+  for (int sg = a.w.long_seg_ptr[li]; sg < a.w.long_seg_ptr[li + 1]; ++sg) {
+    const float* p = a.scratch + (static_cast<int64_t>(sg) * a.H + k) * 3;
+    sa += p[0]; sb += p[1]; sd += p[2];
+  }
+  const int64_t vk = static_cast<int64_t>(a.w.long_row[li]) * a.H + k;
+  a.der_out[vk] = fmaf(-sd, sb, sa);
+  a.dv_out[vk] = sd;
+}
+
+template <typename T, int NJ>
+__device__ __forceinline__ void src_store(const BwdArgs& a, int u, int k, int lane, float del, const float (&acc)[NJ]) {
+  const int D = a.D;
+  const float der = u < a.num_in ? a.der[static_cast<int64_t>(u) * a.H + k] : 0.f;
+  T* o = static_cast<T*>(a.dz) + static_cast<int64_t>(u) * a.lddz + static_cast<int64_t>(k) * D;
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int col = lane + 32 * j;
+    if (col < D) o[col] = from_f<T>(fmaf(der, a.attn_r[k * D + col], fmaf(del, a.attn_l[k * D + col], acc[j])));
+  }
+  if (lane == 0) a.del_out[static_cast<int64_t>(u) * a.H + k] = del;
+}
+
+// dz[u, k] = sum_v a_uv g_v (+ del attn_l + der attn_r), del[u, k] = sum_v a_uv (<g_v, z_u> - D_v) LeakyReLU'(x_uv)
+// over the CSC row u (the destinations v of source u)
+template <typename T, int NJ>
+__device__ __forceinline__ void src_row(const BwdArgs& a, const Walk& w, int u, int e0, int n, int slot, int k,
+                                        int lane) {
+  const int D = a.D;
+  float zr[NJ], acc[NJ], del = 0.f;
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) { zr[j] = 0.f; acc[j] = 0.f; }
+  if (is_kept(a.keep, a.num_in, u)) {
+    const T* zu = static_cast<const T*>(a.z) + static_cast<int64_t>(u) * a.ldz + static_cast<int64_t>(k) * D;
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int col = lane + 32 * j;
+      if (col < D) zr[j] = ldf(zu + col);
+    }
+    for (int b = 0; b < n; b += 32) {
+      const int i = b + lane;
+      int v = 0;
+      float wt = 0.f, sl = 0.f, dv = 0.f;
+      if (i < n) {
+        v = w.pidx[e0 + i] & kColMask;
+        edge_weight(a, u, v, k, wt, sl);
+        dv = a.dv[static_cast<int64_t>(v) * a.H + k];
+      }
+      const int cnt = min(32, n - b);
+      for (int t = 0; t < cnt; ++t) {
+        const float at = __shfl_sync(0xffffffffu, wt, t);
+        const int vt = __shfl_sync(0xffffffffu, v, t);
+        const float st = __shfl_sync(0xffffffffu, sl, t);
+        const float dt = __shfl_sync(0xffffffffu, dv, t);
+        if (at == 0.f) continue;
+        const T* gv = static_cast<const T*>(a.g) + static_cast<int64_t>(vt) * a.ldg + static_cast<int64_t>(k) * D;
+        float dp = 0.f;
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+          const int col = lane + 32 * j;
+          if (col < D) {
+            const float gj = ldf(gv + col);
+            dp = fmaf(gj, zr[j], dp);
+            acc[j] = fmaf(at, gj, acc[j]);
+          }
+        }
+        del = fmaf(at * (warp_sum(dp) - dt), st, del);
+      }
+    }
+  }
+  if (slot < 0) {
+    src_store<T, NJ>(a, u, k, lane, del, acc);
+  } else {
+    float* p = a.scratch + (static_cast<int64_t>(slot) * a.H + k) * (D + 1);
+    if (lane == 0) p[0] = del;
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int col = lane + 32 * j;
+      if (col < D) p[1 + col] = acc[j];
+    }
+  }
+}
+
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32) gat_bwd_src_kernel(BwdArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int c = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (c >= a.w.n_chunks) return;
+  walk_chunk(a.w, c, [&](int u, int e0, int n, int slot) { src_row<T, NJ>(a, a.w, u, e0, n, slot, k, lane); });
+}
+
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32) gat_bwd_src_fixup_kernel(BwdArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int li = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (li >= a.w.n_long) return;
+  const int D = a.D;
+  float del = 0.f, acc[NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) acc[j] = 0.f;
+  for (int sg = a.w.long_seg_ptr[li]; sg < a.w.long_seg_ptr[li + 1]; ++sg) {
+    const float* p = a.scratch + (static_cast<int64_t>(sg) * a.H + k) * (D + 1);
+    del += p[0];
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int col = lane + 32 * j;
+      if (col < D) acc[j] += p[1 + col];
+    }
+  }
+  src_store<T, NJ>(a, a.w.long_row[li], k, lane, del, acc);
+}
+
+// ---------------------------------------------------------------------------------------------------- column sums
+// stage 1: CTA b sums rows [b * R, (b + 1) * R) of 32 columns, 8 row lanes, merged in row-lane order
+template <typename T>
+__global__ void __launch_bounds__(256) gat_colsum_kernel(const T* __restrict__ x, int64_t ldx, int32_t n_rows,
+                                                         int32_t H, int32_t D, const float* __restrict__ coef,
+                                                         int32_t rows_per, float* __restrict__ partial) {
+  __shared__ float red[8][33];
+  const int n_cols = H * D;
+  const int col = blockIdx.y * 32 + threadIdx.x;
+  const int r0 = blockIdx.x * rows_per, r1 = min(n_rows, r0 + rows_per);
+  float acc = 0.f;
+  if (col < n_cols) {
+    const int k = col / D;
+    for (int r = r0 + threadIdx.y; r < r1; r += 8) {
+      const float v = ldf(x + static_cast<int64_t>(r) * ldx + col);
+      acc = coef != nullptr ? fmaf(coef[static_cast<int64_t>(r) * H + k], v, acc) : acc + v;
+    }
+  }
+  red[threadIdx.y][threadIdx.x] = acc;
+  __syncthreads();
+  if (threadIdx.y == 0 && col < n_cols) {
+    float s = red[0][threadIdx.x];
+#pragma unroll
+    for (int i = 1; i < 8; ++i) s += red[i][threadIdx.x];
+    partial[static_cast<int64_t>(blockIdx.x) * n_cols + col] = s;
+  }
+}
+
+__global__ void gat_colsum_final_kernel(const float* __restrict__ partial, int32_t n_blocks, int32_t n_cols,
+                                        float* __restrict__ out) {
+  const int col = blockIdx.x * blockDim.x + threadIdx.x;
+  if (col >= n_cols) return;
+  float s = 0.f;
+  for (int b = 0; b < n_blocks; ++b) s += partial[static_cast<int64_t>(b) * n_cols + col];
+  out[col] = s;
+}
+
+int colsum_blocks(int32_t n_rows) {
+  return static_cast<int>(std::max<int64_t>(1, std::min<int64_t>((n_rows + 255) / 256, 2 * sm_count())));
+}
+
+// ---------------------------------------------------------------------------------------------------- dispatch
+int nj_of(int32_t D) { return D <= 32 ? 1 : D <= 64 ? 2 : D <= 128 ? 4 : D <= 256 ? 8 : D <= 512 ? 16 : 0; }
+
+#define PG_GAT_NJ(T, KERNEL, GRID, ST, ...)                                              \
+  switch (nj) {                                                                          \
+    case 1: KERNEL<T, 1><<<GRID, kGatWarps * 32, 0, ST>>>(__VA_ARGS__); break;           \
+    case 2: KERNEL<T, 2><<<GRID, kGatWarps * 32, 0, ST>>>(__VA_ARGS__); break;           \
+    case 4: KERNEL<T, 4><<<GRID, kGatWarps * 32, 0, ST>>>(__VA_ARGS__); break;           \
+    case 8: KERNEL<T, 8><<<GRID, kGatWarps * 32, 0, ST>>>(__VA_ARGS__); break;           \
+    default: KERNEL<T, 16><<<GRID, kGatWarps * 32, 0, ST>>>(__VA_ARGS__); break;         \
+  }
+
+template <typename T, int NJ>
+void preload_t() {
+  cudaFuncAttributes a;
+  cudaFuncGetAttributes(&a, gat_scores_kernel<T, NJ>);
+  cudaFuncGetAttributes(&a, gat_fwd_kernel<T, NJ>);
+  cudaFuncGetAttributes(&a, gat_fwd_fixup_kernel<T, NJ>);
+  cudaFuncGetAttributes(&a, gat_bwd_dst_kernel<T, NJ>);
+  cudaFuncGetAttributes(&a, gat_bwd_src_kernel<T, NJ>);
+  cudaFuncGetAttributes(&a, gat_bwd_src_fixup_kernel<T, NJ>);
+}
+template <typename T>
+void preload_all() {
+  preload_t<T, 1>(); preload_t<T, 2>(); preload_t<T, 4>(); preload_t<T, 8>(); preload_t<T, 16>();
+  cudaFuncAttributes a;
+  cudaFuncGetAttributes(&a, gat_colsum_kernel<T>);
+}
+
+int check_plan(const pg_csr* g, const char* who) {
+  PG_REQUIRE(g != nullptr, "%s: null plan", who);
+  PG_REQUIRE(g->n_rows == 0 || (g->chunks != nullptr && g->pidx != nullptr && g->prow != nullptr),
+             "%s: the plan has no chunk table (build it with sorted rows and chunks enabled)", who);
+  PG_REQUIRE(g->n_seg == 0 || (g->long_row && g->long_seg_ptr && g->seg_long), "%s: the plan has no long-row split", who);
+  return PG_OK;
+}
+
+}  // namespace
+
+// CUDA loads kernels lazily, and loading one may wait for the device: see exchange.cu's bns_preload.
+static void gat_preload() {
+  static std::once_flag once;
+  std::call_once(once, [] {
+    preload_all<float>();
+    preload_all<__nv_bfloat16>();
+    cudaFuncAttributes a;
+    cudaFuncGetAttributes(&a, gat_bwd_dst_fixup_kernel);
+    cudaFuncGetAttributes(&a, gat_colsum_final_kernel);
+    cudaGetLastError();
+  });
+}
+
+}  // namespace pg
+
+using pg::kGatWarps;
+
+extern "C" int pg_gat_preload(void) {
+  pg::gat_preload();
+  return PG_OK;
+}
+
+extern "C" int pg_gat_scores(const void* z, int64_t ldz, int32_t n_rows, int32_t n_er, int32_t H, int32_t D,
+                             int dtype, const float* attn_l, const float* attn_r, float* el, float* er, void* stream) {
+  pg::gat_preload();
+  PG_REQUIRE(n_rows >= 0 && n_er >= 0 && n_er <= n_rows && H > 0 && D > 0 && ldz >= static_cast<int64_t>(H) * D,
+             "pg_gat_scores: bad sizes");
+  const int nj = pg::nj_of(D);
+  PG_REQUIRE(nj > 0, "pg_gat_scores: head width %d > 512", D);
+  if (n_rows == 0) return PG_OK;
+  PG_REQUIRE(z && attn_l && el && (n_er == 0 || (attn_r && er)), "pg_gat_scores: null argument");
+  const dim3 grid((n_rows + kGatWarps - 1) / kGatWarps, H);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (dtype == PG_F32) {
+    PG_GAT_NJ(float, pg::gat_scores_kernel, grid, st, static_cast<const float*>(z), ldz, n_rows,
+                                                                         n_er, H, D, attn_l, attn_r, el, er);
+  } else if (dtype == PG_BF16) {
+    PG_GAT_NJ(__nv_bfloat16, pg::gat_scores_kernel, grid, st,
+        static_cast<const __nv_bfloat16*>(z), ldz, n_rows, n_er, H, D, attn_l, attn_r, el, er);
+  } else {
+    pg::set_error("pg_gat_scores: unknown dtype %d", dtype);
+    return PG_ERR_INVALID;
+  }
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+extern "C" int pg_gat_aggregate(const pg_csr* g, const void* z, int64_t ldz, int32_t H, int32_t D, int dtype,
+                                const float* el, const float* er, const float* bias, const uint8_t* keep,
+                                int32_t num_in, void* out, int64_t ldo, float* m, float* s, float* scratch,
+                                void* stream) {
+  pg::gat_preload();
+  if (int rc = pg::check_plan(g, "pg_gat_aggregate")) return rc;
+  const int nj = pg::nj_of(D);
+  PG_REQUIRE(H > 0 && nj > 0 && ldz >= static_cast<int64_t>(H) * D && ldo >= static_cast<int64_t>(H) * D,
+             "pg_gat_aggregate: bad sizes (H %d, D %d)", H, D);
+  if (g->n_rows == 0) return PG_OK;
+  PG_REQUIRE(z && el && er && out && m && s && (g->n_seg == 0 || scratch), "pg_gat_aggregate: null argument");
+  pg::FwdArgs a{pg::make_walk(g), z, ldz, el, er, bias, keep, num_in, out, ldo, m, s, scratch, H, D};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const dim3 grid((g->n_chunks + kGatWarps - 1) / kGatWarps, H), grid_fix((g->n_long + kGatWarps - 1) / kGatWarps, H);
+  if (dtype == PG_F32) {
+    if (g->n_chunks) PG_GAT_NJ(float, pg::gat_fwd_kernel, grid, st, a);
+    if (g->n_long) PG_GAT_NJ(float, pg::gat_fwd_fixup_kernel, grid_fix, st, a);
+  } else if (dtype == PG_BF16) {
+    if (g->n_chunks) PG_GAT_NJ(__nv_bfloat16, pg::gat_fwd_kernel, grid, st, a);
+    if (g->n_long) PG_GAT_NJ(__nv_bfloat16, pg::gat_fwd_fixup_kernel, grid_fix, st, a);
+  } else {
+    pg::set_error("pg_gat_aggregate: unknown dtype %d", dtype);
+    return PG_ERR_INVALID;
+  }
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+extern "C" int pg_gat_bwd_dst(const pg_csr* g, const void* z, int64_t ldz, const void* grad, int64_t ldg, int32_t H,
+                              int32_t D, int dtype, const float* el, const float* er, const float* m, const float* s,
+                              const uint8_t* keep, int32_t num_in, float* der, float* dv, float* scratch,
+                              void* stream) {
+  pg::gat_preload();
+  if (int rc = pg::check_plan(g, "pg_gat_bwd_dst")) return rc;
+  const int nj = pg::nj_of(D);
+  const int64_t hd = static_cast<int64_t>(H) * D;
+  PG_REQUIRE(H > 0 && nj > 0 && ldz >= hd && ldg >= hd, "pg_gat_bwd_dst: bad sizes (H %d, D %d)", H, D);
+  if (g->n_rows == 0) return PG_OK;
+  PG_REQUIRE(z && grad && el && er && m && s && der && dv && (g->n_seg == 0 || scratch),
+             "pg_gat_bwd_dst: null argument");
+  pg::BwdArgs a{pg::make_walk(g), z, ldz, grad, ldg, el, er, m, s, nullptr, nullptr, nullptr, nullptr,
+                keep, num_in, der, dv, nullptr, 0, nullptr, scratch, H, D};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const dim3 grid((g->n_chunks + kGatWarps - 1) / kGatWarps, H);
+  if (dtype == PG_F32) {
+    if (g->n_chunks) PG_GAT_NJ(float, pg::gat_bwd_dst_kernel, grid, st, a);
+  } else if (dtype == PG_BF16) {
+    if (g->n_chunks) PG_GAT_NJ(__nv_bfloat16, pg::gat_bwd_dst_kernel, grid, st, a);
+  } else {
+    pg::set_error("pg_gat_bwd_dst: unknown dtype %d", dtype);
+    return PG_ERR_INVALID;
+  }
+  if (g->n_long) {
+    const int n = g->n_long * H;
+    pg::gat_bwd_dst_fixup_kernel<<<(n + 255) / 256, 256, 0, st>>>(a);
+  }
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+extern "C" int pg_gat_bwd_src(const pg_csr* gt, const void* z, int64_t ldz, const void* grad, int64_t ldg, int32_t H,
+                              int32_t D, int dtype, const float* el, const float* er, const float* m, const float* s,
+                              const float* dv, const float* der, const float* attn_l, const float* attn_r,
+                              const uint8_t* keep, int32_t num_in, void* dz, int64_t lddz, float* del,
+                              float* scratch, void* stream) {
+  pg::gat_preload();
+  if (int rc = pg::check_plan(gt, "pg_gat_bwd_src")) return rc;
+  const int nj = pg::nj_of(D);
+  const int64_t hd = static_cast<int64_t>(H) * D;
+  PG_REQUIRE(H > 0 && nj > 0 && ldz >= hd && ldg >= hd && lddz >= hd && num_in >= 0,
+             "pg_gat_bwd_src: bad sizes (H %d, D %d)", H, D);
+  if (gt->n_rows == 0) return PG_OK;
+  PG_REQUIRE(z && grad && el && er && m && s && dv && (num_in == 0 || der) && attn_l && attn_r && dz && del &&
+                 (gt->n_seg == 0 || scratch),
+             "pg_gat_bwd_src: null argument");
+  pg::BwdArgs a{pg::make_walk(gt), z, ldz, grad, ldg, el, er, m, s, dv, der, attn_l, attn_r,
+                keep, num_in, nullptr, nullptr, dz, lddz, del, scratch, H, D};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const dim3 grid((gt->n_chunks + kGatWarps - 1) / kGatWarps, H), grid_fix((gt->n_long + kGatWarps - 1) / kGatWarps, H);
+  if (dtype == PG_F32) {
+    if (gt->n_chunks) PG_GAT_NJ(float, pg::gat_bwd_src_kernel, grid, st, a);
+    if (gt->n_long) PG_GAT_NJ(float, pg::gat_bwd_src_fixup_kernel, grid_fix, st, a);
+  } else if (dtype == PG_BF16) {
+    if (gt->n_chunks) PG_GAT_NJ(__nv_bfloat16, pg::gat_bwd_src_kernel, grid, st, a);
+    if (gt->n_long) PG_GAT_NJ(__nv_bfloat16, pg::gat_bwd_src_fixup_kernel, grid_fix, st, a);
+  } else {
+    pg::set_error("pg_gat_bwd_src: unknown dtype %d", dtype);
+    return PG_ERR_INVALID;
+  }
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+extern "C" int pg_gat_colsum_blocks(int32_t n_rows) { return pg::colsum_blocks(n_rows); }
+
+extern "C" int pg_gat_colsum(const void* x, int64_t ldx, int32_t n_rows, int32_t H, int32_t D, int dtype,
+                             const float* coef, float* out, float* partial, void* stream) {
+  pg::gat_preload();
+  const int n_cols = H * D;
+  PG_REQUIRE(n_rows >= 0 && H > 0 && D > 0 && ldx >= n_cols && out && partial, "pg_gat_colsum: bad arguments");
+  PG_REQUIRE(n_rows == 0 || x, "pg_gat_colsum: null input");
+  const int nb = pg::colsum_blocks(n_rows);
+  const int rows_per = static_cast<int>((static_cast<int64_t>(n_rows) + nb - 1) / nb);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const dim3 grid(nb, (n_cols + 31) / 32), block(32, 8);
+  if (dtype == PG_F32) {
+    pg::gat_colsum_kernel<float><<<grid, block, 0, st>>>(static_cast<const float*>(x), ldx, n_rows, H, D, coef,
+                                                         rows_per, partial);
+  } else if (dtype == PG_BF16) {
+    pg::gat_colsum_kernel<__nv_bfloat16><<<grid, block, 0, st>>>(static_cast<const __nv_bfloat16*>(x), ldx, n_rows,
+                                                                 H, D, coef, rows_per, partial);
+  } else {
+    pg::set_error("pg_gat_colsum: unknown dtype %d", dtype);
+    return PG_ERR_INVALID;
+  }
+  pg::gat_colsum_final_kernel<<<(n_cols + 255) / 256, 256, 0, st>>>(partial, nb, n_cols, out);
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}

@@ -389,6 +389,12 @@ class Buffer(_Exchange):
         bns_sample(self._bns_spec(), self._world.rank, plan, self._num_in, self._num_all, self._bns_mask, self._bns_deg)
         return self._bns_deg
 
+    @property
+    def keep_mask(self):
+        """uint8 [num_all - N_in] device tensor: this epoch's keep mask of the halo rows (1 = kept), rewritten in place by
+        `sample` (the same tensor every epoch, so captured kernels may read it); None without sampling."""
+        return self._bns_mask if self._bns else None
+
     def sample_mask(self):
         """[num_all - N_in] bool copy of the current keep mask of the halo rows (None without sampling)."""
         if not self._bns:

@@ -16,6 +16,9 @@ with getattr(args, 'eval_partitioned', False)), so the parsed flags stay the ref
 training: every epoch each partition keeps a random fraction p of its halo nodes and drops the rest from its graph for
 that epoch, so the halo exchange moves p times the bytes.  Evaluation always uses the full graph.  Like
 `--eval-partitioned` it has a suppressed default: read it with getattr(args, 'sampling_rate', 1.0).
+
+`--model gat` trains graph attention (DGL's GATConv) instead of GraphSAGE; `--n-heads k` (not in the reference, default
+4, suppressed like `--sampling-rate`: read it with getattr(args, 'n_heads', 4)) sets its heads per hidden layer.
 """
 import argparse
 
@@ -23,7 +26,7 @@ import argparse
 _FLAGS = [
     ("dataset", dict(type=str, default='reddit', help="the input dataset (or synthetic:<shape>)")),
     ("graph-name", dict(type=str, default='')),
-    ("model", dict(type=str, default='graphsage', help="model for training (graphsage | gcn)")),
+    ("model", dict(type=str, default='graphsage', help="model for training (graphsage | gcn | gat)")),
     ("dropout", dict(type=float, default=0.5, help="dropout probability")),
     ("lr", dict(type=float, default=1e-2, help="learning rate")),
     ("n-epochs", dict(type=int, default=200, help="the number of training epochs")),
@@ -67,6 +70,16 @@ def _sampling_rate(text):
     return p
 
 
+def _n_heads(text):
+    try:
+        k = int(text)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"invalid head count '{text}'")
+    if k < 1:
+        raise argparse.ArgumentTypeError(f"--n-heads {text}: expected a positive integer")
+    return k
+
+
 def build_parser():
     parser = argparse.ArgumentParser(description='PipeGCN on H100')
     for flag, kw in _FLAGS:
@@ -86,6 +99,8 @@ def build_parser():
     parser.add_argument('--sampling-rate', '--sampling_rate', type=_sampling_rate, default=argparse.SUPPRESS,
                         help="boundary-node sampling: the fraction of halo nodes every partition keeps per epoch "
                              "(synchronous training; default 1 = all)")
+    parser.add_argument('--n-heads', '--n_heads', type=_n_heads, default=argparse.SUPPRESS,
+                        help="--model gat: attention heads of every hidden layer (default 4)")
     return parser
 
 

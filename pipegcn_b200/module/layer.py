@@ -7,6 +7,14 @@ weights).  `graph` is a `pipegcn_b200.graph.PartGraph` instead of a DGL heterogr
 
     training:  out = feat[:N_in] @ W1^T + b1 + ((A @ feat) / in_deg) @ W2^T + b2      (layer.py:44-51)
     eval:      same on a homogeneous graph, degrees taken from the graph               (layer.py:52-62)
+
+`GATLayer` (not in the reference): DGL's `GATConv` with feat_drop = attn_drop = 0, no residual, negative_slope 0.2,
+over the `[inner | halo]` rows h the halo exchange returns (inner rows v, in-edges u -> v, per head):
+
+    z = h @ W^T,  el = <z, attn_l>,  er = <z, attn_r>,
+    out[v] = sum_u softmax_u(LeakyReLU(el[u] + er[v])) z[u] + bias
+
+State-dict keys are GATConv's: `fc.weight` [H*D, d_in], `attn_l` / `attn_r` [1, H, D], `bias` [H*D].
 """
 import math
 
@@ -57,3 +65,30 @@ class GraphSAGELayer(nn.Module):
             return ops.linear(torch.cat((x, ah), dim=1), self.linear.weight, self.linear.bias)
         return ops.sage_linear(x, ah, self.linear1.weight, self.linear1.bias,
                                self.linear2.weight, self.linear2.bias)
+
+
+class GATLayer(nn.Module):
+
+    def __init__(self, in_feats, out_feats, num_heads):
+        super().__init__()
+        self.in_feats, self.out_feats, self.num_heads = in_feats, out_feats, num_heads
+        self.fc = nn.Linear(in_feats, out_feats * num_heads, bias=False)
+        self.attn_l = nn.Parameter(torch.empty(1, num_heads, out_feats))
+        self.attn_r = nn.Parameter(torch.empty(1, num_heads, out_feats))
+        self.bias = nn.Parameter(torch.empty(num_heads * out_feats))
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        """GATConv.reset_parameters."""
+        gain = nn.init.calculate_gain('relu')
+        nn.init.xavier_normal_(self.fc.weight, gain=gain)
+        nn.init.xavier_normal_(self.attn_l, gain=gain)
+        nn.init.xavier_normal_(self.attn_r, gain=gain)
+        nn.init.constant_(self.bias, 0)
+
+    def forward(self, graph, feat, keep=None, drop_bwd=None):
+        """`feat`: the [num_all, d_in] rows of `graph` (a partition's `[inner | halo]`, or a whole graph); returns the
+        [N_in, H*D] inner rows.  `keep`: uint8 keep mask of the halo rows (boundary-node sampling) or None.
+        `drop_bwd`: `feat` already is dropout(F) under that key; the gradient returned is the one with respect to F."""
+        return ops.gat_layer(feat, graph, keep, self.num_heads, self.fc.weight, self.attn_l, self.attn_r, self.bias,
+                             drop_bwd)

@@ -9,13 +9,19 @@ Extra keyword arguments (not in the reference): `buffer` -- the exchange object 
 instead of the process-global `helper.context.buffer` (several simulated ranks in one
 process); `dtype` -- activation storage type, float32 (reference) or bfloat16 (fp32
 accumulate, fp32 master weights).
+
+`GAT` (not in the reference) is the same layer loop with `GATLayer`s: every graph layer whose output feeds another
+layer concatenates `n_heads` heads of d_out / n_heads columns, a graph layer that produces the logits has one head.  The
+exchange moves the layer input h, so pipelining, the corrections, the static layer-0 store and the fused dropout apply
+unchanged; with boundary-node sampling the layers take the buffer's keep mask of the halo rows (`Buffer.keep_mask`),
+and unkept rows are absent from every softmax.
 """
 import torch
 from torch import nn
 import torch.nn.functional as F
 
 from ..helper import context as ctx
-from .layer import GraphSAGELayer
+from .layer import GATLayer, GraphSAGELayer
 
 
 class GNNBase(nn.Module):
@@ -43,7 +49,7 @@ class GraphSAGE(GNNBase):
         self.act_dtype = dtype
         for i, (d_in, d_out) in enumerate(zip(layer_size[:-1], layer_size[1:])):
             if i < self.n_graph_layers:
-                self.layers.append(GraphSAGELayer(d_in, d_out, use_pp=(use_pp and i == 0)))
+                self.layers.append(self._graph_layer(i, d_in, d_out))
             else:
                 self.layers.append(nn.Linear(d_in, d_out))
             if self.use_norm and i < self.n_layers - 1:
@@ -54,6 +60,13 @@ class GraphSAGE(GNNBase):
                     self.norm.append(SyncBatchNorm(d_out, train_size))
                 else:
                     raise ValueError(f"unknown norm '{norm}'")
+
+    def _graph_layer(self, i, d_in, d_out):
+        return GraphSAGELayer(d_in, d_out, use_pp=(self.use_pp and i == 0))
+
+    def _layer_arg(self, in_deg):
+        """The third argument of every graph layer in training: the in-degrees."""
+        return in_deg
 
     def _drop(self, h):
         from .. import ops
@@ -93,6 +106,7 @@ class GraphSAGE(GNNBase):
         from .. import ops
         h = feat if feat.dtype == self.act_dtype else feat.to(self.act_dtype)
         p = self.dropout.p if self.training else 0.0
+        in_deg = self._layer_arg(in_deg)
         self._fused = None
         for i, layer in enumerate(self.layers):
             if i < self.n_graph_layers:
@@ -151,3 +165,36 @@ class GraphSAGE(GNNBase):
 
 
 GCN = GraphSAGE
+
+
+class GAT(GraphSAGE):
+
+    def __init__(self, layer_size, activation, dropout=0.5, norm='layer', train_size=None, n_linear=0, buffer=None,
+                 dtype=torch.float32, n_heads=4):
+        n_graph = len(layer_size) - 1 - n_linear
+        for i in range(n_graph):
+            if i < len(layer_size) - 2 and layer_size[i + 1] % n_heads:
+                raise ValueError(f"GAT: {layer_size[i + 1]} hidden units do not split into {n_heads} heads")
+        self.n_heads = n_heads
+        super().__init__(layer_size, activation, False, dropout=dropout, norm=norm, train_size=train_size,
+                         n_linear=n_linear, buffer=buffer, dtype=dtype)
+
+    def _graph_layer(self, i, d_in, d_out):
+        if i < self.n_layers - 1:
+            return GATLayer(d_in, d_out // self.n_heads, self.n_heads)
+        return GATLayer(d_in, d_out, 1)                  # the logits: one head of n_class
+
+    def _layer_arg(self, in_deg):
+        """The keep mask of this epoch's boundary-node sample (training with sampling), else None."""
+        buf = self._buffer() if self.training else None
+        return getattr(buf, 'keep_mask', None) if buf is not None else None
+
+    def forward(self, g, feat, in_deg=None):
+        from .. import ops
+        ops.gat_preload()
+        return super().forward(g, feat, in_deg)
+
+    def forward_partitioned(self, g, xch, pp_feat=None, push0=False):
+        from .. import ops
+        ops.gat_preload()
+        return (yield from super().forward_partitioned(g, xch, pp_feat, push0))

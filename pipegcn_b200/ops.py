@@ -553,6 +553,163 @@ def sage_linear(x, ah, w1, b1, w2, b2) -> torch.Tensor:
     return linear(x, w1, b1) + linear(ah, w2, b2)
 
 
+# ---- graph attention (csrc/attention.cu) -------------------------------------------------------------------
+def gat_preload():
+    """Load every attention kernel now: a first launch may wait for the device, so it must not happen while a halo
+    wait of a simulated rank spins."""
+    _C.check(_C.lib.pg_gat_preload(), "pg_gat_preload")
+
+
+def _ptr(t):
+    return t.data_ptr() if t is not None else None
+
+
+def _f32(t: torch.Tensor) -> torch.Tensor:
+    return t.detach().to(torch.float32).reshape(-1).contiguous()
+
+
+def gat_scores(z: torch.Tensor, attn_l: torch.Tensor, attn_r: torch.Tensor, heads: int, n_er: int):
+    """(el [rows, H], er [n_er, H]) fp32: the per-head dot products of z with attn_l (every row) and attn_r (the
+    first n_er rows)."""
+    _rows(z)
+    n, hd = z.shape
+    el = torch.empty(n, heads, dtype=torch.float32, device=z.device)
+    er = torch.empty(n_er, heads, dtype=torch.float32, device=z.device)
+    _C.count()
+    _C.check(_C.lib.pg_gat_scores(z.data_ptr(), z.stride(0), n, int(n_er), heads, hd // heads, _C.dtype_code(z.dtype),
+                                  attn_l.data_ptr(), attn_r.data_ptr(), el.data_ptr(), er.data_ptr(), _C.stream_ptr()),
+             "pg_gat_scores")
+    return el, er
+
+
+def _gat_scratch(plan: CsrPlan, heads: int, d: int):
+    return plan.scratch(heads * (d + 2))
+
+
+def gat_aggregate(graph: PartGraph, z, el, er, bias, heads: int, keep=None):
+    """out [N_in, H*D] = per-head edge softmax of LeakyReLU(el[u] + er[v]) over the forward CSR applied to z, + bias;
+    with the softmax statistics m, s [N_in, H] fp32."""
+    plan = graph.fwd
+    n, hd = plan.n_rows, z.shape[1]
+    d = hd // heads
+    out = alloc_rows(n, hd, z.dtype, z.device)
+    m = torch.empty(n, heads, dtype=torch.float32, device=z.device)
+    s = torch.empty(n, heads, dtype=torch.float32, device=z.device)
+    scratch = _gat_scratch(plan, heads, d)
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_gat_aggregate(C.byref(plan.c), z.data_ptr(), z.stride(0), heads, d, _C.dtype_code(z.dtype),
+                                     el.data_ptr(), er.data_ptr(), _ptr(bias), _ptr(keep), graph.num_in,
+                                     out.data_ptr(), out.stride(0), m.data_ptr(), s.data_ptr(), _ptr(scratch),
+                                     _C.stream_ptr()), "pg_gat_aggregate")
+    return out, m, s
+
+
+def gat_bwd_dst(graph: PartGraph, z, g, el, er, m, s, heads: int, keep=None):
+    """(der, dv) [N_in, H] fp32: the gradient of er, and <g, out - bias> per row and head."""
+    plan = graph.fwd
+    n, hd = plan.n_rows, z.shape[1]
+    d = hd // heads
+    der = torch.empty(n, heads, dtype=torch.float32, device=z.device)
+    dv = torch.empty(n, heads, dtype=torch.float32, device=z.device)
+    scratch = _gat_scratch(plan, heads, d)
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_gat_bwd_dst(C.byref(plan.c), z.data_ptr(), z.stride(0), g.data_ptr(), g.stride(0), heads, d,
+                                   _C.dtype_code(z.dtype), el.data_ptr(), er.data_ptr(), m.data_ptr(), s.data_ptr(),
+                                   _ptr(keep), graph.num_in, der.data_ptr(), dv.data_ptr(), _ptr(scratch),
+                                   _C.stream_ptr()), "pg_gat_bwd_dst")
+    return der, dv
+
+
+def gat_bwd_src(graph: PartGraph, z, g, el, er, m, s, dv, der, attn_l, attn_r, heads: int, keep=None):
+    """(dz [num_all, H*D] in z's dtype, del [num_all, H] fp32) over the CSC of the graph."""
+    plan = graph.bwd
+    n, hd = plan.n_rows, z.shape[1]
+    d = hd // heads
+    dz = alloc_rows(n, hd, z.dtype, z.device)
+    dl = torch.empty(n, heads, dtype=torch.float32, device=z.device)
+    scratch = _gat_scratch(plan, heads, d)
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_gat_bwd_src(C.byref(plan.c), z.data_ptr(), z.stride(0), g.data_ptr(), g.stride(0), heads, d,
+                                   _C.dtype_code(z.dtype), el.data_ptr(), er.data_ptr(), m.data_ptr(), s.data_ptr(),
+                                   dv.data_ptr(), der.data_ptr(), attn_l.data_ptr(), attn_r.data_ptr(), _ptr(keep),
+                                   graph.num_in, dz.data_ptr(), dz.stride(0), dl.data_ptr(), _ptr(scratch),
+                                   _C.stream_ptr()), "pg_gat_bwd_src")
+    return dz, dl
+
+
+def gat_colsum(x: torch.Tensor, heads: int = 1, coef: torch.Tensor = None) -> torch.Tensor:
+    """fp32 [H*D]: sum_r coef[r, k] * x[r, k*D + c] (coef None: plain column sums), in a fixed order."""
+    _rows(x)
+    n, hd = x.shape
+    nb = int(_C.lib.pg_gat_colsum_blocks(n))
+    partial = torch.empty(nb * hd, dtype=torch.float32, device=x.device)
+    out = torch.empty(hd, dtype=torch.float32, device=x.device)
+    _C.count(2)
+    _C.check(_C.lib.pg_gat_colsum(x.data_ptr(), x.stride(0), n, heads, hd // heads, _C.dtype_code(x.dtype),
+                                  _ptr(coef), out.data_ptr(), partial.data_ptr(), _C.stream_ptr()), "pg_gat_colsum")
+    return out
+
+
+class GatLayerFn(torch.autograd.Function):
+    """One GAT layer (DGL GATConv, no attention dropout, no residual) over the [inner | halo] rows `feat` of a
+    partition, returning the inner rows:
+
+        z  = feat @ W^T                    [num_all, H*D]   pg_linear over all rows
+        el, er                             [num_all, H]     pg_gat_scores (er of the inner rows only)
+        out = softmax-aggregate(z) + bias  [N_in, H*D]      pg_gat_aggregate (+ softmax statistics m, s)
+
+    Backward: der, D (pg_gat_bwd_dst over the CSR), dz and del (pg_gat_bwd_src over the CSC), d attn_l / d attn_r
+    and the bias gradient as fixed-order column sums, dW = dz^T feat (pg_wgrad), g_feat = dz @ W (pg_linear, with the
+    dropout backward of `drop_bwd` in its epilogue).  `keep`: the boundary-node sample of the halo rows (uint8), or
+    None."""
+
+    @staticmethod
+    def forward(ctx, feat, graph, keep, heads, weight, attn_l, attn_r, bias, drop_bwd=None):
+        ctx.drop_bwd = drop_bwd
+        if feat.stride(1) != 1:
+            feat = feat.contiguous()
+        n_in = graph.num_in
+        z = gemm_nt(presplit(feat), padded_weight(weight, feat.dtype))
+        al, ar = _f32(attn_l), _f32(attn_r)
+        el, er = gat_scores(z, al, ar, heads, n_in)
+        b32 = _f32(bias) if bias is not None else None
+        out, m, s = gat_aggregate(graph, z, el, er, b32, heads, keep)
+        ctx.save_for_backward(feat, z, el, er, m, s, weight)
+        ctx.graph, ctx.keep, ctx.heads, ctx.al, ctx.ar, ctx.b32 = graph, keep, heads, al, ar, b32
+        ctx.attn_shape, ctx.attn_dtype = tuple(attn_l.shape), attn_l.dtype
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        feat, z, el, er, m, s, weight = ctx.saved_tensors
+        graph, heads, keep = ctx.graph, ctx.heads, ctx.keep
+        n_in = graph.num_in
+        colsum = _take_colsum(g)
+        g = _tma_ready(g if g.dtype == feat.dtype else g.to(feat.dtype))
+        der, dv = gat_bwd_dst(graph, z, g, el, er, m, s, heads, keep)
+        dz, dl = gat_bwd_src(graph, z, g, el, er, m, s, dv, der, ctx.al, ctx.ar, heads, keep)
+        g_al = gat_colsum(z, heads, dl).view(ctx.attn_shape).to(ctx.attn_dtype)
+        g_ar = gat_colsum(z[:n_in], heads, der).view(ctx.attn_shape).to(ctx.attn_dtype)
+        gb = None
+        if ctx.b32 is not None:
+            gb = colsum if colsum is not None else gat_colsum(g)
+        dzsp = presplit(dz)
+        g_feat = None
+        if ctx.needs_input_grad[0]:
+            g_feat = alloc_rows(feat.shape[0], feat.shape[1], feat.dtype, feat.device)
+            drop = ctx.drop_bwd if ctx.drop_bwd is not None and ctx.drop_bwd.p > 0 else None
+            db = drop if drop is not None and feat.shape[1] <= 256 and _drop_ok(g_feat) else None
+            gemm_nt(dzsp, padded_weight(weight, feat.dtype, transpose=True), out=g_feat, drop=db)
+            if drop is not None and db is None:
+                dropout_rows(g_feat, drop, out=g_feat)
+        gw = wgrad(dzsp, presplit(feat)).to(weight.dtype)
+        return g_feat, None, None, None, gw, g_al, g_ar, gb, None
+
+
+def gat_layer(feat, graph, keep, heads, weight, attn_l, attn_r, bias, drop_bwd=None) -> torch.Tensor:
+    return GatLayerFn.apply(feat, graph, keep, int(heads), weight, attn_l, attn_r, bias, drop_bwd)
+
+
 # ---- row-wise epilogues (csrc/rowops.cu) -------------------------------------------------------------------
 # column sums of a gradient tensor computed as a by-product by the kernel that produced it, keyed by the
 # tensor's address: the bias gradient of the linear upstream (saves a full pass over [N, d])

@@ -32,7 +32,7 @@ from .helper import context as ctx
 from .helper.feature_buffer import Buffer, EvalExchange, OneShotExchange, check_sampling
 from .helper.reducer import Reducer
 from .helper.timer.comm_timer import CommTimer
-from .module.model import GraphSAGE
+from .module.model import GAT, GraphSAGE
 from .partition import PartitionLayout, get_layer_size
 
 
@@ -41,10 +41,26 @@ def _bns_seed(args):
     return bns_seed(getattr(args, 'seed', 0))
 
 
+def check_model(args):
+    """Refuses, before anything is allocated, a --model gat configuration that is not implemented: --use-pp (the
+    precompute is GraphSAGE's neighbour mean) and a hidden width that does not split into --n-heads heads."""
+    if args.model != 'gat':
+        return
+    if args.use_pp:
+        raise NotImplementedError("--model gat with --use-pp: the precompute is GraphSAGE's neighbour mean")
+    heads = getattr(args, 'n_heads', 4)
+    if heads < 1 or args.n_hidden % heads:
+        raise ValueError(f"--model gat: --n-hidden {args.n_hidden} does not split into --n-heads {heads} heads")
+
+
 def create_model(layer_size, args, buffer=None, dtype=torch.float32):
     if args.model in ('graphsage', 'gcn'):
         return GraphSAGE(layer_size, F.relu, args.use_pp, norm=args.norm, dropout=args.dropout,
                          n_linear=args.n_linear, train_size=args.n_train, buffer=buffer, dtype=dtype)
+    if args.model == 'gat':
+        check_model(args)
+        return GAT(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
+                   train_size=args.n_train, buffer=buffer, dtype=dtype, n_heads=getattr(args, 'n_heads', 4))
     raise NotImplementedError(args.model)
 
 
@@ -93,6 +109,7 @@ class RankEngine:
                  reducer: Optional[Reducer] = None, init_state=None, seg_len=None):
         sampling_rate = check_sampling(getattr(args, 'sampling_rate', 1.0), args.enable_pipeline, args.feat_corr,
                                        args.grad_corr)
+        check_model(args)
         self.args, self.world, self.rank = args, world, world.rank
         dev = world.device
         self.device = dev
@@ -678,6 +695,7 @@ def check_parser(args):
 def init_processes(rank, size, args):
     """Initialise the distributed environment and train this rank (train.py:408-416)."""
     check_sampling(getattr(args, 'sampling_rate', 1.0), args.enable_pipeline, args.feat_corr, args.grad_corr)
+    check_model(args)
     os.environ['MASTER_ADDR'] = args.master_addr
     os.environ['MASTER_PORT'] = '%d' % args.port
     import torch.distributed as dist
