@@ -313,6 +313,48 @@ int pg_bns_mask_rows(const void* src, int64_t ld_src, void* dst, int64_t ld_dst,
                      const uint8_t* mask, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Quantised halo messages (--halo-bits b, b = 8 or 4).  Every message row of d elements travels as b-bit codes plus an
+ * fp32 pair (lo, scale): lo = min, scale = (max - lo) / (2^b - 1) over the d elements (fp32, correctly rounded),
+ *   q = clamp(floor((x - lo) * inv + u), 0, 2^b - 1),  inv = (2^b - 1) / (max - lo)
+ * with every operation rounded separately (no FMA; q = 0 unless scale > 0 and inv is finite), and the receiver decodes
+ * lo + q * scale (a multiply, then an add).  4-bit codes pack two per byte, the even element
+ * in the low nibble; a code row is padded to 16 bytes.  A row with a non-finite element or a non-finite range ships
+ * lo = scale = NaN (every element decodes to NaN); a never-written (zero) row decodes to zeros.  u in [0, 1) is a pure
+ * function of (seed, layer * 2 + direction, the flag value of the message, the receiving rank, the row the data fills
+ * at the receiver = dst_row0 + i, the element) with 24 random bits (csrc/common.cuh: quant_key / quant_u).
+ * ---------------------------------------------------------------------------------------- */
+typedef struct pg_quant {
+  uint64_t seed;
+  int32_t bits;               /* 8 or 4 */
+  int32_t stream;             /* layer * 2 + direction (0 = features, 1 = gradients) */
+} pg_quant;
+/* per message of a quantised push */
+typedef struct pg_qmsg {
+  float* pairs;               /* (lo, scale) of row 0 of the message, [n_rows][2] fp32 -- normally peer memory */
+  int32_t rank;               /* the receiving rank */
+  int32_t pad;
+} pg_qmsg;
+/* pg_halo_push without EMA and dropout, storing codes: message m's row i goes to msgs[m].dst + i * ld_dst (ld_dst in
+ * BYTES, a multiple of 16; dst 16-byte aligned) and its pair to qmsgs[m].pairs + 2 i.  One warp per row.  Flags are
+ * published as by pg_halo_push, also for empty messages; value (+ *value_dev) is also the noise's step. */
+int pg_halo_push_q(const pg_msg* msgs, int32_t n_msgs, int32_t n_ctas, const pg_qmsg* qmsgs, const void* src,
+                   int64_t ld_src, int32_t d, int dtype, uint32_t value, const uint32_t* value_dev, const pg_quant* q,
+                   void* stream);
+/* out[r, 0:d] = decode(codes[r], pairs[r]) for r < n_rows (activation dtype; out 16-byte aligned, ld_out >= d rounded
+ * up to 8).  With `mirror` (fp32 [n_rows, ld_mirror], 16-byte aligned) the receiver's EMA first runs
+ * mirror <- m * mirror + (1 - m) * decoded (two roundings, no FMA) and out receives the mirror.  With `drop` the mask
+ * of that key is applied as pg_dropout_rows(row0 = drop_row0) would apply it to the undropped output. */
+int pg_halo_dequant(const uint8_t* codes, int64_t ld_codes, const float* pairs, int32_t n_rows, int32_t d, int32_t bits,
+                    void* out, int64_t ld_out, int dtype, float* mirror, int64_t ld_mirror, float momentum,
+                    float one_minus, const pg_drop* drop, int64_t drop_row0, void* stream);
+/* pg_boundary_add over code rows: grad[urow[i]] += v_k for k in [uptr[i], uptr[i+1]) in that order, v_k the decoded
+ * slot usrc[k] (with `mirror`: that slot's fp32 mirror after its EMA update) rounded to the activation dtype; the sum
+ * is fp32, rounded to the dtype after every add. */
+int pg_boundary_add_q(void* grad, int64_t ld_grad, int32_t d, int dtype, const uint8_t* codes, int64_t ld_codes,
+                      const float* pairs, int32_t bits, const int32_t* urow, const int32_t* uptr, const int32_t* usrc,
+                      int32_t n_urow, float* mirror, int64_t ld_mirror, float momentum, float one_minus, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Graph attention (GAT, DGL GATConv with negative_slope 0.2, no attention dropout) over the `_U` rows
  * [inner | halo] of one partition.  z [num_all, H * D] (fp32 or bf16, `dtype`) holds H heads of D columns per row;
  * el [num_all, H] and er [N_in, H] are fp32 scores; for the in-edges u -> v of the forward CSR

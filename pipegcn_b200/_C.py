@@ -46,6 +46,14 @@ class pg_bns(C.Structure):
     _fields_ = [("seed", C.c_uint64), ("thresh", C.c_uint32), ("epoch", C.c_uint32), ("epoch_dev", C.c_void_p)]
 
 
+class pg_quant(C.Structure):
+    _fields_ = [("seed", C.c_uint64), ("bits", C.c_int32), ("stream", C.c_int32)]
+
+
+class pg_qmsg(C.Structure):
+    _fields_ = [("pairs", C.c_void_p), ("rank", C.c_int32), ("pad", C.c_int32)]
+
+
 def _load():
     if not _LIB_PATH.exists():
         raise PgError(f"{_LIB_PATH} is missing: build it with `python -m pipegcn_b200.build` "
@@ -91,6 +99,10 @@ def _load():
                                        C.POINTER(pg_bns), vp]),
         "pg_boundary_add_bns": (C.c_int, [vp, i64, vp, i64, i32, C.c_int, vp, vp, vp, i32, vp, C.POINTER(pg_bns), vp]),
         "pg_bns_mask_rows": (C.c_int, [vp, i64, vp, i64, i32, i32, C.c_int, vp, vp]),
+        "pg_halo_push_q": (C.c_int, [vp, i32, i32, vp, vp, i64, i32, C.c_int, u32, vp, C.POINTER(pg_quant), vp]),
+        "pg_halo_dequant": (C.c_int, [vp, i64, vp, i32, i32, i32, vp, i64, C.c_int, vp, i64, f32, f32,
+                                      C.POINTER(pg_drop), i64, vp]),
+        "pg_boundary_add_q": (C.c_int, [vp, i64, i32, C.c_int, vp, i64, vp, i32, vp, vp, vp, i32, vp, i64, f32, f32, vp]),
         "pg_gat_preload": (C.c_int, []),
         "pg_gat_scores": (C.c_int, [vp, i64, i32, i32, i32, i32, C.c_int, vp, vp, vp, vp, vp]),
         "pg_gat_aggregate": (C.c_int, [C.POINTER(pg_csr), vp, i64, i32, i32, C.c_int, vp, vp, vp, vp, i32, vp, i64,

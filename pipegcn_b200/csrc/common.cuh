@@ -212,6 +212,19 @@ __device__ __forceinline__ uint32_t bns_key(uint64_t seed, uint32_t t, uint32_t 
 __device__ __forceinline__ bool bns_keep(uint32_t key, uint32_t h, uint32_t thresh) {
   return mix32(mix32(h ^ key) + key) < thresh;
 }
+// ---- quantised halo messages (pg_quant) ------------------------------------------------------------------------------
+// The stochastic-rounding noise u in [0, 1) of element e of the message row that fills row `row` of the receiver: a pure
+// function of (seed, layer * 2 + direction, step = the message's flag value, receiving rank, row, e), 24 random bits.
+// pipegcn_b200/ops.py (quant_noise_host) ports it to the host.
+__device__ __forceinline__ uint32_t quant_key(uint64_t seed, uint32_t stream, uint32_t step, uint32_t rank) {
+  const uint32_t k = mix32(static_cast<uint32_t>(seed >> 32) + 0x27d4eb2fU * (step + 1u));
+  const uint32_t k2 = mix32((static_cast<uint32_t>(seed) ^ k) + 0x165667b1U * (rank + 1u));
+  return mix32(k2 + 0xd3a2646bU * (stream + 1u));
+}
+__device__ __forceinline__ uint32_t quant_row_key(uint32_t key, uint32_t row) { return mix32(mix32(row ^ key) + key); }
+__device__ __forceinline__ float quant_u(uint32_t row_key, uint32_t e) {
+  return static_cast<float>(mix32(row_key + 0x9e3779b9U * (e + 1u)) >> 8) * 5.9604644775390625e-08f;   // * 2^-24
+}
 
 inline DropArg make_drop(const pg_drop* d) {
   DropArg a{0u, 1.f, 0u, 0u, nullptr, 0};

@@ -604,6 +604,363 @@ extern "C" int pg_bns_mask_rows(const void* src, int64_t ld_src, void* dst, int6
   return PG_OK;
 }
 
+// ---- quantised halo messages (--halo-bits) ----------------------------------------------------
+// A lane owns chunks of 8 consecutive elements: 8 codes are 8 bytes (8-bit) or 4 bytes (4-bit), one vector store.
+namespace pg {
+constexpr int kQChunk = 8;
+
+// elements [e0, e0 + 8) of a row; VEC: 16-byte loads (the row is 16-byte aligned and padded to 8 elements),
+// else scalar loads of the elements < d.  Elements >= d read as 0.
+template <typename T, bool VEC>
+__device__ __forceinline__ void load8(const T* p, int e0, int d, float (&f)[kQChunk]) {
+  if constexpr (VEC) {
+    using P = Pack<T, 16>;
+#pragma unroll
+    for (int h = 0; h < kQChunk / P::V; ++h)
+      P::unpack(*reinterpret_cast<const typename P::Raw*>(p + e0 + h * P::V), f + h * P::V);
+#pragma unroll
+    for (int i = 0; i < kQChunk; ++i) if (e0 + i >= d) f[i] = 0.f;
+  } else {
+#pragma unroll
+    for (int i = 0; i < kQChunk; ++i) {
+      float x = 0.f;
+      if (e0 + i < d) {
+        if constexpr (sizeof(T) == 2) x = __bfloat162float(p[e0 + i]);
+        else x = p[e0 + i];
+      }
+      f[i] = x;
+    }
+  }
+}
+// the inverse; VEC stores the whole chunk (the caller keeps elements >= d as they were)
+template <typename T, bool VEC>
+__device__ __forceinline__ void store8(T* p, int e0, int d, const float (&f)[kQChunk]) {
+  if constexpr (VEC) {
+    using P = Pack<T, 16>;
+#pragma unroll
+    for (int h = 0; h < kQChunk / P::V; ++h) st_vec<16>(p + e0 + h * P::V, P::pack(f + h * P::V));
+  } else {
+#pragma unroll
+    for (int i = 0; i < kQChunk; ++i) {
+      if (e0 + i < d) {
+        if constexpr (sizeof(T) == 2) p[e0 + i] = __float2bfloat16_rn(f[i]);
+        else p[e0 + i] = f[i];
+      }
+    }
+  }
+}
+template <typename T>
+__device__ __forceinline__ float round_to(float x) {
+  if constexpr (sizeof(T) == 2) return __bfloat162float(__float2bfloat16_rn(x));
+  else return x;
+}
+
+template <int BITS> struct Codes;
+template <> struct Codes<8> {
+  using Raw = uint2;
+  __device__ __forceinline__ static Raw pack(const uint32_t (&q)[kQChunk]) {
+    return make_uint2(q[0] | q[1] << 8 | q[2] << 16 | q[3] << 24, q[4] | q[5] << 8 | q[6] << 16 | q[7] << 24);
+  }
+  __device__ __forceinline__ static uint32_t get(const Raw& r, int i) { return ((i < 4 ? r.x : r.y) >> (8 * (i & 3))) & 0xffu; }
+};
+template <> struct Codes<4> {
+  using Raw = uint32_t;
+  __device__ __forceinline__ static Raw pack(const uint32_t (&q)[kQChunk]) {
+    uint32_t w = 0u;
+#pragma unroll
+    for (int i = 0; i < kQChunk; ++i) w |= q[i] << (4 * i);     // even element in the low nibble of its byte
+    return w;
+  }
+  __device__ __forceinline__ static uint32_t get(const Raw& r, int i) { return (r >> (4 * i)) & 0xfu; }
+};
+
+// the decoded chunk c of a code row (elements >= d: 0)
+template <int BITS>
+__device__ __forceinline__ void decode8(const uint8_t* row, float2 ls, int c, int d, float (&f)[kQChunk]) {
+  using Cd = Codes<BITS>;
+  const typename Cd::Raw r = *reinterpret_cast<const typename Cd::Raw*>(row + c * (kQChunk * BITS / 8));
+#pragma unroll
+  for (int i = 0; i < kQChunk; ++i)
+    f[i] = (c * kQChunk + i < d) ? __fadd_rn(ls.x, __fmul_rn(static_cast<float>(Cd::get(r, i)), ls.y)) : 0.f;
+}
+// mirror <- m * mirror + (1 - m) * f (feature_buffer.py:189-191, two roundings), f <- mirror
+__device__ __forceinline__ void ema8(float* mp, float m, float one_minus, float (&f)[kQChunk]) {
+  float4* p4 = reinterpret_cast<float4*>(mp);
+  float4 a = p4[0], b = p4[1];
+  float e[kQChunk] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
+#pragma unroll
+  for (int i = 0; i < kQChunk; ++i) f[i] = __fadd_rn(__fmul_rn(e[i], m), __fmul_rn(one_minus, f[i]));
+  p4[0] = make_float4(f[0], f[1], f[2], f[3]);
+  p4[1] = make_float4(f[4], f[5], f[6], f[7]);
+}
+
+template <typename T, int BITS, bool VEC>
+__global__ void __launch_bounds__(kPushThreads)
+halo_push_q_kernel(const pg_msg* __restrict__ msgs, int n_msgs, const pg_qmsg* __restrict__ qmsgs,
+                   const T* __restrict__ src, int64_t ld_src, int d, uint32_t value,
+                   const uint32_t* __restrict__ value_dev, pg_quant q) {
+  if (value_dev != nullptr) value += *value_dev;
+  int m = 0;
+  while (m + 1 < n_msgs && static_cast<int>(blockIdx.x) >= msgs[m + 1].cta_begin) ++m;
+  // the fields of message m one by one (a copy of the whole descriptor would go through local memory)
+  const pg_msg& msg = msgs[m];
+  const int32_t* idx = msg.idx;
+  const int64_t src_row0 = msg.src_row0, ld_dst = msg.ld_dst, dst_row0 = msg.dst_row0;
+  uint8_t* const dst = static_cast<uint8_t*>(msg.dst);
+  const uint32_t key = quant_key(q.seed, static_cast<uint32_t>(q.stream), value, static_cast<uint32_t>(qmsgs[m].rank));
+  float2* pairs = reinterpret_cast<float2*>(qmsgs[m].pairs);
+  const int row0 = (static_cast<int>(blockIdx.x) - msg.cta_begin) * kPushRows;
+  const int n_rows = msg.n_rows;
+  const int row1 = min(n_rows, row0 + kPushRows);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int nch = (d + kQChunk - 1) / kQChunk;
+  constexpr float qmax = static_cast<float>((1 << BITS) - 1);
+  using Cd = Codes<BITS>;
+
+  for (int r = row0 + warp; r < row1; r += kPushThreads / 32) {
+    const int64_t srow = idx ? static_cast<int64_t>(__ldg(idx + r)) : src_row0 + r;
+    const T* sp = src + srow * ld_src;
+    float lo = INFINITY, hi = -INFINITY;
+    bool bad = false;
+    for (int c = lane; c < nch; c += 32) {
+      float f[kQChunk];
+      load8<T, VEC>(sp, c * kQChunk, d, f);
+#pragma unroll
+      for (int i = 0; i < kQChunk; ++i) {
+        if (c * kQChunk + i < d) {
+          lo = fminf(lo, f[i]);
+          hi = fmaxf(hi, f[i]);
+          bad |= !isfinite(f[i]);
+        }
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      lo = fminf(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+      hi = fmaxf(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+    }
+    bad = __any_sync(0xffffffffu, bad);
+    const float range = __fsub_rn(hi, lo);
+    float scale = __fdiv_rn(range, qmax);
+    const float inv = __fdiv_rn(qmax, range);                                  // (x - lo) / scale as (x - lo) * inv
+    if (bad || !isfinite(scale)) lo = scale = __int_as_float(0x7fc00000);      // NaN: the row decodes to NaN
+    const bool coded = scale > 0.f && isfinite(inv);                           // false: constant / NaN rows, q = 0
+    const uint32_t rk = quant_row_key(key, static_cast<uint32_t>(dst_row0 + r));
+    uint8_t* dp = dst + static_cast<int64_t>(r) * ld_dst;
+    for (int c = lane; c < nch; c += 32) {
+      float f[kQChunk];
+      load8<T, VEC>(sp, c * kQChunk, d, f);
+      uint32_t qs[kQChunk];
+#pragma unroll
+      for (int i = 0; i < kQChunk; ++i) {
+        const int e = c * kQChunk + i;
+        float t = 0.f;
+        if (coded && e < d)
+          t = fminf(fmaxf(floorf(__fadd_rn(__fmul_rn(__fsub_rn(f[i], lo), inv), quant_u(rk, static_cast<uint32_t>(e)))), 0.f), qmax);
+        qs[i] = static_cast<uint32_t>(t);
+      }
+      *reinterpret_cast<typename Cd::Raw*>(dp + c * (kQChunk * BITS / 8)) = Cd::pack(qs);
+    }
+    if (lane == 0) pairs[r] = make_float2(lo, scale);
+  }
+
+  // flags exactly as halo_push_kernel publishes them
+  if (blockIdx.x == 0 && static_cast<int>(threadIdx.x) < n_msgs) {
+    const pg_msg& em = msgs[threadIdx.x];
+    if (em.n_rows == 0 && em.flag != nullptr) st_release_sys(em.flag, value);
+  }
+  if (msg.flag != nullptr) {
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      const int n_ctas = (n_rows + kPushRows - 1) / kPushRows;
+      __threadfence_system();
+      const unsigned prev = atomicAdd(msg.counter, 1u);
+      if (prev == static_cast<unsigned>(n_ctas - 1)) {
+        *msg.counter = 0u;
+        __threadfence_system();
+        st_release_sys(msg.flag, value);
+      }
+    }
+  }
+}
+
+// one warp per row: decode, (EMA), (dropout), store in the activation dtype
+template <typename T, int BITS>
+__global__ void __launch_bounds__(256)
+halo_dequant_kernel(const uint8_t* __restrict__ codes, int64_t ld_codes, const float2* __restrict__ pairs, int n_rows,
+                    int d, T* __restrict__ out, int64_t ld_out, float* __restrict__ mirror, int64_t ld_mirror,
+                    float momentum, float one_minus, DropArg drop, int64_t drop_row0) {
+  const uint32_t drop_hi = drop_seed_hi(drop);
+  using P = Pack<T, 16>;
+  constexpr int V = P::V;                            // elements per 16-byte vector: the dropout mask's unit
+  const int nvec = (d + V - 1) / V;
+  const int nch = (d + kQChunk - 1) / kQChunk;
+  const int lane = threadIdx.x & 31;
+  const int64_t nw = static_cast<int64_t>(gridDim.x) * (blockDim.x >> 5);
+  for (int64_t r = (static_cast<int64_t>(blockIdx.x) * blockDim.x + threadIdx.x) >> 5; r < n_rows; r += nw) {
+    const float2 ls = __ldg(pairs + r);
+    const uint8_t* cr = codes + r * ld_codes;
+    for (int c = lane; c < nch; c += 32) {
+      float f[kQChunk];
+      decode8<BITS>(cr, ls, c, d, f);
+      if (mirror != nullptr) ema8(mirror + r * ld_mirror + c * kQChunk, momentum, one_minus, f);
+      if (drop.thresh16 != 0u) {                   // what pg_dropout_rows makes of the stored (rounded) row
+#pragma unroll
+        for (int i = 0; i < kQChunk; ++i) f[i] = round_to<T>(f[i]);
+#pragma unroll
+        for (int h = 0; h < kQChunk / V; ++h) {
+          float g[V];
+#pragma unroll
+          for (int i = 0; i < V; ++i) g[i] = f[h * V + i];
+          drop_apply<V>(g, static_cast<uint64_t>(drop_row0 + r) * nvec + c * (kQChunk / V) + h, drop.thresh16, drop.scale,
+                        drop.seed_lo, drop_hi);
+#pragma unroll
+          for (int i = 0; i < V; ++i) f[h * V + i] = g[i];
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < kQChunk; ++i) if (c * kQChunk + i >= d) f[i] = 0.f;
+      store8<T, true>(out + r * ld_out, c * kQChunk, d, f);
+    }
+  }
+}
+
+template <typename T, int BITS, bool VEC>
+__global__ void __launch_bounds__(256)
+boundary_add_q_kernel(T* __restrict__ grad, int64_t ld_grad, int d, const uint8_t* __restrict__ codes, int64_t ld_codes,
+                      const float2* __restrict__ pairs, const int32_t* __restrict__ urow, const int32_t* __restrict__ uptr,
+                      const int32_t* __restrict__ usrc, int n_urow, float* __restrict__ mirror, int64_t ld_mirror,
+                      float momentum, float one_minus) {
+  const int w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (w >= n_urow) return;
+  T* gp = grad + static_cast<int64_t>(__ldg(urow + w)) * ld_grad;
+  const int k0 = __ldg(uptr + w), k1 = __ldg(uptr + w + 1);
+  const int nch = (d + kQChunk - 1) / kQChunk;
+  for (int c = lane; c < nch; c += 32) {
+    float g[kQChunk];
+    if constexpr (VEC) {                             // the padding columns are stored back as they were
+      using P = Pack<T, 16>;
+#pragma unroll
+      for (int h = 0; h < kQChunk / P::V; ++h)
+        P::unpack(*reinterpret_cast<const typename P::Raw*>(gp + c * kQChunk + h * P::V), g + h * P::V);
+    } else {
+      load8<T, false>(gp, c * kQChunk, d, g);
+    }
+    for (int k = k0; k < k1; ++k) {
+      const int s = __ldg(usrc + k);
+      float f[kQChunk];
+      decode8<BITS>(codes + static_cast<int64_t>(s) * ld_codes, __ldg(pairs + s), c, d, f);
+      if (mirror != nullptr) ema8(mirror + static_cast<int64_t>(s) * ld_mirror + c * kQChunk, momentum, one_minus, f);
+#pragma unroll
+      for (int i = 0; i < kQChunk; ++i)
+        if (c * kQChunk + i < d) g[i] = round_to<T>(__fadd_rn(g[i], round_to<T>(f[i])));
+    }
+    store8<T, VEC>(gp, c * kQChunk, d, g);
+  }
+}
+
+// see bns_preload: no first launch of a quantised-path kernel may happen while a flag wait spins
+static void quant_preload() {
+  static std::once_flag once;
+  std::call_once(once, [] {
+    cudaFuncAttributes a;
+#define PG_LOAD(F) cudaFuncGetAttributes(&a, F)
+#define PG_LOAD_TB(K, T_, B_) PG_LOAD((K<T_, B_, true>)); PG_LOAD((K<T_, B_, false>))
+    PG_LOAD_TB(halo_push_q_kernel, float, 8); PG_LOAD_TB(halo_push_q_kernel, float, 4);
+    PG_LOAD_TB(halo_push_q_kernel, __nv_bfloat16, 8); PG_LOAD_TB(halo_push_q_kernel, __nv_bfloat16, 4);
+    PG_LOAD_TB(boundary_add_q_kernel, float, 8); PG_LOAD_TB(boundary_add_q_kernel, float, 4);
+    PG_LOAD_TB(boundary_add_q_kernel, __nv_bfloat16, 8); PG_LOAD_TB(boundary_add_q_kernel, __nv_bfloat16, 4);
+    PG_LOAD((halo_dequant_kernel<float, 8>)); PG_LOAD((halo_dequant_kernel<float, 4>));
+    PG_LOAD((halo_dequant_kernel<__nv_bfloat16, 8>)); PG_LOAD((halo_dequant_kernel<__nv_bfloat16, 4>));
+    PG_LOAD(halo_flag_only_kernel);
+#undef PG_LOAD_TB
+#undef PG_LOAD
+    cudaGetLastError();
+  });
+}
+
+// 16-byte aligned rows padded to a multiple of 8 elements: the vector path of load8 / store8
+static bool rows8(const void* p, int64_t ld, int d, int es) {
+  return vec_bytes(p, ld, es) == 16 && ld >= round_up(d, kQChunk);
+}
+static int64_t code_bytes(int d, int bits) { return round_up(static_cast<int64_t>(d) * bits, 8) / 8; }
+}  // namespace pg
+
+extern "C" int pg_halo_push_q(const pg_msg* msgs, int32_t n_msgs, int32_t n_ctas, const pg_qmsg* qmsgs, const void* src,
+                              int64_t ld_src, int32_t d, int dtype, uint32_t value, const uint32_t* value_dev,
+                              const pg_quant* q, void* stream) {
+  pg::quant_preload();
+  PG_REQUIRE(msgs && n_msgs > 0 && n_msgs <= pg::kPushThreads, "pg_halo_push_q: 1..%d messages per launch", pg::kPushThreads);
+  PG_REQUIRE(qmsgs != nullptr && q != nullptr && (q->bits == 8 || q->bits == 4), "pg_halo_push_q: bad quantiser");
+  PG_REQUIRE(src != nullptr || n_ctas == 0, "pg_halo_push_q: null source");
+  PG_REQUIRE(d > 0 && ld_src >= d, "pg_halo_push_q: bad sizes");
+  PG_REQUIRE(dtype == PG_F32 || dtype == PG_BF16, "pg_halo_push_q: unknown dtype %d", dtype);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  if (n_ctas > 0) {
+    const bool vec = pg::rows8(src, ld_src, d, pg::elem_size(dtype));
+#define PG_PUSH_Q(T_, B_, V_) pg::halo_push_q_kernel<T_, B_, V_><<<n_ctas, pg::kPushThreads, 0, st>>>(msgs, n_msgs, qmsgs, static_cast<const T_*>(src), ld_src, d, value, value_dev, *q)
+#define PG_PUSH_QB(T_, B_) do { if (vec) PG_PUSH_Q(T_, B_, true); else PG_PUSH_Q(T_, B_, false); } while (0)
+    if (dtype == PG_F32) { if (q->bits == 8) PG_PUSH_QB(float, 8); else PG_PUSH_QB(float, 4); }
+    else { if (q->bits == 8) PG_PUSH_QB(__nv_bfloat16, 8); else PG_PUSH_QB(__nv_bfloat16, 4); }
+#undef PG_PUSH_QB
+#undef PG_PUSH_Q
+    PG_LAUNCH_CHECK();
+  } else {      // every message is empty: nobody else publishes the flags
+    pg::halo_flag_only_kernel<<<(n_msgs + 63) / 64, 64, 0, st>>>(msgs, n_msgs, value, value_dev);
+    PG_LAUNCH_CHECK();
+  }
+  return PG_OK;
+}
+
+extern "C" int pg_halo_dequant(const uint8_t* codes, int64_t ld_codes, const float* pairs, int32_t n_rows, int32_t d,
+                               int32_t bits, void* out, int64_t ld_out, int dtype, float* mirror, int64_t ld_mirror,
+                               float momentum, float one_minus, const pg_drop* drop, int64_t drop_row0, void* stream) {
+  pg::quant_preload();
+  if (n_rows == 0) return PG_OK;
+  PG_REQUIRE(codes && pairs && out && n_rows > 0 && d > 0 && (bits == 8 || bits == 4), "pg_halo_dequant: bad arguments");
+  PG_REQUIRE(dtype == PG_F32 || dtype == PG_BF16, "pg_halo_dequant: unknown dtype %d", dtype);
+  PG_REQUIRE(ld_codes >= pg::code_bytes(d, bits) && ld_codes % 16 == 0 && reinterpret_cast<uintptr_t>(codes) % 16 == 0 &&
+             reinterpret_cast<uintptr_t>(pairs) % 8 == 0, "pg_halo_dequant: code rows must be 16-byte aligned and padded");
+  PG_REQUIRE(pg::rows8(out, ld_out, d, pg::elem_size(dtype)), "pg_halo_dequant: out rows must be 16-byte aligned and padded to 8 elements");
+  PG_REQUIRE(mirror == nullptr || pg::rows8(mirror, ld_mirror, d, 4), "pg_halo_dequant: mirror rows must be 16-byte aligned and padded to 8");
+  const pg::DropArg da = pg::make_drop(drop);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const unsigned blocks = static_cast<unsigned>(std::min<int64_t>((static_cast<int64_t>(n_rows) * 32 + 255) / 256, pg::sm_count() * 16));
+  const float2* pp = reinterpret_cast<const float2*>(pairs);
+#define PG_DEQ(T_, B_) pg::halo_dequant_kernel<T_, B_><<<blocks, 256, 0, st>>>(codes, ld_codes, pp, n_rows, d, static_cast<T_*>(out), ld_out, mirror, ld_mirror, momentum, one_minus, da, drop_row0)
+  if (dtype == PG_F32) { if (bits == 8) PG_DEQ(float, 8); else PG_DEQ(float, 4); }
+  else { if (bits == 8) PG_DEQ(__nv_bfloat16, 8); else PG_DEQ(__nv_bfloat16, 4); }
+#undef PG_DEQ
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+extern "C" int pg_boundary_add_q(void* grad, int64_t ld_grad, int32_t d, int dtype, const uint8_t* codes, int64_t ld_codes,
+                                 const float* pairs, int32_t bits, const int32_t* urow, const int32_t* uptr,
+                                 const int32_t* usrc, int32_t n_urow, float* mirror, int64_t ld_mirror, float momentum,
+                                 float one_minus, void* stream) {
+  pg::quant_preload();
+  if (n_urow == 0) return PG_OK;
+  PG_REQUIRE(grad && codes && pairs && urow && uptr && usrc && (bits == 8 || bits == 4), "pg_boundary_add_q: null argument");
+  PG_REQUIRE(dtype == PG_F32 || dtype == PG_BF16, "pg_boundary_add_q: unknown dtype %d", dtype);
+  PG_REQUIRE(d > 0 && ld_grad >= d, "pg_boundary_add_q: bad sizes");
+  PG_REQUIRE(ld_codes >= pg::code_bytes(d, bits) && ld_codes % 16 == 0 && reinterpret_cast<uintptr_t>(codes) % 16 == 0 &&
+             reinterpret_cast<uintptr_t>(pairs) % 8 == 0, "pg_boundary_add_q: code rows must be 16-byte aligned and padded");
+  PG_REQUIRE(mirror == nullptr || pg::rows8(mirror, ld_mirror, d, 4), "pg_boundary_add_q: mirror rows must be 16-byte aligned and padded to 8");
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool vec = pg::rows8(grad, ld_grad, d, pg::elem_size(dtype));
+  const unsigned blocks = (static_cast<unsigned>(n_urow) * 32u + 255u) / 256u;
+  const float2* pp = reinterpret_cast<const float2*>(pairs);
+#define PG_BADD_Q(T_, B_, V_) pg::boundary_add_q_kernel<T_, B_, V_><<<blocks, 256, 0, st>>>(static_cast<T_*>(grad), ld_grad, d, codes, ld_codes, pp, urow, uptr, usrc, n_urow, mirror, ld_mirror, momentum, one_minus)
+#define PG_BADD_QB(T_, B_) do { if (vec) PG_BADD_Q(T_, B_, true); else PG_BADD_Q(T_, B_, false); } while (0)
+  if (dtype == PG_F32) { if (bits == 8) PG_BADD_QB(float, 8); else PG_BADD_QB(float, 4); }
+  else { if (bits == 8) PG_BADD_QB(__nv_bfloat16, 8); else PG_BADD_QB(__nv_bfloat16, 4); }
+#undef PG_BADD_QB
+#undef PG_BADD_Q
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
 // ---- symmetric heap + CUDA IPC --------------------------------------------------------------
 extern "C" int pg_heap_alloc(size_t bytes, void** ptr) {
   PG_REQUIRE(ptr != nullptr && bytes > 0, "pg_heap_alloc: bad arguments");

@@ -31,6 +31,7 @@ from typing import List, Optional
 import torch
 
 from .. import _C
+from ..ops import quant_row_bytes
 from ..world import Heap, default_world
 from .timer.timer import comm_timer
 
@@ -167,6 +168,20 @@ def check_sampling(sampling_rate, pipeline=False, corr_feat=False, corr_grad=Fal
     return p
 
 
+def check_halo_bits(halo_bits, sampling_rate=1.0):
+    """The halo message width as 8, 4 or None (exact); raises for another width and for quantised messages together
+    with boundary-node sampling (before anything is allocated)."""
+    if halo_bits is None:
+        return None
+    bits = int(halo_bits)
+    if bits not in (8, 4):
+        raise ValueError(f"--halo-bits {halo_bits}: expected 8 or 4")
+    if float(sampling_rate) < 1.0:
+        raise NotImplementedError(f"--halo-bits {bits} together with --sampling-rate {sampling_rate}: quantised halo "
+                                  "messages are implemented without boundary-node sampling only")
+    return bits
+
+
 class _HaloUpdate(torch.autograd.Function):
     @staticmethod
     def forward(ctx, feat, buf, layer, push_src, drop):
@@ -194,10 +209,14 @@ class Buffer(_Exchange):
     def init_buffer(self, num_in, num_all, boundary, f_recv_shape, layer_size, use_pp=False, backend='nccl',
                     pipeline=False, corr_feat=False, corr_grad=False, corr_momentum=0,
                     dtype=torch.float32, world=None, key='pipegcn.buffer', static_layer0=False, sampling_rate=1.0,
-                    sampling_seed=0):
+                    sampling_seed=0, halo_bits=None, quant_seed=0):
         """`sampling_rate` p < 1: boundary-node sampling (synchronous, no corrections): every epoch this rank keeps a
-        random fraction p of its halo rows (`sample`), the peers push only those, the others read as zero rows."""
+        random fraction p of its halo rows (`sample`), the peers push only those, the others read as zero rows.
+        `halo_bits` 8 or 4: the per-epoch messages of graph layers >= 1 (features and gradients) travel as
+        stochastically rounded `halo_bits`-bit codes with an fp32 (lo, scale) per row, keyed by `quant_seed`; the
+        receiver decodes them (and runs the EMA corrections on its own fp32 mirrors).  Layer 0 stays exact."""
         rate = check_sampling(sampling_rate, pipeline, corr_feat, corr_grad)
+        bits = check_halo_bits(halo_bits, rate)
         if backend not in ('nccl', 'nvlink'):
             # the reference implements gloo only and raises for the rest (feature_buffer.py:204-205);
             # this engine implements the NVLink path only
@@ -236,15 +255,32 @@ class Buffer(_Exchange):
 
         # ---- carve the symmetric heap: flags [L][2][P] (row l * 2 + direction), then the row blocks
         self._ld = [_round_up(d, 8) for d in layer_size]
+        # quantised messages: graph layers >= 1 receive code rows [rows, qld] (bytes) and (lo, scale) pairs [rows, 2]
+        # instead of rows of the activation dtype: features into `qf`, gradients into `qb` (no `b_recv`)
+        self._bits, self._quant_seed = bits, int(quant_seed)
+        self._quant = set(range(1, L)) if bits is not None else set()
+        self._qld = {l: quant_row_bytes(layer_size[l], bits) for l in self._quant}
+        n_halo = max(self._num_all - self._num_in, 1)
         off = _round_up(4 * L * 2 * size, _ALIGN)
-        self._f_off, self._b_off = {}, {}
+        self._f_off, self._b_off, self._qf_off, self._qb_off = {}, {}, {}, {}
+
+        def carve_codes(rows, l):
+            nonlocal off
+            c = off
+            off = _round_up(off + rows * self._qld[l], _ALIGN)
+            p = off
+            off = _round_up(off + rows * 8, _ALIGN)
+            return c, p
         for l in range(L):
             if l == 0 and use_pp:
                 continue
             for v in range(self._nver):
                 self._f_off[(l, v)] = off
                 off = _round_up(off + self._num_all * self._ld[l] * self._es, _ALIGN)
-                if l > 0:
+                if l in self._quant:
+                    self._qf_off[(l, v)] = carve_codes(n_halo, l)
+                    self._qb_off[(l, v)] = carve_codes(max(btot, 1), l)
+                elif l > 0:
                     self._b_off[(l, v)] = off
                     off = _round_up(off + max(btot, 1) * self._ld[l] * self._es, _ALIGN)
         self._x0_off = None
@@ -254,17 +290,32 @@ class Buffer(_Exchange):
         self._publish(key, max(off, _ALIGN), {
             'f_off': dict(self._f_off), 'b_off': dict(self._b_off), 'pl': list(self._pl), 'boff': list(self._boff),
             'ld': list(self._ld), 'nver': self._nver, 'es': self._es, 'x0_off': self._x0_off, 'num_in': self._num_in,
+            'halo_bits': bits, 'qf_off': dict(self._qf_off), 'qb_off': dict(self._qb_off),
         }, (L, 2, size))
         self._x0 = None if self._x0_off is None else self._heap.view(
             self._x0_off, (max(self._num_all - self._num_in, 1), self._ld[0]), dtype)
         self._f_buf = {k: self._heap.view(o, (self._num_all, self._ld[k[0]]), dtype) for k, o in self._f_off.items()}
         self._b_recv = {k: self._heap.view(o, (max(btot, 1), self._ld[k[0]]), dtype) for k, o in self._b_off.items()}
 
-        # ---- sender-side EMA mirrors (fp32), one per (layer, peer)
+        def code_views(offs, rows):
+            return {k: (self._heap.view(c, (rows, self._qld[k[0]]), torch.uint8), self._heap.view(p, (rows, 2), torch.float32))
+                    for k, (c, p) in offs.items()}
+        self._qf, self._qb = code_views(self._qf_off, n_halo), code_views(self._qb_off, max(btot, 1))
+
+        # ---- sender-side EMA mirrors (fp32), one per (layer, peer); a quantised layer keeps receiver-side mirrors of
+        #      what arrived instead, one row per halo row / boundary slot
         self._f_ema = [None] * L
         self._b_ema = [None] * L
+        self._qf_ema = [None] * L
+        self._qb_ema = [None] * L
         for l in range(L):
             if l == 0 and use_pp:
+                continue
+            if l in self._quant:
+                if corr_feat:
+                    self._qf_ema[l] = torch.zeros(n_halo, self._ld[l], device=dev)
+                if corr_grad:
+                    self._qb_ema[l] = torch.zeros(max(btot, 1), self._ld[l], device=dev)
                 continue
             if corr_feat:
                 self._f_ema[l] = {j: torch.zeros(int(boundary[j].numel()), self._ld[l], device=dev) for j in self._peers}
@@ -314,16 +365,23 @@ class Buffer(_Exchange):
             t = tables[j]
             if t['ld'] != self._ld or t['nver'] != self._nver or t['es'] != es:
                 raise RuntimeError(f"rank {j} was initialised with a different layer/dtype/pipeline configuration")
+            if t['halo_bits'] != self._bits:
+                raise RuntimeError(f"rank {j} was initialised with halo_bits={t['halo_bits']}, this rank with "
+                                   f"halo_bits={self._bits}")
         cnt = iter(range(self._counters.numel()))
 
         def counter_ptr():
             return self._counters.data_ptr() + 4 * next(cnt)
 
         self._self_msgs, self._fwd_msgs, self._bwd_msgs = {}, {}, {}
+        self._fwd_q, self._bwd_q = {}, {}
         for (l, v) in self._f_off:
             ld = self._ld[l]
             m = _C.pg_msg(None, 0, self._num_in, 0, self._f_buf[(l, v)].data_ptr(), ld, None, 0, None, None, 0)
             self._self_msgs[(l, v)] = self._msg_set([m])
+            if l in self._quant:
+                self._quant_msgs(l, v, tables, base, counter_ptr)
+                continue
             msgs = []
             for j in self._peers:
                 dst = base[j] + tables[j]['f_off'][(l, v)] + tables[j]['pl'][rank] * ld * es
@@ -367,6 +425,27 @@ class Buffer(_Exchange):
         # device arrays of the flag words this rank waits on, per (layer, direction)
         self._wait = {(l, direction): self._wait_ptrs(l * 2 + direction) for l in range(L) for direction in (0, 1)}
 
+    def _quant_msgs(self, l, v, tables, base, counter_ptr):
+        """The quantised feature and gradient messages of (layer l, version v): code rows into the peers' `qf` / `qb`
+        regions, keyed by the row they fill there."""
+        rank, qld, fwd, bwd, fq, bq = self._world.rank, self._qld[l], [], [], [], []
+        for j in self._peers:
+            t = tables[j]
+            row = t['pl'][rank] - t['num_in']                     # my rows' place among peer j's halo rows
+            c, p = t['qf_off'][(l, v)]
+            fwd.append(_C.pg_msg(self._bidx[j].data_ptr(), 0, int(self._bidx[j].numel()), 0, base[j] + c + row * qld,
+                                 qld, None, 0, self._flag_ptr(base[j], l * 2), counter_ptr(), int(t['pl'][rank])))
+            fq.append((base[j] + p + row * 8, j))
+            c, p = t['qb_off'][(l, v)]
+            slot = t['boff'][rank]
+            bwd.append(_C.pg_msg(None, self._pl[j], int(self._recv_shape[j]), 0, base[j] + c + slot * qld, qld,
+                                 None, 0, self._flag_ptr(base[j], l * 2 + 1), counter_ptr(), int(slot)))
+            bq.append((base[j] + p + slot * 8, j))
+        from ..ops import qmsg_array
+        dev = self._world.device
+        self._fwd_msgs[(l, v)], self._fwd_q[(l, v)] = self._msg_set(fwd), qmsg_array(fq, dev) if fq else None
+        self._bwd_msgs[(l, v)], self._bwd_q[(l, v)] = self._msg_set(bwd), qmsg_array(bq, dev) if bq else None
+
     def _keys(self, pairs):
         return torch.tensor(pairs, dtype=torch.int32, device=self._world.device).reshape(-1, 2).contiguous()
 
@@ -400,6 +479,40 @@ class Buffer(_Exchange):
         if not self._bns:
             return None
         return self._bns_mask[:self._num_all - self._num_in].bool()
+
+    # ------------------------------------------------------------------ quantised messages
+    @property
+    def halo_bits(self):
+        """8 or 4 when the messages of graph layers >= 1 travel quantised, else None."""
+        return self._bits
+
+    def quant_message(self, layer, direction, version=0):
+        """Copies of the raw messages this rank last received for (layer, direction 0 = features / 1 = gradients,
+        version): code rows uint8 [rows, quant_row_bytes(d, bits)] and (lo, scale) fp32 [rows, 2], the rows ordered as
+        this rank's halo rows (features) or its concatenated boundary slots (gradients).  None for an exact layer."""
+        views = (self._qf if direction == 0 else self._qb).get((layer, version))
+        if views is None:
+            return None
+        rows = self._num_all - self._num_in if direction == 0 else int(sum(int(self._bidx[j].numel()) for j in self._peers))
+        return views[0][:rows].clone(), views[1][:rows].clone()
+
+    def _push_q(self, layer, direction, v, src, d, offset):
+        ms = (self._fwd_msgs if direction == 0 else self._bwd_msgs)[(layer, v)]
+        if ms is None:
+            return
+        from ..ops import QuantSpec, halo_push_q
+        qm = (self._fwd_q if direction == 0 else self._bwd_q)[(layer, v)]
+        halo_push_q(ms, qm, src, d, QuantSpec(self._bits, self._quant_seed, layer, direction), *self._val(offset))
+
+    def _dequant(self, layer, v, drop):
+        """Decode the halo rows of (layer, version v) into f_buf (receiver's EMA and dropout on the way)."""
+        from ..ops import halo_dequant
+        n = self._num_all - self._num_in
+        if n == 0:
+            return
+        codes, pairs = self._qf[(layer, v)]
+        halo_dequant(codes[:n], pairs[:n], self._layer_size[layer], self._bits, self._f_buf[(layer, v)][self._num_in:],
+                     self._qf_ema[layer], self._corr_momentum, drop, self._num_in)
 
     def _push_bns(self, ms, keys, src, d, offset, drop=None):
         if ms is None:
@@ -615,10 +728,16 @@ class Buffer(_Exchange):
         src = push_src if push_src is not None else feat      # what the peers receive (clean rows)
         def aliased(v):
             return feat.data_ptr() == self._f_buf[(layer, v)].data_ptr() and feat.stride(0) == self._ld[layer]
+        quant = layer in self._quant
         if not self._pipeline:
             v = 0
             if not aliased(v):
                 self._push(self._self_msgs[(layer, v)], feat, d, 0)
+            if quant:
+                self._push_q(layer, 0, v, src, d, 1)
+                self._wait_flags(layer, 0, 1, f'forward_{layer}')
+                self._dequant(layer, v, drop)
+                return self._f_buf[(layer, v)][:, :d]
             if self._bns:
                 from ..ops import bns_mask_rows
                 self._push_bns(self._fwd_msgs[(layer, v)], self._bns_fwd_keys, src, d, 1, drop)
@@ -634,6 +753,8 @@ class Buffer(_Exchange):
                 self._push(self._self_msgs[(layer, v_use)], feat, d, 0)
             if t > 0:
                 self._wait_flags(layer, 0, 0, f'forward_{layer}')
+            if quant:                                 # epoch 0 decodes the zeroed region: zeros
+                self._dequant(layer, v_use, drop)
             ms = self._fwd_msgs[(layer, v_send)]
             if ms is not None:
                 cur = torch.cuda.current_stream()
@@ -643,8 +764,11 @@ class Buffer(_Exchange):
                     src.record_stream(self._comm_stream)
                 self._keep.append(src)
                 with torch.cuda.stream(self._comm_stream):
-                    # consumed by the peers in the NEXT epoch: their mask of step + 1
-                    self._push(ms, src, d, 1, drop.shifted(1) if drop is not None else None)
+                    if quant:                          # the peers' dequant applies their own mask
+                        self._push_q(layer, 0, v_send, src, d, 1)
+                    else:
+                        # consumed by the peers in the NEXT epoch: their mask of step + 1
+                        self._push(ms, src, d, 1, drop.shifted(1) if drop is not None else None)
                     if zero_copy and not self.graph_mode:
                         ev = torch.cuda.Event()
                         ev.record()
@@ -657,9 +781,12 @@ class Buffer(_Exchange):
         t = epoch
         if grad.stride(1) != 1:
             grad = grad.contiguous()
+        quant = layer in self._quant
         if not self._pipeline:
             v = 0
-            if self._bns:                             # gradients of the kept halo rows only
+            if quant:
+                self._push_q(layer, 1, v, grad, d, epoch - self._epoch + 1)
+            elif self._bns:                           # gradients of the kept halo rows only
                 self._push_bns(self._bwd_msgs[(layer, v)], self._bns_bwd_keys, grad, d, epoch - self._epoch + 1)
             else:
                 self._push(self._bwd_msgs[(layer, v)], grad, d, epoch - self._epoch + 1)
@@ -679,11 +806,20 @@ class Buffer(_Exchange):
                     grad.record_stream(self._comm_stream)
                 self._keep.append(grad)
                 with torch.cuda.stream(self._comm_stream):
-                    self._push(ms, grad, d, epoch - self._epoch + 1)
+                    if quant:
+                        self._push_q(layer, 1, v_send, grad, d, epoch - self._epoch + 1)
+                    else:
+                        self._push(ms, grad, d, epoch - self._epoch + 1)
         return grad[:self._num_in]
 
     def _boundary_add(self, layer, v, grad):
         if self._urow is None:
+            return
+        if layer in self._quant:
+            from ..ops import boundary_add_q
+            codes, pairs = self._qb[(layer, v)]
+            boundary_add_q(grad, self._layer_size[layer], codes, pairs, self._bits, self._urow, self._uptr, self._usrc,
+                           self._qb_ema[layer], self._corr_momentum)
             return
         recv = self._b_recv[(layer, v)]
         _C.count()

@@ -19,6 +19,12 @@ that epoch, so the halo exchange moves p times the bytes.  Evaluation always use
 
 `--model gat` trains graph attention (DGL's GATConv) instead of GraphSAGE; `--n-heads k` (not in the reference, default
 4, suppressed like `--sampling-rate`: read it with getattr(args, 'n_heads', 4)) sets its heads per hidden layer.
+
+`--halo-bits b` (8 or 4; not in the reference) quantises the per-epoch halo messages of graph layers >= 1, features
+forward and gradients backward: every row travels as b-bit codes with an fp32 (lo, scale), stochastically rounded so
+the message stays unbiased, and the receiver decodes it before anything reads it.  Layer 0, --use-pp and the
+evaluation exchange stay exact; it cannot be combined with --sampling-rate p < 1.  Suppressed like `--sampling-rate`:
+read it with getattr(args, 'halo_bits', None).
 """
 import argparse
 
@@ -101,6 +107,9 @@ def build_parser():
                              "(synchronous training; default 1 = all)")
     parser.add_argument('--n-heads', '--n_heads', type=_n_heads, default=argparse.SUPPRESS,
                         help="--model gat: attention heads of every hidden layer (default 4)")
+    parser.add_argument('--halo-bits', '--halo_bits', type=int, choices=[8, 4], default=argparse.SUPPRESS,
+                        help="send the halo messages of graph layers >= 1 as stochastically rounded 8- or 4-bit codes "
+                             "(default: exact)")
     return parser
 
 

@@ -112,6 +112,143 @@ def bns_mask_rows(mask: torch.Tensor, dst: torch.Tensor, src: torch.Tensor = Non
     return dst
 
 
+class QuantSpec:
+    """Key of one quantised message stream (include/pipegcn_b200.h: pg_quant): bits, 64-bit run seed, graph layer and
+    direction (0 = features, 1 = gradients)."""
+
+    def __init__(self, bits: int, seed: int, layer: int = 0, direction: int = 0):
+        if bits not in (8, 4):
+            raise ValueError(f"halo bits {bits}: expected 8 or 4")
+        self.bits, self.seed = int(bits), int(seed) & 0xFFFFFFFFFFFFFFFF
+        self.layer, self.direction = int(layer), int(direction)
+
+    def c(self):
+        return _C.pg_quant(self.seed, self.bits, 2 * self.layer + self.direction)
+
+
+def quant_seed(seed: int) -> int:
+    """Seed of the rounding noise of quantised halo messages from the run's --seed (the same on every rank)."""
+    return (int(seed) * 0x9E3779B97F4A7C15 + 0x7A3B1D5E0C9F4821) & 0xFFFFFFFFFFFFFFFF
+
+
+def quant_row_bytes(d: int, bits: int) -> int:
+    """Bytes of one code row: ceil(d * bits / 8) padded to 16."""
+    return ((int(d) * int(bits) + 7) // 8 + 15) // 16 * 16
+
+
+def quant_link_bytes(rows: int, d: int, bits, elem_size: int = 4) -> int:
+    """Bytes a message of `rows` rows moves: code rows plus the (lo, scale) pairs, or rows * d * elem_size exact."""
+    if bits is None:
+        return int(rows) * int(d) * int(elem_size)
+    return int(rows) * (quant_row_bytes(d, bits) + 8)
+
+
+def quant_noise_host(seed: int, layer: int, direction: int, step: int, rank: int, rows, d: int):
+    """Host port of csrc/common.cuh's quant_key / quant_row_key / quant_u: float32 [len(rows), d] noise u in [0, 1) of
+    the message rows that fill receiver rows `rows` of rank `rank`, in the message whose flag value is `step`."""
+    import numpy as np
+    M = 0xFFFFFFFF
+    seed = int(seed) & 0xFFFFFFFFFFFFFFFF
+    k = _mix32(((seed >> 32) + 0x27D4EB2F * ((step + 1) & M)) & M)
+    k2 = _mix32((((seed & M) ^ k) + 0x165667B1 * ((rank + 1) & M)) & M)
+    key = _mix32((k2 + 0xD3A2646B * ((2 * layer + direction + 1) & M)) & M)
+    r = np.asarray(rows, dtype=np.uint64).reshape(-1) & np.uint64(M)
+    rk = _mix32((_mix32(r ^ np.uint64(key)) + np.uint64(key)) & np.uint64(M))
+    e = np.arange(d, dtype=np.uint64)
+    h = _mix32((rk[:, None] + np.uint64(0x9E3779B9) * (e[None, :] + np.uint64(1))) & np.uint64(M))
+    return (h >> np.uint64(8)).astype(np.float32) * np.float32(2.0 ** -24)
+
+
+def quantise_host(x, bits: int, seed: int, layer: int, direction: int, step: int, rank: int, row0: int):
+    """Host port of pg_halo_push_q for the rows x [n, d] (float32 values) of one message filling receiver rows
+    row0.. of rank `rank`: (codes uint8 [n, quant_row_bytes(d, bits)], lo float32 [n], scale float32 [n])."""
+    import numpy as np
+    x = np.asarray(x, dtype=np.float32)
+    n, d = x.shape
+    qmax = np.float32(2 ** bits - 1)
+    with np.errstate(all='ignore'):
+        bad = ~np.isfinite(x).all(axis=1)
+        lo = x.min(axis=1) if d else np.zeros(n, np.float32)
+        rng = (x.max(axis=1) - lo).astype(np.float32)
+        scale = (rng / qmax).astype(np.float32)
+        inv = (qmax / rng).astype(np.float32)
+        bad |= ~np.isfinite(scale)
+        lo = np.where(bad, np.float32(np.nan), lo).astype(np.float32)
+        scale = np.where(bad, np.float32(np.nan), scale).astype(np.float32)
+        coded = (scale > 0) & np.isfinite(inv)
+        u = quant_noise_host(seed, layer, direction, step, rank, row0 + np.arange(n), d)
+        t = np.floor(((x - lo[:, None]).astype(np.float32) * inv[:, None]).astype(np.float32) + u)
+        q = np.where(coded[:, None], np.clip(t, 0, qmax), 0).astype(np.uint8)
+    codes = np.zeros((n, quant_row_bytes(d, bits)), dtype=np.uint8)
+    if bits == 8:
+        codes[:, :d] = q
+    else:
+        qe = np.zeros((n, d + d % 2), dtype=np.uint8)
+        qe[:, :d] = q
+        codes[:, :(d + 1) // 2] = qe[:, 0::2] | (qe[:, 1::2] << 4)
+    return codes, lo, scale
+
+
+def dequantise_host(codes, lo, scale, bits: int, d: int):
+    """Host port of the decode: float32 [n, d] = lo + q * scale (a multiply, then an add, each rounded)."""
+    import numpy as np
+    codes = np.asarray(codes, dtype=np.uint8)
+    if bits == 8:
+        q = codes[:, :d]
+    else:
+        b = codes[:, :(d + 1) // 2]
+        q = np.stack([b & 15, b >> 4], axis=2).reshape(codes.shape[0], -1)[:, :d]
+    lo = np.asarray(lo, dtype=np.float32)[:, None]
+    scale = np.asarray(scale, dtype=np.float32)[:, None]
+    return (lo + (q.astype(np.float32) * scale).astype(np.float32)).astype(np.float32)
+
+
+def qmsg_array(entries, device) -> torch.Tensor:
+    """Device array of pg_qmsg for one quantised push: `entries` = [(pairs pointer, receiving rank)] per message."""
+    arr = (_C.pg_qmsg * len(entries))(*[_C.pg_qmsg(p, int(r), 0) for p, r in entries])
+    return torch.frombuffer(bytearray(bytes(arr)), dtype=torch.uint8).to(device)
+
+
+def halo_push_q(ms, qmsgs: torch.Tensor, src: torch.Tensor, d: int, spec: QuantSpec, value: int, value_dev=None):
+    """Quantise the rows of `src` the messages of the `_MsgSet` ms name into their code rows and pairs, publish
+    `value` (+ *value_dev) in their flag words (pg_halo_push_q)."""
+    _C.count()
+    _C.check(_C.lib.pg_halo_push_q(ms.ptr, ms.n_msgs, ms.n_ctas, qmsgs.data_ptr(), src.data_ptr(), src.stride(0), d,
+                                   _C.dtype_code(src.dtype), int(value) & 0xFFFFFFFF, value_dev, C.byref(spec.c()),
+                                   _C.stream_ptr()), "pg_halo_push_q")
+
+
+def halo_dequant(codes: torch.Tensor, pairs: torch.Tensor, d: int, bits: int, out: torch.Tensor,
+                 mirror: torch.Tensor = None, momentum: float = 0.0, drop: DropSpec = None, drop_row0: int = 0):
+    """out[r, :d] = decode(codes[r], pairs[r]) (through the EMA `mirror` when given, then the dropout `drop`)."""
+    n = codes.shape[0]
+    if n == 0:
+        return out
+    _C.count()
+    _C.check(_C.lib.pg_halo_dequant(codes.data_ptr(), codes.stride(0), pairs.data_ptr(), n, d, bits, out.data_ptr(),
+                                    out.stride(0), _C.dtype_code(out.dtype),
+                                    mirror.data_ptr() if mirror is not None else None,
+                                    mirror.stride(0) if mirror is not None else 0, momentum, 1 - momentum,
+                                    C.byref(drop.c()) if drop is not None and drop.p > 0 else None, int(drop_row0),
+                                    _C.stream_ptr()), "pg_halo_dequant")
+    return out
+
+
+def boundary_add_q(grad: torch.Tensor, d: int, codes: torch.Tensor, pairs: torch.Tensor, bits: int, urow, uptr, usrc,
+                   mirror: torch.Tensor = None, momentum: float = 0.0):
+    """grad[urow[i], :d] += the decoded slots usrc[uptr[i]:uptr[i+1]] in that order (pg_boundary_add_q)."""
+    if urow is None or urow.numel() == 0:
+        return grad
+    _C.count()
+    _C.check(_C.lib.pg_boundary_add_q(grad.data_ptr(), grad.stride(0), d, _C.dtype_code(grad.dtype), codes.data_ptr(),
+                                      codes.stride(0), pairs.data_ptr(), bits, urow.data_ptr(), uptr.data_ptr(),
+                                      usrc.data_ptr(), int(urow.numel()),
+                                      mirror.data_ptr() if mirror is not None else None,
+                                      mirror.stride(0) if mirror is not None else 0, momentum, 1 - momentum,
+                                      _C.stream_ptr()), "pg_boundary_add_q")
+    return grad
+
+
 def _drop_ok(t: torch.Tensor) -> bool:
     """The mask is defined on 16-byte vectors of padded, aligned rows."""
     return t.dim() == 2 and t.is_cuda and t.stride(1) == 1 and (t.stride(0) * t.element_size()) % 16 == 0 \

@@ -29,7 +29,7 @@ import torch.nn.functional as F
 
 from .graph import PartGraph
 from .helper import context as ctx
-from .helper.feature_buffer import Buffer, EvalExchange, OneShotExchange, check_sampling
+from .helper.feature_buffer import Buffer, EvalExchange, OneShotExchange, check_halo_bits, check_sampling
 from .helper.reducer import Reducer
 from .helper.timer.comm_timer import CommTimer
 from .module.model import GAT, GraphSAGE
@@ -39,6 +39,11 @@ from .partition import PartitionLayout, get_layer_size
 def _bns_seed(args):
     from .ops import bns_seed
     return bns_seed(getattr(args, 'seed', 0))
+
+
+def _quant_seed(args):
+    from .ops import quant_seed
+    return quant_seed(getattr(args, 'seed', 0))
 
 
 def check_model(args):
@@ -109,6 +114,7 @@ class RankEngine:
                  reducer: Optional[Reducer] = None, init_state=None, seg_len=None):
         sampling_rate = check_sampling(getattr(args, 'sampling_rate', 1.0), args.enable_pipeline, args.feat_corr,
                                        args.grad_corr)
+        halo_bits = check_halo_bits(getattr(args, 'halo_bits', None), sampling_rate)
         check_model(args)
         self.args, self.world, self.rank = args, world, world.rank
         dev = world.device
@@ -126,7 +132,8 @@ class RankEngine:
                                 corr_grad=args.grad_corr, corr_momentum=args.corr_momentum,
                                 dtype=self.dtype, world=world,
                                 static_layer0=bool(getattr(args, 'static_layer0', True)),
-                                sampling_rate=sampling_rate, sampling_seed=_bns_seed(args))
+                                sampling_rate=sampling_rate, sampling_seed=_bns_seed(args),
+                                halo_bits=halo_bits, quant_seed=_quant_seed(args))
         self.feat = layout.feat.to(dev).to(self.dtype)
         # the collective set-up; its first step (allocate and publish this rank's heaps) runs here.  The ranks of a
         # LocalWorld run the rest together (`LocalTrainer`), every other rank runs it now
@@ -694,7 +701,8 @@ def check_parser(args):
 
 def init_processes(rank, size, args):
     """Initialise the distributed environment and train this rank (train.py:408-416)."""
-    check_sampling(getattr(args, 'sampling_rate', 1.0), args.enable_pipeline, args.feat_corr, args.grad_corr)
+    rate = check_sampling(getattr(args, 'sampling_rate', 1.0), args.enable_pipeline, args.feat_corr, args.grad_corr)
+    check_halo_bits(getattr(args, 'halo_bits', None), rate)
     check_model(args)
     os.environ['MASTER_ADDR'] = args.master_addr
     os.environ['MASTER_PORT'] = '%d' % args.port
