@@ -121,6 +121,9 @@ int pg_row_div(const void* x, int64_t ldx, void* out, int64_t ldo, int32_t n_row
  * dtype_in PG_BF16 -> bf16 wgmma, PG_F32 -> tf32 wgmma; fp32 accumulation in registers;
  * dtype_out selects the element type of c.  n <= 256.  All operands row-major with 16-byte
  * aligned rows (TMA); k tails and the m tail are zero-filled / masked.  `srcs` is a HOST array.
+ * When c's rows are 16-byte aligned (base and ldc) the epilogue stores with TMA, which may also write the rest of
+ * the 16-byte vector holding column n-1 (columns [n, n rounded up to 16 bytes) of every row, never past ldc);
+ * other outputs are written exactly in columns [0, n).
  * Replaces `self.linear1(feat[0:num_dst]) + self.linear2(ah)` at
  * PipeGCN/module/layer.py:51 (two pairs: inner rows x W1, neighbour mean x W2,
  * bias = b1 + b2) and, with one pair, the dX products of its autograd (row_div = in_deg fuses the

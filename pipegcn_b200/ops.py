@@ -37,6 +37,34 @@ class DropSpec:
         return _C.pg_drop(self.p, self.seed, self.step.data_ptr() if self.step is not None else None, self.step_off)
 
 
+DROP_MUL = (0x9E3779B1, 0x85EBCA6B, 0xC2B2AE35, 0x27D4EB2F)
+
+
+def dropout_keep_host(spec: DropSpec, step, row0: int, n_rows: int, d: int, elem_size: int):
+    """Host port of csrc/common.cuh's drop_seed_hi / drop_base / drop_bits: numpy bool [n_rows, d], True where the mask
+    of `spec` keeps element (row0 + r, c) of a tensor of d columns of `elem_size`-byte elements.  `step` is the value
+    of the device counter spec.step points at, or None for a key without a counter (spec.step is None)."""
+    import numpy as np
+    M = 0xFFFFFFFF
+    u64 = np.uint64
+    thresh16 = int(np.float32(spec.p) * np.float32(65536.0) + np.float32(0.5))   # make_drop: fp32 arithmetic
+    seed_lo, seed_hi = spec.seed & M, spec.seed >> 32
+    key = seed_hi if step is None else (seed_hi + 0x632BE5AB * ((int(step) + spec.step_off + 1) & M)) & M
+    key = int(_mix32(key))
+    v = 16 // int(elem_size)
+    nvec = (int(d) + v - 1) // v
+    col = np.arange(d, dtype=np.uint64)
+    i = (np.arange(n_rows, dtype=np.uint64)[:, None] + u64(row0)) * u64(nvec) + col[None, :] // u64(v)
+    lo, hi = i & u64(M), i >> u64(32)
+    base = _mix32(((lo ^ u64(seed_lo)) + ((u64(key) + hi * u64(0x9E3779B9)) & u64(M))) & u64(M))
+    pair = (col % u64(v)) // u64(2)
+    mul = np.asarray(DROP_MUL, dtype=np.uint64)[(pair & u64(3)).astype(np.int64)]
+    h = (base * mul[None, :]) & u64(M)
+    h ^= h >> u64(16)
+    bits = np.where((col % u64(2)) == 0, h & u64(0xFFFF), h >> u64(16))
+    return bits >= u64(thresh16)
+
+
 def layer_seed(layer: int) -> int:
     """Dropout seed of graph layer `layer`: the same on every rank (all ranks seed torch identically, train.py:298)."""
     return (torch.initial_seed() * 0x9E3779B97F4A7C15 + (layer + 1) * 0xD1B54A32D192ED03) & 0xFFFFFFFFFFFFFFFF
@@ -423,17 +451,17 @@ def gemm_nt(a0, b0, a1=None, b1=None, bias=None, row_div=None, out=None, out_dty
     for a, b in pairs:
         assert a.shape[0] == m and b.shape[0] == n and a.shape[1] == b.shape[1] and a.dtype == b.dtype == a0.dtype
     if n > 256:
-        # one N tile holds at most 256 columns: split the weight rows
-        outs = [gemm_nt(raw[0][0], b0[i:i + 256], raw[1][0] if len(raw) > 1 else None,
-                        None if len(raw) == 1 else _plain(raw[1][1])[i:i + 256],
-                        None if bias is None else bias[i:i + 256], row_div, None, out_dtype)
-                for i in range(0, n, 256)]
+        # one N tile holds at most 256 columns: split the weight rows, each product writing its 256-column slice of
+        # one output (padded rows like every other output: 16-byte aligned, usable by the row kernels and TMA)
         assert drop is None or drop.p == 0, "fused dropout with n > 256 is not supported"
-        res = torch.cat(outs, dim=1)
-        if out is not None:
-            out.copy_(res)
-            return out
-        return res
+        if out is None:
+            out = alloc_rows(m, n, out_dtype or a0.dtype, a0.device)
+        assert out.shape == (m, n) and out.stride(1) == 1
+        for i in range(0, n, 256):
+            gemm_nt(raw[0][0], b0[i:i + 256], raw[1][0] if len(raw) > 1 else None,
+                    None if len(raw) == 1 else _plain(raw[1][1])[i:i + 256],
+                    None if bias is None else bias[i:i + 256], row_div, out[:, i:i + 256], out_dtype)
+        return out
     if out is None:
         out = alloc_rows(m, n, out_dtype or a0.dtype, a0.device)
     assert out.shape == (m, n) and out.stride(1) == 1

@@ -1,50 +1,29 @@
-"""CPU check (numpy) of the counter-based dropout mask of csrc/common.cuh (drop_base / drop_bits): keep rate per
+"""CPU check (numpy) of the counter-based dropout mask of csrc/common.cuh (drop_base / drop_bits, ported to
+the host as pipegcn_b200.ops.dropout_keep_host): keep rate per
 element position, correlation between the 8 elements of a 16-byte vector, between neighbouring vectors / rows,
 between epochs (the device-side step counter enters the key), and the variance of the kept count per vector.
 
     python tools/dropout_hash_quality.py            # prints one line per p; every z should be a few units at most
 """
+import sys
+from pathlib import Path
+
 import numpy as np
 
-M = np.uint64(0xffffffff)
-MUL = [0x9e3779b1, 0x85ebca6b, 0xc2b2ae35, 0x27d4eb2f]
+sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
+from pipegcn_b200.ops import DROP_MUL, DropSpec, dropout_keep_host  # noqa: E402
+
+MUL = list(DROP_MUL)          # drop_bits' per-pair multipliers (tests/test_host_logic_cpu.py checks them against the kernel)
 
 
-def u32(x):
-    return x & M
-
-
-def mix32(x):
-    x = u32(x)
-    x ^= x >> np.uint64(16)
-    x = u32(x * np.uint64(0x7feb352d))
-    x ^= x >> np.uint64(15)
-    x = u32(x * np.uint64(0x846ca68b))
-    x ^= x >> np.uint64(16)
-    return x
-
-
-def key_of(seed_hi, step):
-    return int(mix32(np.uint64((seed_hi + 0x632be5ab * (step + 1)) & 0xffffffff)))
-
-
-def masks(i, seed_lo, key, thresh16):
-    lo, hi = u32(i), i >> np.uint64(32)
-    base = mix32(u32((lo ^ np.uint64(seed_lo)) + u32(np.uint64(key) + u32(hi * np.uint64(0x9e3779b9)))))
-    cols = []
-    for k in range(4):
-        h = u32(base * np.uint64(MUL[k]))
-        h ^= h >> np.uint64(16)
-        cols.append((h & np.uint64(0xffff)) >= thresh16)
-        cols.append((h >> np.uint64(16)) >= thresh16)
-    return np.stack(cols, 1).astype(np.float64)
+def masks(n, seed, step, p):
+    """Keep mask [n, 8] of the first n 16-byte bf16 vectors (one vector per row) under the key (seed, step)."""
+    return dropout_keep_host(DropSpec(p, seed), step, 0, n, 8, 2).astype(np.float64)
 
 
 def main(n=1 << 21):
-    i = np.arange(n, dtype=np.uint64)
     for p in (0.5, 0.1, 0.3, 0.9):
-        t = np.uint64(int(p * 65536 + 0.5))
-        ms = [masks(i, 0xdeadbeef, key_of(777, e), t) for e in range(5)]
+        ms = [masks(n, (777 << 32) | 0xdeadbeef, e, p) for e in range(5)]
         m = ms[0]
         z_mean = np.abs(m.mean(0) - (1 - p)).max() / np.sqrt(p * (1 - p) / n)
         c = np.corrcoef(m.T)
