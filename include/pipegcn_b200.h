@@ -399,6 +399,30 @@ int pg_gat_colsum(const void* x, int64_t ldx, int32_t n_rows, int32_t H, int32_t
                   float* out, float* partial, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Max-pool GraphSAGE (DGL SAGEConv(aggregator_type='pool')) over the `_U` rows [inner | halo] of one partition.
+ * Q [num_all, d] (fp32 or bf16, `dtype`) is the pooled transform h Wp^T + bp.  For the in-edges u -> v of the forward
+ * CSR g (each edge once):
+ *   M[v, c] = max_u Q[u, c],  A[v, c] = the u that gives it,  hn[v, c] = ReLU(M[v, c])
+ * A tie goes to the first source in CSR order; the first NaN source becomes the value and the argmax; a row without
+ * in-edges gets hn = 0 and A = -1.  A holds int32 `_U` row ids (bit 31 of pg_csr::pidx stripped).  Rows of q, hn, A,
+ * grad and gq start on 16-byte boundaries with strides that are multiples of 16 bytes, covering the last 16-byte
+ * vector of a row of q, A and grad (the padded rows of the activations).  The plans must carry the chunk table
+ * (pg_csr::chunks); scratch is fp32 [n_seg][ld_scratch] (may be NULL when n_seg == 0).  No atomics: the results are the
+ * same bits from run to run.
+ * ---------------------------------------------------------------------------------------- */
+/* loads every pool kernel (call it before any halo wait can spin: a first launch may wait for the device) */
+int pg_pool_preload(void);
+/* hn [N_in, d] (activation dtype) and A [N_in, d] int32 over the forward CSR g; ld_scratch >= 2 d */
+int pg_max_aggregate(const pg_csr* g, const void* q, int64_t ldq, int32_t d, int dtype, void* hn, int64_t ldh,
+                     int32_t* arg, int64_t lda, float* scratch, int64_t ld_scratch, void* stream);
+/* gq[u, c] = [Q[u, c] > 0] * sum over the destinations v of CSC row u (gt = the transposed plan, rows = all num_all
+ * `_U` rows) with A[v, c] == u of grad[v, c], accumulated in fp32 in CSC order and stored in the activation dtype;
+ * a row without out-edges gets 0.  grad = dL/d hn [N_in, d]; ld_scratch >= d */
+int pg_max_aggregate_bwd(const pg_csr* gt, const void* q, int64_t ldq, const int32_t* arg, int64_t lda,
+                         const void* grad, int64_t ldg, int32_t d, int dtype, void* gq, int64_t ldgq, float* scratch,
+                         int64_t ld_scratch, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Symmetric heap: device memory that peers map through CUDA IPC (host pointers out).
  * ---------------------------------------------------------------------------------------- */
 #define PG_IPC_HANDLE_BYTES 64

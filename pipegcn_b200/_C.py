@@ -113,6 +113,10 @@ def _load():
                                      vp, vp, vp, i32, vp, i64, vp, vp, vp]),
         "pg_gat_colsum_blocks": (C.c_int, [i32]),
         "pg_gat_colsum": (C.c_int, [vp, i64, i32, i32, i32, C.c_int, vp, vp, vp, vp]),
+        "pg_pool_preload": (C.c_int, []),
+        "pg_max_aggregate": (C.c_int, [C.POINTER(pg_csr), vp, i64, i32, C.c_int, vp, i64, vp, i64, vp, i64, vp]),
+        "pg_max_aggregate_bwd": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, vp, i64, i32, C.c_int, vp, i64, vp,
+                                           i64, vp]),
         "pg_heap_alloc": (C.c_int, [C.c_size_t, C.POINTER(vp)]),
         "pg_heap_free": (C.c_int, [vp]),
         "pg_ipc_export": (C.c_int, [vp, C.c_char_p]),

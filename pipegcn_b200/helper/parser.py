@@ -25,6 +25,11 @@ forward and gradients backward: every row travels as b-bit codes with an fp32 (l
 the message stays unbiased, and the receiver decodes it before anything reads it.  Layer 0, --use-pp and the
 evaluation exchange stay exact; it cannot be combined with --sampling-rate p < 1.  Suppressed like `--sampling-rate`:
 read it with getattr(args, 'halo_bits', None).
+
+`--aggregator {mean,pool}` (not in the reference) selects the neighbour reduction of the GraphSAGE layers: `mean` (the
+reference's) or `pool`, Hamilton et al.'s max-pool aggregator (DGL `SAGEConv(aggregator_type='pool')`): every layer
+takes the element-wise neighbour maximum of ReLU(h Wp^T + bp).  It cannot be combined with --model gat or --use-pp.
+Suppressed like `--sampling-rate`: read it with getattr(args, 'aggregator', 'mean').
 """
 import argparse
 
@@ -110,6 +115,8 @@ def build_parser():
     parser.add_argument('--halo-bits', '--halo_bits', type=int, choices=[8, 4], default=argparse.SUPPRESS,
                         help="send the halo messages of graph layers >= 1 as stochastically rounded 8- or 4-bit codes "
                              "(default: exact)")
+    parser.add_argument('--aggregator', choices=['mean', 'pool'], default=argparse.SUPPRESS,
+                        help="GraphSAGE neighbour aggregator: mean (default) or pool (max over ReLU(h Wp^T + bp))")
     return parser
 
 

@@ -8,6 +8,13 @@ weights).  `graph` is a `pipegcn_b200.graph.PartGraph` instead of a DGL heterogr
     training:  out = feat[:N_in] @ W1^T + b1 + ((A @ feat) / in_deg) @ W2^T + b2      (layer.py:44-51)
     eval:      same on a homogeneous graph, degrees taken from the graph               (layer.py:52-62)
 
+`aggregator='pool'` (not in the reference): the max-pool aggregator of DGL's `SAGEConv(aggregator_type='pool')`, with
+a third linear `pool` [d_in, d_in] (state-dict keys `pool.weight` / `pool.bias`, drawn after linear1 and linear2):
+
+    out = feat[:N_in] @ W1^T + b1 + ReLU(max_{u -> v} (feat[u] @ Wp^T + bp)) @ W2^T + b2
+
+the same in training and evaluation (a row without in-edges aggregates to 0).
+
 `GATLayer` (not in the reference): DGL's `GATConv` with feat_drop = attn_drop = 0, no residual, negative_slope 0.2,
 over the `[inner | halo]` rows h the halo exchange returns (inner rows v, in-edges u -> v, per head):
 
@@ -26,18 +33,27 @@ from .. import ops
 
 class GraphSAGELayer(nn.Module):
 
-    def __init__(self, in_feats, out_feats, bias=True, use_pp=False):
+    def __init__(self, in_feats, out_feats, bias=True, use_pp=False, aggregator='mean'):
         super().__init__()
         self.in_feats, self.out_feats, self.use_pp = in_feats, out_feats, use_pp
+        if aggregator not in ('mean', 'pool'):
+            raise ValueError(f"aggregator '{aggregator}': expected 'mean' or 'pool'")
+        if aggregator == 'pool' and use_pp:
+            raise NotImplementedError("the pool aggregator with use_pp: the precompute is a neighbour mean")
+        self.aggregator = aggregator
         if use_pp:
             self.linear = nn.Linear(2 * in_feats, out_feats, bias=bias)
         else:
             self.linear1 = nn.Linear(in_feats, out_feats, bias=bias)
             self.linear2 = nn.Linear(in_feats, out_feats, bias=bias)
+        if aggregator == 'pool':
+            self.pool = nn.Linear(in_feats, in_feats, bias=bias)
         self.reset_parameters()
 
     def _linears(self):
-        return [self.linear] if self.use_pp else [self.linear1, self.linear2]
+        if self.use_pp:
+            return [self.linear]
+        return [self.linear1, self.linear2] + ([self.pool] if self.aggregator == 'pool' else [])
 
     def reset_parameters(self):
         lins = self._linears()
@@ -51,7 +67,12 @@ class GraphSAGELayer(nn.Module):
 
     def forward(self, graph, feat, in_deg, drop_bwd=None):
         """`drop_bwd` (not in the reference): `feat` is already dropout(F) under that key -- the layer's gradient with
-        respect to F then includes the dropout backward (fused into the transposed aggregate's store)."""
+        respect to F then includes the dropout backward (fused into the transposed aggregate's store).  A pool layer
+        takes the keep mask of the halo rows (boundary-node sampling, uint8) or None in place of `in_deg`."""
+        if self.aggregator == 'pool':
+            return ops.sage_pool_layer(feat, graph, in_deg if self.training else None, self.linear1.weight,
+                                       self.linear1.bias, self.linear2.weight, self.linear2.bias, self.pool.weight,
+                                       self.pool.bias, drop_bwd)
         if self.training:
             if self.use_pp:
                 return ops.linear(feat, self.linear.weight, self.linear.bias)

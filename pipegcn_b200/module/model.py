@@ -10,6 +10,10 @@ instead of the process-global `helper.context.buffer` (several simulated ranks i
 process); `dtype` -- activation storage type, float32 (reference) or bfloat16 (fp32
 accumulate, fp32 master weights).
 
+`aggregator='pool'` (not in the reference) builds max-pool GraphSAGE layers (DGL SAGEConv(aggregator_type='pool'),
+module/layer.py); with boundary-node sampling they take the buffer's keep mask of the halo rows in place of the
+in-degrees, and zero the pooled transform of the unkept rows before the maximum.
+
 `GAT` (not in the reference) is the same layer loop with `GATLayer`s: every graph layer whose output feeds another
 layer concatenates `n_heads` heads of d_out / n_heads columns, a graph layer that produces the logits has one head.  The
 exchange moves the layer input h, so pipelining, the corrections, the static layer-0 store and the fused dropout apply
@@ -43,8 +47,13 @@ class GNNBase(nn.Module):
 class GraphSAGE(GNNBase):
 
     def __init__(self, layer_size, activation, use_pp, dropout=0.5, norm='layer', train_size=None, n_linear=0,
-                 buffer=None, dtype=torch.float32):
+                 buffer=None, dtype=torch.float32, aggregator='mean'):
         super().__init__(layer_size, activation, use_pp, dropout, norm, n_linear)
+        if aggregator not in ('mean', 'pool'):
+            raise ValueError(f"aggregator '{aggregator}': expected 'mean' or 'pool'")
+        if aggregator == 'pool' and use_pp:
+            raise NotImplementedError("the pool aggregator with use_pp: the precompute is a neighbour mean")
+        self.aggregator = aggregator
         self.buffer = buffer
         self.act_dtype = dtype
         for i, (d_in, d_out) in enumerate(zip(layer_size[:-1], layer_size[1:])):
@@ -62,10 +71,16 @@ class GraphSAGE(GNNBase):
                     raise ValueError(f"unknown norm '{norm}'")
 
     def _graph_layer(self, i, d_in, d_out):
+        if self.aggregator == 'pool':
+            return GraphSAGELayer(d_in, d_out, aggregator='pool')
         return GraphSAGELayer(d_in, d_out, use_pp=(self.use_pp and i == 0))
 
     def _layer_arg(self, in_deg):
-        """The third argument of every graph layer in training: the in-degrees."""
+        """The third argument of every graph layer in training: the in-degrees, or for pool layers the keep mask of
+        this epoch's boundary-node sample (training with sampling), else None."""
+        if self.aggregator == 'pool':
+            buf = self._buffer() if self.training else None
+            return getattr(buf, 'keep_mask', None) if buf is not None else None
         return in_deg
 
     def _drop(self, h):
@@ -104,6 +119,8 @@ class GraphSAGE(GNNBase):
 
     def forward(self, g, feat, in_deg=None):
         from .. import ops
+        if self.aggregator == 'pool':
+            ops.pool_preload()
         h = feat if feat.dtype == self.act_dtype else feat.to(self.act_dtype)
         p = self.dropout.p if self.training else 0.0
         in_deg = self._layer_arg(in_deg)
@@ -141,6 +158,8 @@ class GraphSAGE(GNNBase):
         cat(feat, neighbour mean) of the inner rows.  Returns the logits [N_in, C]."""
         from .. import ops
         assert not self.training
+        if self.aggregator == 'pool':
+            ops.pool_preload()
         h = None
         for i, layer in enumerate(self.layers):
             if i < self.n_graph_layers:

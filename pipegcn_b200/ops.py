@@ -875,6 +875,121 @@ def gat_layer(feat, graph, keep, heads, weight, attn_l, attn_r, bias, drop_bwd=N
     return GatLayerFn.apply(feat, graph, keep, int(heads), weight, attn_l, attn_r, bias, drop_bwd)
 
 
+# ---- max-pool GraphSAGE (csrc/pool.cu) ---------------------------------------------------------------------
+def pool_preload():
+    """Load every pool kernel now (see gat_preload)."""
+    _C.check(_C.lib.pg_pool_preload(), "pg_pool_preload")
+
+
+def _scratch_ld(d: int) -> int:
+    return (int(d) + 7) // 8 * 8
+
+
+def max_aggregate(plan: CsrPlan, q: torch.Tensor):
+    """(hn, A) over the forward CSR `plan`: hn [n_rows, d] = ReLU(max over the in-edges u -> v of q[u]) in q's dtype
+    (0 for a row without in-edges), A [n_rows, d] int32 = the u of that maximum (the first in CSR order on a tie, -1
+    for a row without in-edges)."""
+    _rows(q)
+    d = q.shape[1]
+    hn = alloc_rows(plan.n_rows, d, q.dtype, q.device)
+    arg = alloc_rows(plan.n_rows, d, torch.int32, q.device)
+    ld_s = _scratch_ld(2 * d)
+    scratch = plan.scratch(2 * d)
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_max_aggregate(C.byref(plan.c), q.data_ptr(), q.stride(0), d, _C.dtype_code(q.dtype),
+                                     hn.data_ptr(), hn.stride(0), arg.data_ptr(), arg.stride(0), _ptr(scratch), ld_s,
+                                     _C.stream_ptr()), "pg_max_aggregate")
+    return hn, arg
+
+
+def max_aggregate_bwd(plan_t: CsrPlan, q: torch.Tensor, arg: torch.Tensor, g: torch.Tensor) -> torch.Tensor:
+    """gq [plan_t.n_rows, d] in q's dtype: gq[u, c] = [q[u, c] > 0] * sum over the CSC row u of `plan_t` of g[v, c]
+    where arg[v, c] == u, accumulated in fp32 in CSC order."""
+    _rows(q), _rows(arg), _rows(g)
+    d = q.shape[1]
+    assert g.dtype == q.dtype and arg.dtype == torch.int32 and g.shape[1] == d and arg.shape == g.shape
+    gq = alloc_rows(plan_t.n_rows, d, q.dtype, q.device)
+    scratch = plan_t.scratch(d)
+    _C.count(2 if plan_t.n_long else 1)
+    _C.check(_C.lib.pg_max_aggregate_bwd(C.byref(plan_t.c), q.data_ptr(), q.stride(0), arg.data_ptr(), arg.stride(0),
+                                         g.data_ptr(), g.stride(0), d, _C.dtype_code(q.dtype), gq.data_ptr(),
+                                         gq.stride(0), _ptr(scratch), _scratch_ld(d), _C.stream_ptr()),
+             "pg_max_aggregate_bwd")
+    return gq
+
+
+class SagePoolLayerFn(torch.autograd.Function):
+    """One max-pool GraphSAGE layer (DGL SAGEConv(aggregator_type='pool')) over the [inner | halo] rows `feat` of a
+    partition, returning the inner rows:
+
+        Q   = feat @ Wp^T + bp                           [num_all, d_in]  pg_linear over all rows
+        hn  = ReLU(max_{u -> v} Q[u]), A = its argmax    [N_in, d_in]     pg_max_aggregate
+        out = feat[:N_in] @ W1^T + hn @ W2^T + (b1 + b2) [N_in, d_out]    pg_linear, two sources
+
+    ReLU(max Q) = max ReLU(Q) exactly, so the ReLU is the aggregate's store.  Backward: g_neigh = g @ W2 (pg_linear),
+    gQ = [Q > 0] * the g_neigh of the destinations whose argmax is u (pg_max_aggregate_bwd over the CSC),
+    g_feat = g @ W1 + gQ @ Wp (one two-source pg_linear on the inner rows, gQ @ Wp on the halo rows, the dropout
+    backward of `drop_bwd` in their epilogues), dW1 = g^T feat[:N_in], dW2 = g^T hn, dWp = gQ^T feat (pg_wgrad),
+    dbp = colsum(gQ).  `keep`: the boundary-node sample of the halo rows (uint8) or None; an unkept halo row's Q is
+    zeroed, so it can win only where the output is 0, and gets no gradient."""
+
+    @staticmethod
+    def forward(ctx, feat, graph, keep, w1, b1, w2, b2, wp, bp, drop_bwd=None):
+        ctx.drop_bwd = drop_bwd
+        if feat.stride(1) != 1:
+            feat = feat.contiguous()
+        n_in = graph.num_in
+        fsp = presplit(feat)                   # fp32: one split of feat for both products
+        q = gemm_nt(fsp, padded_weight(wp, feat.dtype), bias=bp)
+        if keep is not None and feat.shape[0] > n_in:
+            bns_mask_rows(keep, q[n_in:])
+        hn, arg = max_aggregate(graph.fwd, q)
+        bias = None
+        if b1 is not None:
+            bias = b1.detach().float() + b2.detach().float()
+        out = gemm_nt(fsp.rows(0, n_in) if isinstance(fsp, Split) else feat[:n_in], padded_weight(w1, feat.dtype),
+                      hn, padded_weight(w2, feat.dtype), bias=bias)
+        ctx.graph = graph
+        ctx.has_bias, ctx.has_pbias = b1 is not None, bp is not None
+        ctx.save_for_backward(feat, q, arg, hn, w1, w2, wp)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        feat, q, arg, hn, w1, w2, wp = ctx.saved_tensors
+        graph = ctx.graph
+        n_in = graph.num_in
+        colsum = _take_colsum(g)
+        g = _tma_ready(g if g.dtype == feat.dtype else g.to(feat.dtype))
+        gsp = presplit(g)                      # fp32: one split of g serves g_neigh, the g_feat product and dW1 / dW2
+        g_neigh = gemm_nt(gsp, padded_weight(w2, feat.dtype, transpose=True))
+        gq = max_aggregate_bwd(graph.bwd, q, arg, g_neigh)
+        gqsp = presplit(gq)
+        is_split = isinstance(gqsp, Split)
+        g_feat = None
+        if ctx.needs_input_grad[0]:
+            g_feat = alloc_rows(feat.shape[0], feat.shape[1], feat.dtype, feat.device)
+            wpt = padded_weight(wp, feat.dtype, transpose=True)
+            drop = ctx.drop_bwd if ctx.drop_bwd is not None and ctx.drop_bwd.p > 0 else None
+            db = drop if drop is not None and feat.shape[1] <= 256 and _drop_ok(g_feat) else None
+            gemm_nt(gsp, padded_weight(w1, feat.dtype, transpose=True), gqsp.rows(0, n_in) if is_split else gq[:n_in],
+                    wpt, out=g_feat[:n_in], drop=db)
+            if feat.shape[0] > n_in:
+                gemm_nt(gqsp.rows(n_in) if is_split else gq[n_in:], wpt, out=g_feat[n_in:], drop=db, drop_row0=n_in)
+            if drop is not None and db is None:
+                dropout_rows(g_feat, drop, out=g_feat)
+        gw1 = wgrad(gsp, feat[:n_in]).to(w1.dtype)
+        gw2 = wgrad(gsp, hn).to(w2.dtype)
+        gwp = wgrad(gqsp, feat).to(wp.dtype)
+        gb = (colsum if colsum is not None else g.float().sum(0)) if ctx.has_bias else None
+        gbp = gat_colsum(gq) if ctx.has_pbias else None
+        return g_feat, None, None, gw1, gb, gw2, gb, gwp, gbp, None
+
+
+def sage_pool_layer(feat, graph, keep, w1, b1, w2, b2, wp, bp, drop_bwd=None) -> torch.Tensor:
+    return SagePoolLayerFn.apply(feat, graph, keep, w1, b1, w2, b2, wp, bp, drop_bwd)
+
+
 # ---- row-wise epilogues (csrc/rowops.cu) -------------------------------------------------------------------
 # column sums of a gradient tensor computed as a by-product by the kernel that produced it, keyed by the
 # tensor's address: the bias gradient of the linear upstream (saves a full pass over [N, d])

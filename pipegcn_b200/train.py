@@ -47,8 +47,17 @@ def _quant_seed(args):
 
 
 def check_model(args):
-    """Refuses, before anything is allocated, a --model gat configuration that is not implemented: --use-pp (the
-    precompute is GraphSAGE's neighbour mean) and a hidden width that does not split into --n-heads heads."""
+    """Refuses, before anything is allocated, a configuration that is not implemented: --model gat with --use-pp (the
+    precompute is GraphSAGE's neighbour mean) or with a hidden width that does not split into --n-heads heads, and
+    --aggregator pool with --model gat (an attention layer has no aggregator) or with --use-pp (a neighbour mean)."""
+    aggregator = getattr(args, 'aggregator', 'mean')
+    if aggregator not in ('mean', 'pool'):
+        raise ValueError(f"--aggregator {aggregator}: expected mean or pool")
+    if aggregator == 'pool':
+        if args.model == 'gat':
+            raise ValueError("--aggregator pool is a GraphSAGE aggregator; --model gat has none")
+        if args.use_pp:
+            raise NotImplementedError("--aggregator pool with --use-pp: the precompute is a neighbour mean")
     if args.model != 'gat':
         return
     if args.use_pp:
@@ -59,11 +68,13 @@ def check_model(args):
 
 
 def create_model(layer_size, args, buffer=None, dtype=torch.float32):
+    check_model(args)
     if args.model in ('graphsage', 'gcn'):
+        aggregator = getattr(args, 'aggregator', 'mean')
+        kw = {} if aggregator == 'mean' else dict(aggregator=aggregator)
         return GraphSAGE(layer_size, F.relu, args.use_pp, norm=args.norm, dropout=args.dropout,
-                         n_linear=args.n_linear, train_size=args.n_train, buffer=buffer, dtype=dtype)
+                         n_linear=args.n_linear, train_size=args.n_train, buffer=buffer, dtype=dtype, **kw)
     if args.model == 'gat':
-        check_model(args)
         return GAT(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
                    train_size=args.n_train, buffer=buffer, dtype=dtype, n_heads=getattr(args, 'n_heads', 4))
     raise NotImplementedError(args.model)
