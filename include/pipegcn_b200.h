@@ -399,6 +399,37 @@ int pg_gat_colsum(const void* x, int64_t ldx, int32_t n_rows, int32_t H, int32_t
                   float* out, float* partial, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Dynamic graph attention (GATv2, DGL GATv2Conv with share_weights=False, negative_slope 0.2, no attention dropout)
+ * over the `_U` rows [inner | halo] of one partition.  zs [num_all, H * D] and zd [N_in, H * D] (fp32 or bf16,
+ * `dtype`) are the source and destination transforms, attn fp32 [H * D]; for the in-edges u -> v of the forward CSR,
+ * per head k:
+ *   t_uv = zs[u, k] + zd[v, k],  e_uv = <attn[k], LeakyReLU(t_uv)>,  a_uv = softmax over u of e_uv,
+ *   out[v, k] = sum_u a_uv zs[u, k]      (a row without a kept in-edge gets 0)
+ * `keep` and the chunk-table plan as for pg_gat_*; fp32 accumulation, no atomics, no per-edge storage, D <= 512; the
+ * results are the same bits from run to run.  Scratch (fp32, may be NULL when n_seg == 0): n_seg * H * (D + 2) floats
+ * for the aggregate, n_seg * H * (4 D + 1) for the destination pass, n_seg * H * D for the source pass.
+ * ---------------------------------------------------------------------------------------- */
+int pg_gatv2_preload(void);
+/* out (activation dtype) and the softmax statistics m (maximum), s (sum of exp(e - m)), fp32 [N_in, H] */
+int pg_gatv2_aggregate(const pg_csr* g, const void* zs, int64_t ldzs, const void* zd, int64_t ldzd, int32_t H,
+                       int32_t D, int dtype, const float* attn, const uint8_t* keep, int32_t num_in, void* out,
+                       int64_t ldo, float* m, float* s, float* scratch, void* stream);
+/* backward over the forward CSR, grad = dL/d out, dot_uv = <grad[v, k], zs[u, k]>:
+ *   dv[v, k] = D_v = sum_u a_uv dot_uv,  de_uv = a_uv (dot_uv - D_v)
+ *   dzd[v, k] = sum_u de_uv attn[k] ⊙ LeakyReLU'(t_uv)                 (activation dtype)
+ *   pattn[v, k] = sum_u de_uv LeakyReLU(t_uv)  (fp32 [N_in, H * D], row stride ldp: d attn is its column sum) */
+int pg_gatv2_bwd_dst(const pg_csr* g, const void* zs, int64_t ldzs, const void* zd, int64_t ldzd, const void* grad,
+                     int64_t ldg, int32_t H, int32_t D, int dtype, const float* attn, const float* m, const float* s,
+                     const uint8_t* keep, int32_t num_in, void* dzd, int64_t lddzd, float* dv, float* pattn,
+                     int64_t ldp, float* scratch, void* stream);
+/* backward over the CSC gt (rows = all `_U` rows u, columns = destinations v):
+ *   dzs[u, k] = sum_v a_uv grad[v, k] + de_uv attn[k] ⊙ LeakyReLU'(t_uv)   (activation dtype; unkept halo rows: 0) */
+int pg_gatv2_bwd_src(const pg_csr* gt, const void* zs, int64_t ldzs, const void* zd, int64_t ldzd, const void* grad,
+                     int64_t ldg, int32_t H, int32_t D, int dtype, const float* attn, const float* m, const float* s,
+                     const float* dv, const uint8_t* keep, int32_t num_in, void* dzs, int64_t lddzs, float* scratch,
+                     void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Max-pool GraphSAGE (DGL SAGEConv(aggregator_type='pool')) over the `_U` rows [inner | halo] of one partition.
  * Q [num_all, d] (fp32 or bf16, `dtype`) is the pooled transform h Wp^T + bp.  For the in-edges u -> v of the forward
  * CSR g (each edge once):

@@ -1,5 +1,6 @@
 // Graph attention (GAT, DGL GATConv semantics) on sm_90a: attention scores, the edge-softmax aggregate and its two
-// backward passes, and the fixed-order column reductions of the attention-vector gradients.
+// backward passes, and the fixed-order column reductions of the attention-vector gradients.  The GATv2 (GATv2Conv)
+// aggregate and its two backward passes share the chunk walk, the keep test and the forward fix-up (section GATv2).
 //
 // One warp owns one (row, head) pair: lane l holds the columns l, l + 32, ... of the head's D columns, so every
 // per-head dot product is one warp butterfly (all lanes end with the same bits: IEEE addition commutes).  Edges are
@@ -476,6 +477,413 @@ int colsum_blocks(int32_t n_rows) {
   return static_cast<int>(std::max<int64_t>(1, std::min<int64_t>((n_rows + 255) / 256, 2 * sm_count())));
 }
 
+// ---------------------------------------------------------------------------------------------------- GATv2
+// GATv2Conv: e_uv = <attn[k], LeakyReLU(zs[u, k] + zd[v, k])>.  The score is no longer two per-node scalars, so every
+// edge needs a D-wide sum in the forward and in both backward passes.  A warp still owns one (row, head) pair with lane
+// l holding the columns l, l + 32, ..., but it takes E edges at a time: E row gathers in flight, and the per-lane
+// partial sums of all of them reduced together by warp_sum_n (2E values in 4E - 1 + log2(32 / 2E) shuffles instead
+// of 10E).  Every sum is taken over warp_sum's tree (offsets 16, 8, 4, 2, 1; IEEE addition commutes), so a score or a
+// dot has the same bits in every pass and in every slot of a batch: the backward recomputes a_uv exactly.
+// edges in flight per warp: the most that every pass compiles with at NJ columns per lane without local-memory spills
+template <int NJ> __host__ __device__ constexpr int v2_edges() { return NJ <= 2 ? 2 : NJ <= 4 ? 4 : NJ <= 8 ? 2 : 1; }
+
+// x[i] <- the warp sum of x[i], on every lane (N a power of two <= 32)
+template <int N>
+__device__ __forceinline__ void warp_sum_n(float (&x)[N], int lane) {
+  // step o keeps half of the live values: the half selected by lane bit o, plus the partner's copy of the same half
+#pragma unroll
+  for (int n = N, o = 16; n > 1; n >>= 1, o >>= 1) {
+    const bool hi = (lane & o) != 0;
+#pragma unroll
+    for (int i = 0; i < n / 2; ++i) {
+      const float send = hi ? x[i] : x[i + n / 2];
+      const float own = hi ? x[i + n / 2] : x[i];
+      x[i] = own + __shfl_xor_sync(0xffffffffu, send, o);
+    }
+  }
+#pragma unroll
+  for (int o = 16 / N; o > 0; o >>= 1) x[0] += __shfl_xor_sync(0xffffffffu, x[0], o);
+  // value t now sits on the lanes whose bit o of every halving step is bit n / 2 of t
+  const float r = x[0];
+#pragma unroll
+  for (int t = 0; t < N; ++t) {
+    int src = 0;
+#pragma unroll
+    for (int n = N, o = 16; n > 1; n >>= 1, o >>= 1) src |= (t & (n / 2)) ? o : 0;
+    x[t] = __shfl_sync(0xffffffffu, r, src);
+  }
+}
+
+__device__ __forceinline__ float lrelu(float x) { return x > 0.f ? x : x * kNegSlope; }
+
+// the D columns of head k of one row: lane l takes l, l + 32, ... (0 past D)
+template <typename T, int NJ>
+__device__ __forceinline__ void load_head(const T* row, int D, int lane, float (&r)[NJ]) {
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int col = lane + 32 * j;
+    r[j] = col < D ? ldf(row + col) : 0.f;
+  }
+}
+template <int NJ>
+__device__ __forceinline__ void load_head_f32(const float* row, int D, int lane, float (&r)[NJ]) {
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int col = lane + 32 * j;
+    r[j] = col < D ? row[col] : 0.f;
+  }
+}
+
+// the per-lane partial of <attn, LeakyReLU(zs_u + zd_v)> (zs_u + zd_v in that order in every pass)
+template <int NJ>
+__device__ __forceinline__ float score_part(const float (&zs)[NJ], const float (&zd)[NJ], const float (&at)[NJ]) {
+  float p = 0.f;
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) p = fmaf(at[j], lrelu(zs[j] + zd[j]), p);
+  return p;
+}
+
+// the per-lane partial of <g_v, zs_u>
+template <int NJ>
+__device__ __forceinline__ float dot_part(const float (&g)[NJ], const float (&zs)[NJ]) {
+  float p = 0.f;
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) p = fmaf(g[j], zs[j], p);
+  return p;
+}
+
+struct V2Args {
+  Walk w;
+  const void* zs; int64_t ldzs;           // [num_all, H * D]
+  const void* zd; int64_t ldzd;           // [N_in, H * D]
+  const void* g; int64_t ldg;             // backward: dL/d out [N_in, H * D]
+  const float* attn;                      // [H * D]
+  const float* m; const float* s;         // [N_in, H]
+  const float* dv;                        // source pass: D_v [N_in, H]
+  const uint8_t* keep; int32_t num_in;
+  void* out; int64_t ldo;                 // forward: out; destination pass: d zd; source pass: d zs
+  float* m_out; float* s_out;             // forward
+  float* dv_out; float* pattn; int64_t ldp;  // destination pass
+  float* scratch;
+  int32_t H, D;
+};
+
+// the forward's (m, s, acc) partials and their fix-up are GAT's (FwdArgs, gat_fwd_fixup_kernel, no bias)
+__host__ __device__ FwdArgs v2_fwd_args(const V2Args& a) {
+  return FwdArgs{a.w, a.zs, a.ldzs, nullptr, nullptr, nullptr, a.keep, a.num_in, a.out, a.ldo, a.m_out, a.s_out,
+                 a.scratch, a.H, a.D};
+}
+
+// online softmax of one row (or segment) for head k, E in-edges at a time
+template <typename T, int NJ>
+__device__ __forceinline__ void v2_fwd_row(const V2Args& a, const FwdArgs& f, int v, int e0, int n, int slot, int k,
+                                           int lane) {
+  constexpr int E = v2_edges<NJ>();
+  const int D = a.D;
+  const T* zs = static_cast<const T*>(a.zs) + static_cast<int64_t>(k) * D;
+  float zdv[NJ], at[NJ], acc[NJ];
+  load_head<T, NJ>(static_cast<const T*>(a.zd) + static_cast<int64_t>(v) * a.ldzd + static_cast<int64_t>(k) * D, D,
+                   lane, zdv);
+  load_head_f32<NJ>(a.attn + k * D, D, lane, at);
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) acc[j] = 0.f;
+  float m = -INFINITY, s = 0.f;
+  for (int b = 0; b < n; b += E) {
+    int u[E];
+    float x[E][NJ], p[E];
+#pragma unroll
+    for (int t = 0; t < E; ++t) {
+      u[t] = -1;
+      if (b + t < n) {
+        const int ut = a.w.pidx[e0 + b + t] & kColMask;
+        if (is_kept(a.keep, a.num_in, ut)) u[t] = ut;
+      }
+    }
+#pragma unroll
+    for (int t = 0; t < E; ++t) {
+      if (u[t] >= 0) {
+        load_head<T, NJ>(zs + static_cast<int64_t>(u[t]) * a.ldzs, D, lane, x[t]);
+      } else {
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) x[t][j] = 0.f;
+      }
+    }
+#pragma unroll
+    for (int t = 0; t < E; ++t) p[t] = score_part<NJ>(x[t], zdv, at);
+    warp_sum_n<E>(p, lane);
+    float bm = -INFINITY;
+#pragma unroll
+    for (int t = 0; t < E; ++t) if (u[t] >= 0) bm = fmaxf(bm, p[t]);
+    if (bm == -INFINITY) continue;            // warp-uniform: no kept source in this batch
+    const float mn = fmaxf(m, bm);
+    const float sc = expf(m - mn);
+    s *= sc;
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) acc[j] *= sc;
+#pragma unroll
+    for (int t = 0; t < E; ++t) {
+      if (u[t] < 0) continue;
+      const float pt = expf(p[t] - mn);
+      s += pt;
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) acc[j] = fmaf(pt, x[t][j], acc[j]);
+    }
+    m = mn;
+  }
+  if (slot < 0) {
+    fwd_store<T, NJ>(f, v, k, lane, m, s, acc);
+  } else {
+    float* p = a.scratch + (static_cast<int64_t>(slot) * a.H + k) * (D + 2);
+    if (lane == 0) { p[0] = m; p[1] = s; }
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int col = lane + 32 * j;
+      if (col < D) p[2 + col] = acc[j];
+    }
+  }
+}
+
+template <typename T, int NJ>
+// no __launch_bounds__: with it ptxas spills the bf16 NJ = 4 instance (launched with kGatWarps * 32 threads as well)
+__global__ void gatv2_fwd_kernel(V2Args a) {
+  const int lane = threadIdx.x & 31;
+  const int c = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (c >= a.w.n_chunks) return;
+  const FwdArgs f = v2_fwd_args(a);
+  walk_chunk(a.w, c, [&](int v, int e0, int n, int slot) { v2_fwd_row<T, NJ>(a, f, v, e0, n, slot, k, lane); });
+}
+
+// destination pass results of row v, head k from the sums over its in-edges (the weights w = a_uv, ad = a_uv dot_uv):
+//   sd = D_v = sum ad,  A = sum ad σ',  B = sum w σ',  C = sum ad LeakyReLU(t),  Q = sum w LeakyReLU(t)  (per column)
+//   d zd = attn (A - D_v B),  d attn contribution = C - D_v Q,  since de_uv = a_uv dot_uv - a_uv D_v
+template <typename T, int NJ>
+__device__ __forceinline__ void v2_dst_store(const V2Args& a, int v, int k, int lane, float sd, const float (&A)[NJ],
+                                             const float (&B)[NJ], const float (&C)[NJ], const float (&Q)[NJ]) {
+  const int D = a.D;
+  T* o = static_cast<T*>(a.out) + static_cast<int64_t>(v) * a.ldo + static_cast<int64_t>(k) * D;
+  float* pa = a.pattn + static_cast<int64_t>(v) * a.ldp + static_cast<int64_t>(k) * D;
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int col = lane + 32 * j;
+    if (col < D) {
+      o[col] = from_f<T>(a.attn[k * D + col] * fmaf(-sd, B[j], A[j]));
+      pa[col] = fmaf(-sd, Q[j], C[j]);
+    }
+  }
+  if (lane == 0) a.dv_out[static_cast<int64_t>(v) * a.H + k] = sd;
+}
+
+// scratch of a long-row segment: [H][4 D + 1] = (sd, A[D], B[D], C[D], Q[D])
+template <typename T, int NJ>
+__device__ __forceinline__ void v2_dst_row(const V2Args& a, int v, int e0, int n, int slot, int k, int lane) {
+  constexpr int E = v2_edges<NJ>();
+  const int D = a.D;
+  const T* zs = static_cast<const T*>(a.zs) + static_cast<int64_t>(k) * D;
+  float zdv[NJ], at[NJ], gv[NJ], A[NJ], B[NJ], C[NJ], Q[NJ];
+  load_head<T, NJ>(static_cast<const T*>(a.zd) + static_cast<int64_t>(v) * a.ldzd + static_cast<int64_t>(k) * D, D,
+                   lane, zdv);
+  load_head<T, NJ>(static_cast<const T*>(a.g) + static_cast<int64_t>(v) * a.ldg + static_cast<int64_t>(k) * D, D,
+                   lane, gv);
+  load_head_f32<NJ>(a.attn + k * D, D, lane, at);
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) { A[j] = 0.f; B[j] = 0.f; C[j] = 0.f; Q[j] = 0.f; }
+  float sd = 0.f;
+  const int64_t vk = static_cast<int64_t>(v) * a.H + k;
+  const float mv = a.m[vk], sv = a.s[vk];
+  for (int b = 0; sv > 0.f && b < n; b += E) {
+    int u[E];
+    float x[E][NJ], p[2 * E];
+#pragma unroll
+    for (int t = 0; t < E; ++t) {
+      u[t] = -1;
+      if (b + t < n) {
+        const int ut = a.w.pidx[e0 + b + t] & kColMask;
+        if (is_kept(a.keep, a.num_in, ut)) u[t] = ut;
+      }
+    }
+#pragma unroll
+    for (int t = 0; t < E; ++t) {
+      if (u[t] >= 0) {
+        load_head<T, NJ>(zs + static_cast<int64_t>(u[t]) * a.ldzs, D, lane, x[t]);
+      } else {
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) x[t][j] = 0.f;
+      }
+    }
+#pragma unroll
+    for (int t = 0; t < E; ++t) {
+      p[t] = score_part<NJ>(x[t], zdv, at);
+      p[E + t] = dot_part<NJ>(gv, x[t]);
+    }
+    warp_sum_n<2 * E>(p, lane);
+#pragma unroll
+    for (int t = 0; t < E; ++t) {
+      if (u[t] < 0) continue;
+      const float w = __fdiv_rn(expf(p[t] - mv), sv);
+      const float ad = w * p[E + t];
+      sd += ad;
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) {
+        const float tt = x[t][j] + zdv[j];
+        const float sl = tt > 0.f ? 1.f : kNegSlope, lr = lrelu(tt);
+        A[j] = fmaf(ad, sl, A[j]);
+        B[j] = fmaf(w, sl, B[j]);
+        C[j] = fmaf(ad, lr, C[j]);
+        Q[j] = fmaf(w, lr, Q[j]);
+      }
+    }
+  }
+  if (slot < 0) {
+    v2_dst_store<T, NJ>(a, v, k, lane, sd, A, B, C, Q);
+  } else {
+    float* p = a.scratch + (static_cast<int64_t>(slot) * a.H + k) * (4 * D + 1);
+    if (lane == 0) p[0] = sd;
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int col = lane + 32 * j;
+      if (col < D) { p[1 + col] = A[j]; p[1 + D + col] = B[j]; p[1 + 2 * D + col] = C[j]; p[1 + 3 * D + col] = Q[j]; }
+    }
+  }
+}
+
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32) gatv2_bwd_dst_kernel(V2Args a) {
+  const int lane = threadIdx.x & 31;
+  const int c = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (c >= a.w.n_chunks) return;
+  walk_chunk(a.w, c, [&](int v, int e0, int n, int slot) { v2_dst_row<T, NJ>(a, v, e0, n, slot, k, lane); });
+}
+
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32) gatv2_bwd_dst_fixup_kernel(V2Args a) {
+  const int lane = threadIdx.x & 31;
+  const int li = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (li >= a.w.n_long) return;
+  const int D = a.D;
+  float sd = 0.f, A[NJ], B[NJ], C[NJ], Q[NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) { A[j] = 0.f; B[j] = 0.f; C[j] = 0.f; Q[j] = 0.f; }
+  for (int sg = a.w.long_seg_ptr[li]; sg < a.w.long_seg_ptr[li + 1]; ++sg) {
+    const float* p = a.scratch + (static_cast<int64_t>(sg) * a.H + k) * (4 * D + 1);
+    sd += p[0];
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int col = lane + 32 * j;
+      if (col < D) { A[j] += p[1 + col]; B[j] += p[1 + D + col]; C[j] += p[1 + 2 * D + col]; Q[j] += p[1 + 3 * D + col]; }
+    }
+  }
+  v2_dst_store<T, NJ>(a, a.w.long_row[li], k, lane, sd, A, B, C, Q);
+}
+
+template <typename T, int NJ>
+__device__ __forceinline__ void v2_src_store(const V2Args& a, int u, int k, int lane, const float (&acc)[NJ]) {
+  T* o = static_cast<T*>(a.out) + static_cast<int64_t>(u) * a.ldo + static_cast<int64_t>(k) * a.D;
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int col = lane + 32 * j;
+    if (col < a.D) o[col] = from_f<T>(acc[j]);
+  }
+}
+
+// d zs[u, k] = sum_v a_uv g_v + de_uv attn ⊙ σ'(t_uv) over the CSC row u (the destinations v of source u), with
+// de_uv = a_uv (<g_v, zs_u> - D_v); an unkept source gets 0.  Scratch of a long-row segment: [H][D].
+template <typename T, int NJ>
+__device__ __forceinline__ void v2_src_row(const V2Args& a, int u, int e0, int n, int slot, int k, int lane) {
+  constexpr int E = v2_edges<NJ>();
+  const int D = a.D;
+  float acc[NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) acc[j] = 0.f;
+  if (is_kept(a.keep, a.num_in, u)) {
+    const T* zd = static_cast<const T*>(a.zd) + static_cast<int64_t>(k) * D;
+    const T* g = static_cast<const T*>(a.g) + static_cast<int64_t>(k) * D;
+    float zsu[NJ], at[NJ];
+    load_head<T, NJ>(static_cast<const T*>(a.zs) + static_cast<int64_t>(u) * a.ldzs + static_cast<int64_t>(k) * D, D,
+                     lane, zsu);
+    load_head_f32<NJ>(a.attn + k * D, D, lane, at);
+    for (int b = 0; b < n; b += E) {
+      int v[E];
+      float y[E][NJ], gg[E][NJ], p[2 * E], mv[E], sv[E], dv[E];
+#pragma unroll
+      for (int t = 0; t < E; ++t) v[t] = b + t < n ? a.w.pidx[e0 + b + t] & kColMask : -1;
+#pragma unroll
+      for (int t = 0; t < E; ++t) {
+        if (v[t] >= 0) {
+          load_head<T, NJ>(zd + static_cast<int64_t>(v[t]) * a.ldzd, D, lane, y[t]);
+          load_head<T, NJ>(g + static_cast<int64_t>(v[t]) * a.ldg, D, lane, gg[t]);
+          const int64_t vk = static_cast<int64_t>(v[t]) * a.H + k;
+          mv[t] = a.m[vk]; sv[t] = a.s[vk]; dv[t] = a.dv[vk];
+        } else {
+#pragma unroll
+          for (int j = 0; j < NJ; ++j) { y[t][j] = 0.f; gg[t][j] = 0.f; }
+          mv[t] = 0.f; sv[t] = 0.f; dv[t] = 0.f;
+        }
+      }
+#pragma unroll
+      for (int t = 0; t < E; ++t) {
+        p[t] = score_part<NJ>(zsu, y[t], at);
+        p[E + t] = dot_part<NJ>(gg[t], zsu);
+      }
+      warp_sum_n<2 * E>(p, lane);
+#pragma unroll
+      for (int t = 0; t < E; ++t) {
+        if (!(sv[t] > 0.f)) continue;         // also the slots past the row's end
+        const float w = __fdiv_rn(expf(p[t] - mv[t]), sv[t]);
+        const float de = w * (p[E + t] - dv[t]);
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+          const float tt = zsu[j] + y[t][j];
+          acc[j] = fmaf(w, gg[t][j], acc[j]);
+          acc[j] = fmaf(tt > 0.f ? de : de * kNegSlope, at[j], acc[j]);
+        }
+      }
+    }
+  }
+  if (slot < 0) {
+    v2_src_store<T, NJ>(a, u, k, lane, acc);
+  } else {
+    float* p = a.scratch + (static_cast<int64_t>(slot) * a.H + k) * D;
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int col = lane + 32 * j;
+      if (col < D) p[col] = acc[j];
+    }
+  }
+}
+
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32) gatv2_bwd_src_kernel(V2Args a) {
+  const int lane = threadIdx.x & 31;
+  const int c = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (c >= a.w.n_chunks) return;
+  walk_chunk(a.w, c, [&](int u, int e0, int n, int slot) { v2_src_row<T, NJ>(a, u, e0, n, slot, k, lane); });
+}
+
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32) gatv2_bwd_src_fixup_kernel(V2Args a) {
+  const int lane = threadIdx.x & 31;
+  const int li = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (li >= a.w.n_long) return;
+  const int D = a.D;
+  float acc[NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) acc[j] = 0.f;
+  for (int sg = a.w.long_seg_ptr[li]; sg < a.w.long_seg_ptr[li + 1]; ++sg) {
+    const float* p = a.scratch + (static_cast<int64_t>(sg) * a.H + k) * D;
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int col = lane + 32 * j;
+      if (col < D) acc[j] += p[col];
+    }
+  }
+  v2_src_store<T, NJ>(a, a.w.long_row[li], k, lane, acc);
+}
+
 // ---------------------------------------------------------------------------------------------------- dispatch
 int nj_of(int32_t D) { return D <= 32 ? 1 : D <= 64 ? 2 : D <= 128 ? 4 : D <= 256 ? 8 : D <= 512 ? 16 : 0; }
 
@@ -497,6 +905,22 @@ void preload_t() {
   cudaFuncGetAttributes(&a, gat_bwd_dst_kernel<T, NJ>);
   cudaFuncGetAttributes(&a, gat_bwd_src_kernel<T, NJ>);
   cudaFuncGetAttributes(&a, gat_bwd_src_fixup_kernel<T, NJ>);
+}
+template <typename T, int NJ>
+void preload_v2_t() {
+  cudaFuncAttributes a;
+  cudaFuncGetAttributes(&a, gatv2_fwd_kernel<T, NJ>);
+  cudaFuncGetAttributes(&a, gat_fwd_fixup_kernel<T, NJ>);
+  cudaFuncGetAttributes(&a, gatv2_bwd_dst_kernel<T, NJ>);
+  cudaFuncGetAttributes(&a, gatv2_bwd_dst_fixup_kernel<T, NJ>);
+  cudaFuncGetAttributes(&a, gatv2_bwd_src_kernel<T, NJ>);
+  cudaFuncGetAttributes(&a, gatv2_bwd_src_fixup_kernel<T, NJ>);
+}
+template <typename T>
+void preload_v2_all() {
+  preload_v2_t<T, 1>(); preload_v2_t<T, 2>(); preload_v2_t<T, 4>(); preload_v2_t<T, 8>(); preload_v2_t<T, 16>();
+  cudaFuncAttributes a;
+  cudaFuncGetAttributes(&a, gat_colsum_kernel<T>);
 }
 template <typename T>
 void preload_all() {
@@ -523,6 +947,17 @@ static void gat_preload() {
     preload_all<__nv_bfloat16>();
     cudaFuncAttributes a;
     cudaFuncGetAttributes(&a, gat_bwd_dst_fixup_kernel);
+    cudaFuncGetAttributes(&a, gat_colsum_final_kernel);
+    cudaGetLastError();
+  });
+}
+
+static void gatv2_preload() {
+  static std::once_flag once;
+  std::call_once(once, [] {
+    preload_v2_all<float>();
+    preload_v2_all<__nv_bfloat16>();
+    cudaFuncAttributes a;
     cudaFuncGetAttributes(&a, gat_colsum_final_kernel);
     cudaGetLastError();
   });
@@ -678,6 +1113,104 @@ extern "C" int pg_gat_colsum(const void* x, int64_t ldx, int32_t n_rows, int32_t
     return PG_ERR_INVALID;
   }
   pg::gat_colsum_final_kernel<<<(n_cols + 255) / 256, 256, 0, st>>>(partial, nb, n_cols, out);
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+extern "C" int pg_gatv2_preload(void) {
+  pg::gatv2_preload();
+  return PG_OK;
+}
+
+extern "C" int pg_gatv2_aggregate(const pg_csr* g, const void* zs, int64_t ldzs, const void* zd, int64_t ldzd,
+                                  int32_t H, int32_t D, int dtype, const float* attn, const uint8_t* keep,
+                                  int32_t num_in, void* out, int64_t ldo, float* m, float* s, float* scratch,
+                                  void* stream) {
+  pg::gatv2_preload();
+  if (int rc = pg::check_plan(g, "pg_gatv2_aggregate")) return rc;
+  const int nj = pg::nj_of(D);
+  const int64_t hd = static_cast<int64_t>(H) * D;
+  PG_REQUIRE(H > 0 && nj > 0 && ldzs >= hd && ldzd >= hd && ldo >= hd, "pg_gatv2_aggregate: bad sizes (H %d, D %d)",
+             H, D);
+  if (g->n_rows == 0) return PG_OK;
+  PG_REQUIRE(zs && zd && attn && out && m && s && (g->n_seg == 0 || scratch), "pg_gatv2_aggregate: null argument");
+  pg::V2Args a{pg::make_walk(g), zs, ldzs, zd, ldzd, nullptr, 0, attn, nullptr, nullptr, nullptr, keep, num_in,
+               out, ldo, m, s, nullptr, nullptr, 0, scratch, H, D};
+  const pg::FwdArgs f = pg::v2_fwd_args(a);
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const dim3 grid((g->n_chunks + kGatWarps - 1) / kGatWarps, H), grid_fix((g->n_long + kGatWarps - 1) / kGatWarps, H);
+  if (dtype == PG_F32) {
+    if (g->n_chunks) PG_GAT_NJ(float, pg::gatv2_fwd_kernel, grid, st, a);
+    if (g->n_long) PG_GAT_NJ(float, pg::gat_fwd_fixup_kernel, grid_fix, st, f);
+  } else if (dtype == PG_BF16) {
+    if (g->n_chunks) PG_GAT_NJ(__nv_bfloat16, pg::gatv2_fwd_kernel, grid, st, a);
+    if (g->n_long) PG_GAT_NJ(__nv_bfloat16, pg::gat_fwd_fixup_kernel, grid_fix, st, f);
+  } else {
+    pg::set_error("pg_gatv2_aggregate: unknown dtype %d", dtype);
+    return PG_ERR_INVALID;
+  }
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+extern "C" int pg_gatv2_bwd_dst(const pg_csr* g, const void* zs, int64_t ldzs, const void* zd, int64_t ldzd,
+                                const void* grad, int64_t ldg, int32_t H, int32_t D, int dtype, const float* attn,
+                                const float* m, const float* s, const uint8_t* keep, int32_t num_in, void* dzd,
+                                int64_t lddzd, float* dv, float* pattn, int64_t ldp, float* scratch, void* stream) {
+  pg::gatv2_preload();
+  if (int rc = pg::check_plan(g, "pg_gatv2_bwd_dst")) return rc;
+  const int nj = pg::nj_of(D);
+  const int64_t hd = static_cast<int64_t>(H) * D;
+  PG_REQUIRE(H > 0 && nj > 0 && ldzs >= hd && ldzd >= hd && ldg >= hd && lddzd >= hd && ldp >= hd,
+             "pg_gatv2_bwd_dst: bad sizes (H %d, D %d)", H, D);
+  if (g->n_rows == 0) return PG_OK;
+  PG_REQUIRE(zs && zd && grad && attn && m && s && dzd && dv && pattn && (g->n_seg == 0 || scratch),
+             "pg_gatv2_bwd_dst: null argument");
+  pg::V2Args a{pg::make_walk(g), zs, ldzs, zd, ldzd, grad, ldg, attn, m, s, nullptr, keep, num_in,
+               dzd, lddzd, nullptr, nullptr, dv, pattn, ldp, scratch, H, D};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const dim3 grid((g->n_chunks + kGatWarps - 1) / kGatWarps, H), grid_fix((g->n_long + kGatWarps - 1) / kGatWarps, H);
+  if (dtype == PG_F32) {
+    if (g->n_chunks) PG_GAT_NJ(float, pg::gatv2_bwd_dst_kernel, grid, st, a);
+    if (g->n_long) PG_GAT_NJ(float, pg::gatv2_bwd_dst_fixup_kernel, grid_fix, st, a);
+  } else if (dtype == PG_BF16) {
+    if (g->n_chunks) PG_GAT_NJ(__nv_bfloat16, pg::gatv2_bwd_dst_kernel, grid, st, a);
+    if (g->n_long) PG_GAT_NJ(__nv_bfloat16, pg::gatv2_bwd_dst_fixup_kernel, grid_fix, st, a);
+  } else {
+    pg::set_error("pg_gatv2_bwd_dst: unknown dtype %d", dtype);
+    return PG_ERR_INVALID;
+  }
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+extern "C" int pg_gatv2_bwd_src(const pg_csr* gt, const void* zs, int64_t ldzs, const void* zd, int64_t ldzd,
+                                const void* grad, int64_t ldg, int32_t H, int32_t D, int dtype, const float* attn,
+                                const float* m, const float* s, const float* dv, const uint8_t* keep, int32_t num_in,
+                                void* dzs, int64_t lddzs, float* scratch, void* stream) {
+  pg::gatv2_preload();
+  if (int rc = pg::check_plan(gt, "pg_gatv2_bwd_src")) return rc;
+  const int nj = pg::nj_of(D);
+  const int64_t hd = static_cast<int64_t>(H) * D;
+  PG_REQUIRE(H > 0 && nj > 0 && ldzs >= hd && ldzd >= hd && ldg >= hd && lddzs >= hd && num_in >= 0,
+             "pg_gatv2_bwd_src: bad sizes (H %d, D %d)", H, D);
+  if (gt->n_rows == 0) return PG_OK;
+  PG_REQUIRE(zs && (num_in == 0 || (zd && grad && m && s && dv)) && attn && dzs && (gt->n_seg == 0 || scratch),
+             "pg_gatv2_bwd_src: null argument");
+  pg::V2Args a{pg::make_walk(gt), zs, ldzs, zd, ldzd, grad, ldg, attn, m, s, dv, keep, num_in,
+               dzs, lddzs, nullptr, nullptr, nullptr, nullptr, 0, scratch, H, D};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const dim3 grid((gt->n_chunks + kGatWarps - 1) / kGatWarps, H), grid_fix((gt->n_long + kGatWarps - 1) / kGatWarps, H);
+  if (dtype == PG_F32) {
+    if (gt->n_chunks) PG_GAT_NJ(float, pg::gatv2_bwd_src_kernel, grid, st, a);
+    if (gt->n_long) PG_GAT_NJ(float, pg::gatv2_bwd_src_fixup_kernel, grid_fix, st, a);
+  } else if (dtype == PG_BF16) {
+    if (gt->n_chunks) PG_GAT_NJ(__nv_bfloat16, pg::gatv2_bwd_src_kernel, grid, st, a);
+    if (gt->n_long) PG_GAT_NJ(__nv_bfloat16, pg::gatv2_bwd_src_fixup_kernel, grid_fix, st, a);
+  } else {
+    pg::set_error("pg_gatv2_bwd_src: unknown dtype %d", dtype);
+    return PG_ERR_INVALID;
+  }
   PG_LAUNCH_CHECK();
   return PG_OK;
 }

@@ -17,8 +17,9 @@ training: every epoch each partition keeps a random fraction p of its halo nodes
 that epoch, so the halo exchange moves p times the bytes.  Evaluation always uses the full graph.  Like
 `--eval-partitioned` it has a suppressed default: read it with getattr(args, 'sampling_rate', 1.0).
 
-`--model gat` trains graph attention (DGL's GATConv) instead of GraphSAGE; `--n-heads k` (not in the reference, default
-4, suppressed like `--sampling-rate`: read it with getattr(args, 'n_heads', 4)) sets its heads per hidden layer.
+`--model gat` trains graph attention (DGL's GATConv) instead of GraphSAGE, and `--model gatv2` dynamic graph attention
+(DGL's GATv2Conv); `--n-heads k` (not in the reference, default 4, suppressed like `--sampling-rate`: read it with
+getattr(args, 'n_heads', 4)) sets the heads per hidden layer of either.
 
 `--halo-bits b` (8 or 4; not in the reference) quantises the per-epoch halo messages of graph layers >= 1, features
 forward and gradients backward: every row travels as b-bit codes with an fp32 (lo, scale), stochastically rounded so
@@ -28,7 +29,7 @@ read it with getattr(args, 'halo_bits', None).
 
 `--aggregator {mean,pool}` (not in the reference) selects the neighbour reduction of the GraphSAGE layers: `mean` (the
 reference's) or `pool`, Hamilton et al.'s max-pool aggregator (DGL `SAGEConv(aggregator_type='pool')`): every layer
-takes the element-wise neighbour maximum of ReLU(h Wp^T + bp).  It cannot be combined with --model gat or --use-pp.
+takes the element-wise neighbour maximum of ReLU(h Wp^T + bp).  It cannot be combined with --model gat, --model gatv2 or --use-pp.
 Suppressed like `--sampling-rate`: read it with getattr(args, 'aggregator', 'mean').
 """
 import argparse
@@ -37,7 +38,7 @@ import argparse
 _FLAGS = [
     ("dataset", dict(type=str, default='reddit', help="the input dataset (or synthetic:<shape>)")),
     ("graph-name", dict(type=str, default='')),
-    ("model", dict(type=str, default='graphsage', help="model for training (graphsage | gcn | gat)")),
+    ("model", dict(type=str, default='graphsage', help="model for training (graphsage | gcn | gat | gatv2)")),
     ("dropout", dict(type=float, default=0.5, help="dropout probability")),
     ("lr", dict(type=float, default=1e-2, help="learning rate")),
     ("n-epochs", dict(type=int, default=200, help="the number of training epochs")),
@@ -111,7 +112,7 @@ def build_parser():
                         help="boundary-node sampling: the fraction of halo nodes every partition keeps per epoch "
                              "(synchronous training; default 1 = all)")
     parser.add_argument('--n-heads', '--n_heads', type=_n_heads, default=argparse.SUPPRESS,
-                        help="--model gat: attention heads of every hidden layer (default 4)")
+                        help="--model gat / gatv2: attention heads of every hidden layer (default 4)")
     parser.add_argument('--halo-bits', '--halo_bits', type=int, choices=[8, 4], default=argparse.SUPPRESS,
                         help="send the halo messages of graph layers >= 1 as stochastically rounded 8- or 4-bit codes "
                              "(default: exact)")

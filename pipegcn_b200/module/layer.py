@@ -22,6 +22,19 @@ over the `[inner | halo]` rows h the halo exchange returns (inner rows v, in-edg
     out[v] = sum_u softmax_u(LeakyReLU(el[u] + er[v])) z[u] + bias
 
 State-dict keys are GATConv's: `fc.weight` [H*D, d_in], `attn_l` / `attn_r` [1, H, D], `bias` [H*D].
+
+`GATv2Layer` (not in the reference): DGL's `GATv2Conv` with share_weights=False, bias=True, feat_drop = attn_drop = 0,
+no residual, negative_slope 0.2 (Brody et al., "How Attentive are Graph Attention Networks?", ICLR 2022), over the
+same rows, per head k:
+
+    zs = h @ W_s^T + b_s  (every row),  zd = h[:N_in] @ W_d^T + b_d  (destination rows),
+    e_uv = <attn[k], LeakyReLU(zs[u, k] + zd[v, k])>,
+    out[v, k] = sum_u softmax_u(e_uv) zs[u, k]                    (no output bias; 0 for a row without in-edges)
+
+State-dict keys are GATv2Conv's: `fc_src.weight` / `fc_dst.weight` [H*D, d_in], `fc_src.bias` / `fc_dst.bias` [H*D],
+`attn` [1, H, D].  Initialisation is GATv2Conv.reset_parameters, in this draw order, with
+gain = calculate_gain('relu'): xavier_normal_(fc_src.weight), fc_src.bias = 0, xavier_normal_(fc_dst.weight),
+fc_dst.bias = 0, xavier_normal_(attn).
 """
 import math
 
@@ -113,3 +126,28 @@ class GATLayer(nn.Module):
         `drop_bwd`: `feat` already is dropout(F) under that key; the gradient returned is the one with respect to F."""
         return ops.gat_layer(feat, graph, keep, self.num_heads, self.fc.weight, self.attn_l, self.attn_r, self.bias,
                              drop_bwd)
+
+
+class GATv2Layer(nn.Module):
+
+    def __init__(self, in_feats, out_feats, num_heads):
+        super().__init__()
+        self.in_feats, self.out_feats, self.num_heads = in_feats, out_feats, num_heads
+        self.fc_src = nn.Linear(in_feats, out_feats * num_heads, bias=True)
+        self.fc_dst = nn.Linear(in_feats, out_feats * num_heads, bias=True)
+        self.attn = nn.Parameter(torch.empty(1, num_heads, out_feats))
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        """GATv2Conv.reset_parameters (share_weights=False)."""
+        gain = nn.init.calculate_gain('relu')
+        nn.init.xavier_normal_(self.fc_src.weight, gain=gain)
+        nn.init.constant_(self.fc_src.bias, 0)
+        nn.init.xavier_normal_(self.fc_dst.weight, gain=gain)
+        nn.init.constant_(self.fc_dst.bias, 0)
+        nn.init.xavier_normal_(self.attn, gain=gain)
+
+    def forward(self, graph, feat, keep=None, drop_bwd=None):
+        """As GATLayer.forward."""
+        return ops.gatv2_layer(feat, graph, keep, self.num_heads, self.fc_src.weight, self.fc_src.bias,
+                               self.fc_dst.weight, self.fc_dst.bias, self.attn, drop_bwd)

@@ -19,13 +19,16 @@ layer concatenates `n_heads` heads of d_out / n_heads columns, a graph layer tha
 exchange moves the layer input h, so pipelining, the corrections, the static layer-0 store and the fused dropout apply
 unchanged; with boundary-node sampling the layers take the buffer's keep mask of the halo rows (`Buffer.keep_mask`),
 and unkept rows are absent from every softmax.
+
+`GATv2(GAT)` (not in the reference) is `GAT` with `GATv2Layer`s (DGL's GATv2Conv): the same heads, keep mask and
+partitioned evaluation; only the graph layers and the kernels they load differ.
 """
 import torch
 from torch import nn
 import torch.nn.functional as F
 
 from ..helper import context as ctx
-from .layer import GATLayer, GraphSAGELayer
+from .layer import GATLayer, GATv2Layer, GraphSAGELayer
 
 
 class GNNBase(nn.Module):
@@ -208,12 +211,26 @@ class GAT(GraphSAGE):
         buf = self._buffer() if self.training else None
         return getattr(buf, 'keep_mask', None) if buf is not None else None
 
-    def forward(self, g, feat, in_deg=None):
+    def _preload(self):
         from .. import ops
         ops.gat_preload()
+
+    def forward(self, g, feat, in_deg=None):
+        self._preload()
         return super().forward(g, feat, in_deg)
 
     def forward_partitioned(self, g, xch, pp_feat=None, push0=False):
-        from .. import ops
-        ops.gat_preload()
+        self._preload()
         return (yield from super().forward_partitioned(g, xch, pp_feat, push0))
+
+
+class GATv2(GAT):
+
+    def _graph_layer(self, i, d_in, d_out):
+        if i < self.n_layers - 1:
+            return GATv2Layer(d_in, d_out // self.n_heads, self.n_heads)
+        return GATv2Layer(d_in, d_out, 1)                # the logits: one head of n_class
+
+    def _preload(self):
+        from .. import ops
+        ops.gatv2_preload()

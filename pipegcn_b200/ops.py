@@ -875,6 +875,131 @@ def gat_layer(feat, graph, keep, heads, weight, attn_l, attn_r, bias, drop_bwd=N
     return GatLayerFn.apply(feat, graph, keep, int(heads), weight, attn_l, attn_r, bias, drop_bwd)
 
 
+# ---- dynamic graph attention, GATv2 (csrc/attention.cu) ----------------------------------------------------
+def gatv2_preload():
+    """Load every GATv2 kernel now (see gat_preload)."""
+    _C.check(_C.lib.pg_gatv2_preload(), "pg_gatv2_preload")
+
+
+def gatv2_aggregate(graph: PartGraph, zs, zd, attn, heads: int, keep=None):
+    """out [N_in, H*D] = per-head edge softmax of <attn, LeakyReLU(zs[u] + zd[v])> over the forward CSR applied to zs;
+    with the softmax statistics m, s [N_in, H] fp32.  attn: fp32 [H*D]."""
+    plan = graph.fwd
+    n, hd = plan.n_rows, zs.shape[1]
+    d = hd // heads
+    out = alloc_rows(n, hd, zs.dtype, zs.device)
+    m = torch.empty(n, heads, dtype=torch.float32, device=zs.device)
+    s = torch.empty(n, heads, dtype=torch.float32, device=zs.device)
+    scratch = plan.scratch(heads * (d + 2))
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_gatv2_aggregate(C.byref(plan.c), zs.data_ptr(), zs.stride(0), zd.data_ptr(), zd.stride(0), heads,
+                                       d, _C.dtype_code(zs.dtype), attn.data_ptr(), _ptr(keep), graph.num_in,
+                                       out.data_ptr(), out.stride(0), m.data_ptr(), s.data_ptr(), _ptr(scratch),
+                                       _C.stream_ptr()), "pg_gatv2_aggregate")
+    return out, m, s
+
+
+def gatv2_bwd_dst(graph: PartGraph, zs, zd, g, attn, m, s, heads: int, keep=None):
+    """(dzd [N_in, H*D] in zs's dtype, dv [N_in, H] fp32, pattn [N_in, H*D] fp32) over the forward CSR: the gradient
+    of zd, D_v = <g_v, out_v>, and the per-row terms of the attn gradient (its column sum)."""
+    plan = graph.fwd
+    n, hd = plan.n_rows, zs.shape[1]
+    d = hd // heads
+    dzd = alloc_rows(n, hd, zs.dtype, zs.device)
+    dv = torch.empty(n, heads, dtype=torch.float32, device=zs.device)
+    pattn = alloc_rows(n, hd, torch.float32, zs.device)
+    scratch = plan.scratch(heads * (4 * d + 1))
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_gatv2_bwd_dst(C.byref(plan.c), zs.data_ptr(), zs.stride(0), zd.data_ptr(), zd.stride(0),
+                                     g.data_ptr(), g.stride(0), heads, d, _C.dtype_code(zs.dtype), attn.data_ptr(),
+                                     m.data_ptr(), s.data_ptr(), _ptr(keep), graph.num_in, dzd.data_ptr(),
+                                     dzd.stride(0), dv.data_ptr(), pattn.data_ptr(), pattn.stride(0), _ptr(scratch),
+                                     _C.stream_ptr()), "pg_gatv2_bwd_dst")
+    return dzd, dv, pattn
+
+
+def gatv2_bwd_src(graph: PartGraph, zs, zd, g, attn, m, s, dv, heads: int, keep=None):
+    """dzs [num_all, H*D] in zs's dtype over the CSC of the graph (0 on unkept halo rows)."""
+    plan = graph.bwd
+    n, hd = plan.n_rows, zs.shape[1]
+    d = hd // heads
+    dzs = alloc_rows(n, hd, zs.dtype, zs.device)
+    scratch = plan.scratch(heads * d)
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_gatv2_bwd_src(C.byref(plan.c), zs.data_ptr(), zs.stride(0), zd.data_ptr(), zd.stride(0),
+                                     g.data_ptr(), g.stride(0), heads, d, _C.dtype_code(zs.dtype), attn.data_ptr(),
+                                     m.data_ptr(), s.data_ptr(), dv.data_ptr(), _ptr(keep), graph.num_in,
+                                     dzs.data_ptr(), dzs.stride(0), _ptr(scratch), _C.stream_ptr()), "pg_gatv2_bwd_src")
+    return dzs
+
+
+class GatV2LayerFn(torch.autograd.Function):
+    """One GATv2 layer (DGL GATv2Conv, share_weights=False, no attention dropout, no residual) over the [inner | halo]
+    rows `feat` of a partition, returning the inner rows:
+
+        zs  = feat @ W_s^T + b_s           [num_all, H*D]   pg_linear over all rows
+        zd  = feat[:N_in] @ W_d^T + b_d    [N_in, H*D]      pg_linear over the inner rows
+        out = softmax-aggregate(zs)        [N_in, H*D]      pg_gatv2_aggregate (+ softmax statistics m, s)
+
+    Backward: dzd, D_v and the attn terms (pg_gatv2_bwd_dst over the CSR), dzs (pg_gatv2_bwd_src over the CSC), d attn
+    and the bias gradients as fixed-order column sums, dW_s = dzs^T feat, dW_d = dzd^T feat[:N_in] (pg_wgrad),
+    g_feat = dzs @ W_s (+ dzd @ W_d on the inner rows, one two-source pg_linear), with the dropout backward of
+    `drop_bwd` in its epilogue.  `keep`: the boundary-node sample of the halo rows (uint8), or None."""
+
+    @staticmethod
+    def forward(ctx, feat, graph, keep, heads, w_s, b_s, w_d, b_d, attn, drop_bwd=None):
+        ctx.drop_bwd = drop_bwd
+        if feat.stride(1) != 1:
+            feat = feat.contiguous()
+        n_in = graph.num_in
+        fsp = presplit(feat)                   # fp32: one split of feat for both products
+        zs = gemm_nt(fsp, padded_weight(w_s, feat.dtype), bias=b_s)
+        zd = gemm_nt(fsp.rows(0, n_in) if isinstance(fsp, Split) else feat[:n_in], padded_weight(w_d, feat.dtype),
+                     bias=b_d)
+        a32 = _f32(attn)
+        out, m, s = gatv2_aggregate(graph, zs, zd, a32, heads, keep)
+        ctx.save_for_backward(feat, zs, zd, m, s, w_s, w_d)
+        ctx.graph, ctx.keep, ctx.heads, ctx.a32 = graph, keep, heads, a32
+        ctx.attn_shape, ctx.attn_dtype = tuple(attn.shape), attn.dtype
+        ctx.has_bias = b_s is not None, b_d is not None
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        feat, zs, zd, m, s, w_s, w_d = ctx.saved_tensors
+        graph, heads, keep = ctx.graph, ctx.heads, ctx.keep
+        n_in = graph.num_in
+        _take_colsum(g)                        # no output bias: the by-product is not needed
+        g = _tma_ready(g if g.dtype == feat.dtype else g.to(feat.dtype))
+        dzd, dv, pattn = gatv2_bwd_dst(graph, zs, zd, g, ctx.a32, m, s, heads, keep)
+        dzs = gatv2_bwd_src(graph, zs, zd, g, ctx.a32, m, s, dv, heads, keep)
+        g_attn = gat_colsum(pattn).view(ctx.attn_shape).to(ctx.attn_dtype)
+        gbs = gat_colsum(dzs) if ctx.has_bias[0] else None
+        gbd = gat_colsum(dzd) if ctx.has_bias[1] else None
+        dzsp, dzdp = presplit(dzs), presplit(dzd)
+        is_split = isinstance(dzsp, Split)
+        g_feat = None
+        if ctx.needs_input_grad[0]:
+            g_feat = alloc_rows(feat.shape[0], feat.shape[1], feat.dtype, feat.device)
+            wst = padded_weight(w_s, feat.dtype, transpose=True)
+            drop = ctx.drop_bwd if ctx.drop_bwd is not None and ctx.drop_bwd.p > 0 else None
+            db = drop if drop is not None and feat.shape[1] <= 256 and _drop_ok(g_feat) else None
+            gemm_nt(dzsp.rows(0, n_in) if is_split else dzs[:n_in], wst, dzdp,
+                    padded_weight(w_d, feat.dtype, transpose=True), out=g_feat[:n_in], drop=db)
+            if feat.shape[0] > n_in:
+                gemm_nt(dzsp.rows(n_in) if is_split else dzs[n_in:], wst, out=g_feat[n_in:], drop=db, drop_row0=n_in)
+            if drop is not None and db is None:
+                dropout_rows(g_feat, drop, out=g_feat)
+        fsp = presplit(feat)
+        gws = wgrad(dzsp, fsp).to(w_s.dtype)
+        gwd = wgrad(dzdp, fsp.rows(0, n_in) if isinstance(fsp, Split) else feat[:n_in]).to(w_d.dtype)
+        return g_feat, None, None, None, gws, gbs, gwd, gbd, g_attn, None
+
+
+def gatv2_layer(feat, graph, keep, heads, w_s, b_s, w_d, b_d, attn, drop_bwd=None) -> torch.Tensor:
+    return GatV2LayerFn.apply(feat, graph, keep, int(heads), w_s, b_s, w_d, b_d, attn, drop_bwd)
+
+
 # ---- max-pool GraphSAGE (csrc/pool.cu) ---------------------------------------------------------------------
 def pool_preload():
     """Load every pool kernel now (see gat_preload)."""

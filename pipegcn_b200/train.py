@@ -32,7 +32,7 @@ from .helper import context as ctx
 from .helper.feature_buffer import Buffer, EvalExchange, OneShotExchange, check_halo_bits, check_sampling
 from .helper.reducer import Reducer
 from .helper.timer.comm_timer import CommTimer
-from .module.model import GAT, GraphSAGE
+from .module.model import GAT, GATv2, GraphSAGE
 from .partition import PartitionLayout, get_layer_size
 
 
@@ -47,24 +47,27 @@ def _quant_seed(args):
 
 
 def check_model(args):
-    """Refuses, before anything is allocated, a configuration that is not implemented: --model gat with --use-pp (the
-    precompute is GraphSAGE's neighbour mean) or with a hidden width that does not split into --n-heads heads, and
-    --aggregator pool with --model gat (an attention layer has no aggregator) or with --use-pp (a neighbour mean)."""
+    """Refuses, before anything is allocated, a configuration that is not implemented: --model gat or gatv2 with
+    --use-pp (the precompute is GraphSAGE's neighbour mean) or with a hidden width that does not split into --n-heads
+    heads, and --aggregator pool with an attention model (an attention layer has no aggregator) or with --use-pp (a
+    neighbour mean)."""
+    attention = args.model in ('gat', 'gatv2')
     aggregator = getattr(args, 'aggregator', 'mean')
     if aggregator not in ('mean', 'pool'):
         raise ValueError(f"--aggregator {aggregator}: expected mean or pool")
     if aggregator == 'pool':
-        if args.model == 'gat':
-            raise ValueError("--aggregator pool is a GraphSAGE aggregator; --model gat has none")
+        if attention:
+            raise ValueError(f"--aggregator pool is a GraphSAGE aggregator; --model {args.model} has none")
         if args.use_pp:
             raise NotImplementedError("--aggregator pool with --use-pp: the precompute is a neighbour mean")
-    if args.model != 'gat':
+    if not attention:
         return
     if args.use_pp:
-        raise NotImplementedError("--model gat with --use-pp: the precompute is GraphSAGE's neighbour mean")
+        raise NotImplementedError(f"--model {args.model} with --use-pp: the precompute is GraphSAGE's neighbour mean")
     heads = getattr(args, 'n_heads', 4)
     if heads < 1 or args.n_hidden % heads:
-        raise ValueError(f"--model gat: --n-hidden {args.n_hidden} does not split into --n-heads {heads} heads")
+        raise ValueError(f"--model {args.model}: --n-hidden {args.n_hidden} does not split into --n-heads {heads} "
+                         "heads")
 
 
 def create_model(layer_size, args, buffer=None, dtype=torch.float32):
@@ -74,8 +77,9 @@ def create_model(layer_size, args, buffer=None, dtype=torch.float32):
         kw = {} if aggregator == 'mean' else dict(aggregator=aggregator)
         return GraphSAGE(layer_size, F.relu, args.use_pp, norm=args.norm, dropout=args.dropout,
                          n_linear=args.n_linear, train_size=args.n_train, buffer=buffer, dtype=dtype, **kw)
-    if args.model == 'gat':
-        return GAT(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
+    if args.model in ('gat', 'gatv2'):
+        cls = GAT if args.model == 'gat' else GATv2
+        return cls(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
                    train_size=args.n_train, buffer=buffer, dtype=dtype, n_heads=getattr(args, 'n_heads', 4))
     raise NotImplementedError(args.model)
 
