@@ -111,6 +111,22 @@ int pg_aggregate(const pg_csr* g, const void* x, int64_t ldx, void* out, int64_t
 int pg_aggregate_drop(const pg_csr* g, const void* x, int64_t ldx, void* out, int64_t ldo, int32_t d, int dtype,
                       const float* row_div, int32_t acc_rows, float* scratch, const pg_drop* drop, void* stream);
 
+/*
+ * Neighbour aggregate with a per-source and a per-destination scale (GraphConv's symmetric norm, c = deg^-1/2):
+ *   out[r, 0:d] = dst_scale[r] * ( sum_{e in row r} src_scale[indices[e]] * x[indices[e], 0:d] )  ( + bias[0:d] )
+ * then, if `drop` is given, that key's dropout mask as the row is stored (as pg_aggregate_drop).  The sum is fp32 in the
+ * order of pg_aggregate (CSR order within a chunk or segment, long-row segment partials merged in segment order), each
+ * term one multiply-add; then the multiply by dst_scale, then the bias, then one rounding to `dtype`.  With
+ * src_scale == 1 and dst_scale = 1 / row_div (fp32 IEEE division) the result has the bits of pg_aggregate.
+ * src_scale: fp32 [source rows]; dst_scale: fp32 [n_rows]; bias: fp32 [d] or NULL; scratch as pg_aggregate.
+ * No accumulate mode, no atomics: the same bits from run to run.
+ */
+int pg_aggregate_scaled(const pg_csr* g, const void* x, int64_t ldx, void* out, int64_t ldo, int32_t d, int dtype,
+                        const float* src_scale, const float* dst_scale, const float* bias, float* scratch,
+                        const pg_drop* drop, void* stream);
+/* loads every pg_aggregate_scaled kernel (call it before any halo wait can spin: a first launch may wait for the device) */
+int pg_aggregate_scaled_preload(void);
+
 /* out[r, 0:d] = x[r, 0:d] / row_div[r]   (gradient of `/ degs`, layer.py:50) */
 int pg_row_div(const void* x, int64_t ldx, void* out, int64_t ldo, int32_t n_rows, int32_t d, int dtype,
                const float* row_div, void* stream);

@@ -68,6 +68,9 @@ def _load():
         "pg_aggregate": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, i32, C.c_int, vp, i32, vp, vp]),
         "pg_aggregate_drop": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, i32, C.c_int, vp, i32, vp,
                                         C.POINTER(pg_drop), vp]),
+        "pg_aggregate_scaled": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, i32, C.c_int, vp, vp, vp, vp,
+                                          C.POINTER(pg_drop), vp]),
+        "pg_aggregate_scaled_preload": (C.c_int, []),
         "pg_row_div": (C.c_int, [vp, i64, vp, i64, i32, i32, C.c_int, vp, vp]),
         "pg_linear": (C.c_int, [C.c_int, C.c_int, C.POINTER(pg_gemm_src), i32, vp, vp, vp, i64, i32, i32, vp]),
         "pg_linear_drop": (C.c_int, [C.c_int, C.c_int, C.POINTER(pg_gemm_src), i32, vp, vp, vp, i64, i32, i32,

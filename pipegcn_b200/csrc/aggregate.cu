@@ -9,16 +9,57 @@
 // in flight per group before they are accumulated.  Rows longer than seg_len are cut into
 // segments reduced by different groups into fp32 partials and summed in segment order by a
 // fix-up kernel: deterministic, no atomics.
+//
+// Every kernel has a compile-time switch SC (pg_aggregate_scaled, GraphConv's symmetric norm):
+//   out[r,:] = dst_scale[r] * ( sum_{e in row r} src_scale[indices[e]] * x[indices[e],:] )  (+ bias)
+// The lane that loads a column id also loads its source scale; the scale travels with the id (one more shuffle per
+// edge) and is applied as a multiply-add per element.  dst_scale arrives in the row_div slot and is a multiplier.
+// SC = false instantiations are the plain aggregate, instruction for instruction.  The SC kernels hold the scales of
+// the rows in flight as well: they are compiled for one resident CTA per SM fewer (agg_occ does not apply), which
+// keeps every one of them free of local-memory spills.
 #include <algorithm>
+#include <mutex>
+#include <type_traits>
 #include <string.h>
 #include "common.cuh"
 
 namespace pg {
 
-template <typename T, int VB, int G, int VPL, int U>
+// the operands of the SC instantiations that have no slot in the plain aggregate's arguments
+struct ScaleArg {
+  const float* src;    // [source rows] multiplier of every gathered row
+  const float* bias;   // [d] added after the row scale, or NULL
+  int d;               // columns of the bias (the pad columns of a vector get none)
+};
+
+// the factor every output row is multiplied by: dst_scale[row] (SC), else the IEEE reciprocal of row_div[row]
+template <bool SC>
+__device__ __forceinline__ float row_scale(const float* __restrict__ row_div, int row) {
+  if constexpr (SC) return __ldg(row_div + row);
+  return row_div != nullptr ? 1.f / __ldg(row_div + row) : 1.f;
+}
+// the scale operands a walker holds: none in the plain instantiations, so their code is that of pg_aggregate
+struct NoScale {};
+template <bool SC> using ScaleOf = std::conditional_t<SC, ScaleArg, NoScale>;
+
+// r[0:V] += bias[o:o+V] (SC with a bias; columns past d add nothing)
+
+template <bool SC, int V, typename S>
+__device__ __forceinline__ void add_bias(float* r, const S& sc, int64_t o) {
+  if constexpr (SC) {
+    if (sc.bias != nullptr) {
+#pragma unroll
+      for (int i = 0; i < V; ++i)
+        if (o + i < sc.d) r[i] += __ldg(sc.bias + o + i);
+    }
+  }
+}
+
+template <typename T, int VB, int G, int VPL, int U, bool SC>
 __global__ void __launch_bounds__(256)
 agg_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict__ out, int64_t ldo, int nvec,
-           const float* __restrict__ row_div, int acc_rows, float* __restrict__ scratch, int64_t lds, DropArg drop) {
+           const float* __restrict__ row_div, int acc_rows, float* __restrict__ scratch, int64_t lds, DropArg drop,
+           ScaleArg sc) {
   using P = Pack<T, VB>;
   using Raw = typename P::Raw;
   constexpr int V = P::V;
@@ -74,17 +115,34 @@ agg_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict_
 #pragma unroll
         for (int j = 0; j < VPL; ++j)
           if (act[j]) v[u][j] = ld_vec<VB>(xc[j] + static_cast<uint64_t>(src[u]) * ldx_bytes);
+      float ss[U];
+      if constexpr (SC) {
+#pragma unroll
+        for (int u = 0; u < U; ++u) ss[u] = __ldg(sc.src + src[u]);
+      }
 #pragma unroll
       for (int u = 0; u < U; ++u)
 #pragma unroll
-        for (int j = 0; j < VPL; ++j)
-          if (act[j]) P::add(acc[j], v[u][j]);
+        for (int j = 0; j < VPL; ++j) {
+          if constexpr (SC) {
+            if (act[j]) P::fma(acc[j], v[u][j], ss[u]);
+          } else {
+            if (act[j]) P::add(acc[j], v[u][j]);
+          }
+        }
     }
     for (; e < end; ++e) {
       const uint32_t s = static_cast<uint32_t>(__ldg(g.indices + e));
+      if constexpr (SC) {
+        const float s1 = __ldg(sc.src + s);
 #pragma unroll
-      for (int j = 0; j < VPL; ++j)
-        if (act[j]) P::add(acc[j], ld_vec<VB>(xc[j] + static_cast<uint64_t>(s) * ldx_bytes));
+        for (int j = 0; j < VPL; ++j)
+          if (act[j]) P::fma(acc[j], ld_vec<VB>(xc[j] + static_cast<uint64_t>(s) * ldx_bytes), s1);
+      } else {
+#pragma unroll
+        for (int j = 0; j < VPL; ++j)
+          if (act[j]) P::add(acc[j], ld_vec<VB>(xc[j] + static_cast<uint64_t>(s) * ldx_bytes));
+      }
     }
 
     if (seg >= 0) {
@@ -100,7 +158,7 @@ agg_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict_
       // `/ degs` (layer.py:50) as one IEEE reciprocal per row and a multiply per element (<= 1 ulp from the
       // division): the per-element IEEE division took its slow path on every exact zero (dropout) and was
       // a third of the kernel's instructions in the ncu source view
-      const float inv = row_div ? 1.f / __ldg(row_div + row) : 1.f;
+      const float inv = row_scale<SC>(row_div, row);
       T* op = out + static_cast<int64_t>(row) * ldo;
 #pragma unroll
       for (int j = 0; j < VPL; ++j) {
@@ -112,6 +170,7 @@ agg_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict_
           const float a = (i & 1) ? acc[j][i / 2].y : acc[j][i / 2].x;
           r[i] = a * inv;
         }
+        add_bias<SC, V>(r, sc, o);
         if (row < acc_rows) {
           float ov[V];
           P::unpack(*reinterpret_cast<const Raw*>(op + o), ov);
@@ -129,10 +188,10 @@ agg_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict_
 // sums the fp32 partials of every long row and writes the row: one CTA per long row, warp w adds the segments
 // s0 + w, s0 + w + 8, ... (four in flight), then the eight warp sums are added in warp order -- a fixed order, so the
 // result does not depend on scheduling
-template <typename T, int VB>
+template <typename T, int VB, bool SC>
 __global__ void __launch_bounds__(256)
 agg_fixup_kernel(pg_csr g, T* __restrict__ out, int64_t ldo, int nvec, const float* __restrict__ row_div,
-                 int acc_rows, const float* __restrict__ scratch, int64_t lds, DropArg drop) {
+                 int acc_rows, const float* __restrict__ scratch, int64_t lds, DropArg drop, ScaleArg sc) {
   using P = Pack<T, VB>;
   constexpr int V = P::V;
   __shared__ float part[8][32 * V];
@@ -140,7 +199,7 @@ agg_fixup_kernel(pg_csr g, T* __restrict__ out, int64_t ldo, int nvec, const flo
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
   const int row = __ldg(g.long_row + li);
   const int s0 = __ldg(g.long_seg_ptr + li), s1 = __ldg(g.long_seg_ptr + li + 1);
-  const float inv = row_div ? 1.f / __ldg(row_div + row) : 1.f;
+  const float inv = row_scale<SC>(row_div, row);
   T* op = out + static_cast<int64_t>(row) * ldo;
   for (int v0 = 0; v0 < nvec; v0 += 32) {
     const int vi = v0 + lane;
@@ -176,6 +235,7 @@ agg_fixup_kernel(pg_csr g, T* __restrict__ out, int64_t ldo, int nvec, const flo
         for (int w = 1; w < 8; ++w) a += part[w][lane * V + i];
         r[i] = a * inv;
       }
+      add_bias<SC, V>(r, sc, static_cast<int64_t>(vi) * V);
       if (row < acc_rows) {
         float o[V];
         P::unpack(*reinterpret_cast<const typename P::Raw*>(op + static_cast<int64_t>(vi) * V), o);
@@ -249,13 +309,14 @@ template <> __device__ __forceinline__ void st_vec_cs<4>(void* p, uint32_t v) { 
 
 struct Chunk { int e_beg, n, item, kind_rows; };   // kind = kind_rows & 3 (0: n_rows rows of n edges, 1: one row, 2: segment)
 
-template <typename T, int VB, int VPL, int U, bool HINT>
+template <typename T, int VB, int VPL, int U, bool HINT, bool SC>
 struct Agg2 {
   using P = Pack<T, VB>;
   using Raw = typename P::Raw;
   static constexpr int V = P::V;
   static constexpr int NA = P::NA;
   static constexpr int kVPL = VPL;
+  static constexpr bool kSC = SC;
   static constexpr unsigned kFull = 0xffffffffu;
 
   const char* xc[VPL];      // this lane's column(s) of source row 0
@@ -269,6 +330,7 @@ struct Agg2 {
   int nvec;
   DropArg drop;             // dropout applied to every row as it is written (thresh16 == 0: none)
   uint32_t drop_hi;
+  ScaleOf<SC> sc;
   float2 acc[VPL][NA];
 
   __device__ __forceinline__ void zero() {
@@ -285,9 +347,17 @@ struct Agg2 {
   }
   // lanes past the row width (act[j] false) read column 0 like lane 0 does (same address: no extra traffic) and
   // are only masked at the store: the loads and adds of the inner loops carry no predicates
-  __device__ __forceinline__ void add(const Raw (&v)[VPL]) {
+  __device__ __forceinline__ void add(const Raw (&v)[VPL], float s) {
 #pragma unroll
-    for (int j = 0; j < VPL; ++j) P::add(acc[j], v[j]);
+    for (int j = 0; j < VPL; ++j) {
+      if constexpr (SC) P::fma(acc[j], v[j], s);
+      else P::add(acc[j], v[j]);
+    }
+  }
+  // source scale of column id `id` (hot flag in bit 31)
+  __device__ __forceinline__ float scale_of(uint32_t id) const {
+    if constexpr (SC) return __ldg(sc.src + (id & 0x7fffffffu));
+    else return 1.f;
   }
   // the ragged end of a batch: every load is issued (positions past the end fetch a valid row: lanes past the
   // chunk hold column 0) and the fetched bits are ANDed with 0 / ~0 -- no predicated loads, no divergent code
@@ -316,6 +386,7 @@ struct Agg2 {
         float r[V];
 #pragma unroll
         for (int i = 0; i < V; ++i) r[i] = ((i & 1) ? acc[j][i / 2].y : acc[j][i / 2].x) * inv;
+        add_bias<SC, V>(r, sc, o);
         if (row < acc_rows) {
           float ov[V];
           P::unpack(*reinterpret_cast<const Raw*>(op + o), ov);
@@ -333,18 +404,23 @@ struct Agg2 {
 
   // a chunk of n_rows whole rows of `len` (<= 32) entries each, n_rows * len <= 32: U neighbour rows in flight
   // across row boundaries; a row is flushed as soon as its last entry has been added (warp-uniform branch)
-  __device__ __forceinline__ void small_chunk(uint32_t my_idx, int my_row, float my_inv, int n_rows, int len) {
+  __device__ __forceinline__ void small_chunk(uint32_t my_idx, float my_sc, int my_row, float my_inv, int n_rows,
+                                              int len) {
     const int n_e = n_rows * len;
     int r = 0, cnt = 0;
 #pragma unroll 1
     for (int u0 = 0; u0 < n_e; u0 += U) {
       Raw v[U][VPL];
+      float s[U];
 #pragma unroll
-      for (int u = 0; u < U; ++u) ld_rows(v[u], __shfl_sync(kFull, my_idx, (u0 + u) & 31));   // lanes >= n_e hold 0
+      for (int u = 0; u < U; ++u) {
+        ld_rows(v[u], __shfl_sync(kFull, my_idx, (u0 + u) & 31));   // lanes >= n_e hold 0
+        s[u] = SC ? __shfl_sync(kFull, my_sc, (u0 + u) & 31) : 1.f;
+      }
 #pragma unroll
       for (int u = 0; u < U; ++u) {
         if (u0 + u < n_e) {
-          add(v[u]);
+          add(v[u], s[u]);
           if (++cnt == len) {
             flush(__shfl_sync(kFull, my_row, r), __shfl_sync(kFull, my_inv, r));
             ++r;
@@ -359,36 +435,46 @@ struct Agg2 {
 
   // B neighbour rows (columns my_idx[u0 .. u0+B) of the current 32 indices) fetched, then added in order
   template <int B>
-  __device__ __forceinline__ void batch(uint32_t my_idx, int u0) {
+  __device__ __forceinline__ void batch(uint32_t my_idx, float my_sc, int u0) {
     Raw v[B][VPL];
+    float s[B];
 #pragma unroll
-    for (int u = 0; u < B; ++u) ld_rows(v[u], __shfl_sync(kFull, my_idx, u0 + u));
+    for (int u = 0; u < B; ++u) {
+      ld_rows(v[u], __shfl_sync(kFull, my_idx, u0 + u));
+      s[u] = SC ? __shfl_sync(kFull, my_sc, u0 + u) : 1.f;
+    }
 #pragma unroll
-    for (int u = 0; u < B; ++u) add(v[u]);
+    for (int u = 0; u < B; ++u) add(v[u], s[u]);
   }
 
   // one row / one segment of n_e entries: 32 indices per coalesced load (the next 32 prefetched), U rows in flight
   __device__ __forceinline__ void long_row(const uint32_t* __restrict__ pidx, int n_e, int lane) {
     uint32_t nxt = lane < n_e ? __ldcs(pidx + lane) : 0u;
+    float nxt_sc = (SC && lane < n_e) ? scale_of(nxt) : 1.f;
 #pragma unroll 1
     for (int base = 0; base < n_e; base += 32) {
       const uint32_t my_idx = nxt;
-      if (base + 32 + lane < n_e) nxt = __ldcs(pidx + base + 32 + lane);
+      const float my_sc = nxt_sc;
+      if (base + 32 + lane < n_e) {
+        nxt = __ldcs(pidx + base + 32 + lane);
+        if constexpr (SC) nxt_sc = scale_of(nxt);
+      }
       const int n = min(32, n_e - base);
       int u0 = 0;
 #pragma unroll 1
-      for (; u0 + U <= n; u0 += U) batch<U>(my_idx, u0);
+      for (; u0 + U <= n; u0 += U) batch<U>(my_idx, my_sc, u0);
       // ragged end of the row: 4 + 2 + 1 neighbour rows, no predicated loads
-      if (n - u0 >= 4) { batch<4>(my_idx, u0); u0 += 4; }
-      if (n - u0 >= 2) { batch<2>(my_idx, u0); u0 += 2; }
-      if (n - u0 >= 1) { batch<1>(my_idx, u0); }
+      if (n - u0 >= 4) { batch<4>(my_idx, my_sc, u0); u0 += 4; }
+      if (n - u0 >= 2) { batch<2>(my_idx, my_sc, u0); u0 += 2; }
+      if (n - u0 >= 1) { batch<1>(my_idx, my_sc, u0); }
     }
   }
 };
 
 template <typename A, typename T>
 __device__ __forceinline__ void agg2_setup(A& a, const T* x, uint32_t ldx_bytes, T* out, int64_t ldo, int acc_rows, int nvec,
-                                           const DropArg& drop) {
+                                           const DropArg& drop, const ScaleArg& sc) {
+  if constexpr (A::kSC) a.sc = sc;
   a.ldx_bytes = ldx_bytes;
   a.out = out;
   a.ldo = ldo;
@@ -411,11 +497,12 @@ __device__ __forceinline__ void agg2_columns(A& a, const T* x, int c0, int lane,
 }
 
 // chunks [0, n_chunks_long): one row (kind 1) or one segment of a long row (kind 2) per warp
-template <typename T, int VB, int VPL, int U, bool HINT, int OCC>
-__global__ void __launch_bounds__(256, (VPL == 1 ? OCC : (VPL == 2 ? 2 : 1)))
+template <typename T, int VB, int VPL, int U, bool HINT, int OCC, bool SC>
+__global__ void __launch_bounds__(256, (VPL == 1 ? (SC ? (HINT ? 2 : 3) : OCC) : (VPL == 2 ? 2 : 1)))
 agg2_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict__ out, int64_t ldo, int nvec,
-                 const float* __restrict__ row_div, int acc_rows, float* __restrict__ scratch, int64_t lds, DropArg drop) {
-  using A = Agg2<T, VB, VPL, U, HINT>;
+                 const float* __restrict__ row_div, int acc_rows, float* __restrict__ scratch, int64_t lds, DropArg drop,
+                 ScaleArg sc) {
+  using A = Agg2<T, VB, VPL, U, HINT, SC>;
   constexpr int V = A::V;
   const int lane = threadIdx.x & 31;
   const int cid = blockIdx.x * 8 + (threadIdx.x >> 5);
@@ -423,7 +510,7 @@ agg2_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __res
   const int4 c = __ldcs(reinterpret_cast<const int4*>(g.chunks) + cid);
   const uint32_t* __restrict__ pidx = reinterpret_cast<const uint32_t*>(g.pidx) + c.x;
   A a;
-  agg2_setup(a, x, ldx_bytes, out, ldo, acc_rows, nvec, drop);
+  agg2_setup(a, x, ldx_bytes, out, ldo, acc_rows, nvec, drop, sc);
   if (HINT) {
     a.pol_hot = l2_policy_evict_last();
     a.pol_cold = l2_policy_evict_first();
@@ -442,7 +529,7 @@ agg2_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __res
       }
     } else {
       const int row = __ldg(g.prow + c.z);
-      a.flush(row, row_div != nullptr ? 1.f / __ldg(row_div + row) : 1.f);
+      a.flush(row, row_scale<SC>(row_div, row));
     }
   }
 }
@@ -465,11 +552,12 @@ template <int N> __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
-template <typename T, int VPL, int D, bool HINT>
-__global__ void __launch_bounds__(256, (VPL == 1 ? 6 : 3))
+template <typename T, int VPL, int D, bool HINT, bool SC>
+__global__ void __launch_bounds__(256, (VPL == 1 ? (SC ? 4 : 6) : (SC ? 2 : 3)))
 agg3_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict__ out, int64_t ldo, int nvec,
-                 const float* __restrict__ row_div, int acc_rows, float* __restrict__ scratch, int64_t lds, DropArg drop) {
-  using A = Agg2<T, 16, VPL, 1, HINT>;
+                 const float* __restrict__ row_div, int acc_rows, float* __restrict__ scratch, int64_t lds, DropArg drop,
+                 ScaleArg sc) {
+  using A = Agg2<T, 16, VPL, 1, HINT, SC>;
   using Raw = typename A::Raw;
   constexpr int V = A::V;
   constexpr unsigned kFull = 0xffffffffu;
@@ -484,7 +572,7 @@ agg3_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __res
   // this lane's 16 bytes of slot 0 (piece j at + j * 512)
   const uint32_t ring = static_cast<uint32_t>(__cvta_generic_to_shared(agg3_ring)) + warp * (D * kSlotBytes) + lane * 16;
   A a;
-  agg2_setup(a, x, ldx_bytes, out, ldo, acc_rows, nvec, drop);
+  agg2_setup(a, x, ldx_bytes, out, ldo, acc_rows, nvec, drop, sc);
   if (HINT) {
     a.pol_hot = l2_policy_evict_last();
     a.pol_cold = l2_policy_evict_first();
@@ -502,6 +590,7 @@ agg3_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __res
     agg2_columns(a, x, c0, lane, nvec);
     uint32_t idx_a = lane < n_e ? __ldcs(pidx + lane) : 0u;
     uint32_t idx_b = 32 + lane < n_e ? __ldcs(pidx + 32 + lane) : 0u;
+    float sc_a = (SC && lane < n_e) ? a.scale_of(idx_a) : 1.f;
 #pragma unroll
     for (int k = 0; k < D - 1; ++k) {                       // prologue: rows 0 .. D-2 (all inside the first 32 indices)
       const uint32_t s = __shfl_sync(kFull, idx_a, k);
@@ -524,9 +613,10 @@ agg3_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __res
         for (int j = 0; j < VPL; ++j)
           asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];"
                        : "=r"(v[j].x), "=r"(v[j].y), "=r"(v[j].z), "=r"(v[j].w) : "r"(src + j * 512));
-        a.add(v);
+        a.add(v, SC ? __shfl_sync(kFull, sc_a, u) : 1.f);
       }
       idx_a = idx_b;
+      if constexpr (SC) sc_a = base + 32 + lane < n_e ? a.scale_of(idx_a) : 1.f;
       idx_b = base + 64 + lane < n_e ? __ldcs(pidx + base + 64 + lane) : 0u;
     }
     if ((c.w & 3) == 2) {
@@ -540,38 +630,40 @@ agg3_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __res
       }
     } else {
       const int row = __ldg(g.prow + c.z);
-      a.flush(row, row_div != nullptr ? 1.f / __ldg(row_div + row) : 1.f);
+      a.flush(row, row_scale<SC>(row_div, row));
     }
   }
 }
 
 // chunks [n_chunks_long, n_chunks): n_rows whole rows of equal length (<= 32 entries together) per warp
-template <typename T, int VB, int VPL, int U, bool HINT>
-__global__ void __launch_bounds__(256, (VPL == 1 ? 4 : (VPL == 2 ? 2 : 1)))
+template <typename T, int VB, int VPL, int U, bool HINT, bool SC>
+__global__ void __launch_bounds__(256, (VPL == 1 ? (SC ? (HINT ? 2 : 3) : 4) : (VPL == 2 ? 2 : 1)))
 agg2_small_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict__ out, int64_t ldo, int nvec,
-                  const float* __restrict__ row_div, int acc_rows, DropArg drop) {
-  using A = Agg2<T, VB, VPL, U, HINT>;
+                  const float* __restrict__ row_div, int acc_rows, DropArg drop, ScaleArg sc) {
+  using A = Agg2<T, VB, VPL, U, HINT, SC>;
   const int lane = threadIdx.x & 31;
   const int cid = g.n_chunks_long + blockIdx.x * 8 + (threadIdx.x >> 5);
   if (cid >= g.n_chunks) return;
   const int4 c = __ldcs(reinterpret_cast<const int4*>(g.chunks) + cid);
   const int n_rows = c.w >> 2, len = c.y, n_e = len * n_rows;
   const uint32_t my_idx = lane < n_e ? __ldcs(reinterpret_cast<const uint32_t*>(g.pidx) + c.x + lane) : 0u;
+  const float my_sc = (SC && lane < n_e) ? __ldg(sc.src + (my_idx & 0x7fffffffu)) : 1.f;
   int my_row = 0;
   float my_inv = 1.f;
   if (lane < n_rows) {
     my_row = __ldg(g.prow + c.z + lane);
-    if (row_div != nullptr) my_inv = 1.f / __ldg(row_div + my_row);
+    if constexpr (SC) my_inv = __ldg(row_div + my_row);
+    else if (row_div != nullptr) my_inv = 1.f / __ldg(row_div + my_row);
   }
   A a;
-  agg2_setup(a, x, ldx_bytes, out, ldo, acc_rows, nvec, drop);
+  agg2_setup(a, x, ldx_bytes, out, ldo, acc_rows, nvec, drop, sc);
   if (HINT) {
     a.pol_hot = l2_policy_evict_last();
     a.pol_cold = l2_policy_evict_first();
   }
   for (int c0 = 0; c0 < nvec; c0 += 32 * VPL) {
     agg2_columns(a, x, c0, lane, nvec);
-    a.small_chunk(my_idx, my_row, my_inv, n_rows, len);
+    a.small_chunk(my_idx, my_sc, my_row, my_inv, n_rows, len);
   }
 }
 
@@ -583,7 +675,7 @@ agg2_small_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __re
 //   chunks of short rows : lane group q takes the rows q, q + R, ... of the chunk; all groups walk rows of the same
 //                          length, so the flush points are warp-uniform and only the stores are predicated
 // Same chunk plan, same coalesced index loads + shuffles as the full-width kernels.
-template <typename T, int VB, int G>
+template <typename T, int VB, int G, bool SC>
 struct AggN {
   using P = Pack<T, VB>;
   using Raw = typename P::Raw;
@@ -591,6 +683,7 @@ struct AggN {
   static constexpr int NA = P::NA;
   static constexpr int R = 32 / G;
   static constexpr int U = 8;
+  static constexpr bool kSC = SC;
   static constexpr unsigned kFull = 0xffffffffu;
   const char* xc;           // this lane's column of source row 0
   bool act;                 // lane's column exists
@@ -600,6 +693,7 @@ struct AggN {
   int col, q, acc_rows, nvec;
   DropArg drop;
   uint32_t drop_hi;
+  ScaleOf<SC> sc;
   float2 acc[NA];
 
   __device__ __forceinline__ void zero() {
@@ -609,12 +703,20 @@ struct AggN {
   __device__ __forceinline__ Raw ld_row(uint32_t s) const {
     return ld_vec<VB>(xc + static_cast<uint64_t>(s & 0x7fffffffu) * ldx_bytes);
   }
-  __device__ __forceinline__ void add_masked(Raw t, bool keep) {
+  __device__ __forceinline__ void add(const Raw& t, float s) {
+    if constexpr (SC) P::fma(acc, t, s);
+    else P::add(acc, t);
+  }
+  __device__ __forceinline__ void add_masked(Raw t, bool keep, float s) {
     const uint32_t m = keep ? 0xffffffffu : 0u;
     uint32_t* w = reinterpret_cast<uint32_t*>(&t);
 #pragma unroll
     for (int i = 0; i < VB / 4; ++i) w[i] &= m;
-    P::add(acc, t);
+    add(t, s);
+  }
+  __device__ __forceinline__ float scale_of(uint32_t id) const {
+    if constexpr (SC) return __ldg(sc.src + (id & 0x7fffffffu));
+    else return 1.f;
   }
   __device__ __forceinline__ void store(int row, float inv, bool valid) {
     if (valid && act) {
@@ -622,6 +724,7 @@ struct AggN {
       float r[V];
 #pragma unroll
       for (int i = 0; i < V; ++i) r[i] = ((i & 1) ? acc[i / 2].y : acc[i / 2].x) * inv;
+      add_bias<SC, V>(r, sc, static_cast<int64_t>(col) * V);
       if (row < acc_rows) {
         float ov[V];
         P::unpack(*reinterpret_cast<const Raw*>(op), ov);
@@ -648,7 +751,8 @@ struct AggN {
 
 template <typename A, typename T>
 __device__ __forceinline__ void aggn_setup(A& a, const T* x, uint32_t ldx_bytes, T* out, int64_t ldo, int acc_rows, int nvec,
-                                           const DropArg& drop, int lane) {
+                                           const DropArg& drop, const ScaleArg& sc, int lane) {
+  if constexpr (A::kSC) a.sc = sc;
   constexpr int G = 32 / A::R;
   a.col = lane % G;
   a.q = lane / G;
@@ -664,11 +768,12 @@ __device__ __forceinline__ void aggn_setup(A& a, const T* x, uint32_t ldx_bytes,
   a.zero();
 }
 
-template <typename T, int VB, int G>
-__global__ void __launch_bounds__(256, 4)
+template <typename T, int VB, int G, bool SC>
+__global__ void __launch_bounds__(256, SC ? (G == 16 ? 2 : 3) : 4)
 aggn_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict__ out, int64_t ldo, int nvec,
-                 const float* __restrict__ row_div, int acc_rows, float* __restrict__ scratch, int64_t lds, DropArg drop) {
-  using A = AggN<T, VB, G>;
+                 const float* __restrict__ row_div, int acc_rows, float* __restrict__ scratch, int64_t lds, DropArg drop,
+                 ScaleArg sc) {
+  using A = AggN<T, VB, G, SC>;
   using Raw = typename A::Raw;
   constexpr int V = A::V, R = A::R, U = A::U;
   constexpr unsigned kFull = 0xffffffffu;
@@ -679,25 +784,34 @@ aggn_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __res
   const uint32_t* __restrict__ pidx = reinterpret_cast<const uint32_t*>(g.pidx) + c.x;
   const int n_e = c.y;
   A a;
-  aggn_setup(a, x, ldx_bytes, out, ldo, acc_rows, nvec, drop, lane);
+  aggn_setup(a, x, ldx_bytes, out, ldo, acc_rows, nvec, drop, sc, lane);
   uint32_t nxt = lane < n_e ? __ldcs(pidx + lane) : 0u;
+  float nxt_sc = (SC && lane < n_e) ? a.scale_of(nxt) : 1.f;
 #pragma unroll 1
   for (int base = 0; base < n_e; base += 32) {
     const uint32_t my_idx = nxt;                          // lanes past the end hold column 0: a valid row
-    if (base + 32 + lane < n_e) nxt = __ldcs(pidx + base + 32 + lane);
+    const float my_sc = nxt_sc;
+    if (base + 32 + lane < n_e) {
+      nxt = __ldcs(pidx + base + 32 + lane);
+      if constexpr (SC) nxt_sc = a.scale_of(nxt);
+    }
     const int n = min(32, n_e - base);
     // step u of this block: group q fetches entry u * R + q
 #pragma unroll 1
     for (int u0 = 0; u0 * R < n; u0 += U) {
       Raw v[U];
+      float s[U];
 #pragma unroll
-      for (int u = 0; u < U; ++u) v[u] = a.ld_row(__shfl_sync(kFull, my_idx, ((u0 + u) * R + a.q) & 31));
+      for (int u = 0; u < U; ++u) {
+        v[u] = a.ld_row(__shfl_sync(kFull, my_idx, ((u0 + u) * R + a.q) & 31));
+        s[u] = SC ? __shfl_sync(kFull, my_sc, ((u0 + u) * R + a.q) & 31) : 1.f;
+      }
       if (n == 32 && (u0 + U) * R <= 32) {
 #pragma unroll
-        for (int u = 0; u < U; ++u) A::P::add(a.acc, v[u]);
+        for (int u = 0; u < U; ++u) a.add(v[u], s[u]);
       } else {
 #pragma unroll
-        for (int u = 0; u < U; ++u) a.add_masked(v[u], (u0 + u) * R + a.q < n);
+        for (int u = 0; u < U; ++u) a.add_masked(v[u], (u0 + u) * R + a.q < n, s[u]);
       }
     }
   }
@@ -710,15 +824,15 @@ aggn_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __res
     }
   } else {
     const int row = __ldg(g.prow + c.z);
-    a.store(row, row_div != nullptr ? 1.f / __ldg(row_div + row) : 1.f, a.q == 0);
+    a.store(row, row_scale<SC>(row_div, row), a.q == 0);
   }
 }
 
-template <typename T, int VB, int G>
-__global__ void __launch_bounds__(256, 4)
+template <typename T, int VB, int G, bool SC>
+__global__ void __launch_bounds__(256, SC ? (G == 16 ? 2 : 3) : 4)
 aggn_small_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict__ out, int64_t ldo, int nvec,
-                  const float* __restrict__ row_div, int acc_rows, DropArg drop) {
-  using A = AggN<T, VB, G>;
+                  const float* __restrict__ row_div, int acc_rows, DropArg drop, ScaleArg sc) {
+  using A = AggN<T, VB, G, SC>;
   using Raw = typename A::Raw;
   constexpr int R = A::R, U = A::U;
   constexpr unsigned kFull = 0xffffffffu;
@@ -728,14 +842,16 @@ aggn_small_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __re
   const int4 c = __ldcs(reinterpret_cast<const int4*>(g.chunks) + cid);
   const int n_rows = c.w >> 2, len = c.y, n_e = len * n_rows;
   const uint32_t my_idx = lane < n_e ? __ldcs(reinterpret_cast<const uint32_t*>(g.pidx) + c.x + lane) : 0u;
+  const float my_sc = (SC && lane < n_e) ? __ldg(sc.src + (my_idx & 0x7fffffffu)) : 1.f;
   int my_row = 0;
   float my_inv = 1.f;
   if (lane < n_rows) {
     my_row = __ldg(g.prow + c.z + lane);
-    if (row_div != nullptr) my_inv = 1.f / __ldg(row_div + my_row);
+    if constexpr (SC) my_inv = __ldg(row_div + my_row);
+    else if (row_div != nullptr) my_inv = 1.f / __ldg(row_div + my_row);
   }
   A a;
-  aggn_setup(a, x, ldx_bytes, out, ldo, acc_rows, nvec, drop, lane);
+  aggn_setup(a, x, ldx_bytes, out, ldo, acc_rows, nvec, drop, sc, lane);
   // group q walks the rows q, q + R, ...: T rows of `len` entries each, the same positions in every group
   const int t_rows = (n_rows + R - 1) / R;
   if (len == 0) {
@@ -751,17 +867,19 @@ aggn_small_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __re
 #pragma unroll 1
   for (int p0 = 0; p0 < n_pos; p0 += U) {
     Raw v[U];
+    float s[U];
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       const int rq = t_ld * R + a.q;
       v[u] = a.ld_row(__shfl_sync(kFull, my_idx, (rq * len + k_ld) & 31));      // lanes >= n_e hold column 0
+      s[u] = SC ? __shfl_sync(kFull, my_sc, (rq * len + k_ld) & 31) : 1.f;
       if (++k_ld == len) { k_ld = 0; ++t_ld; }
     }
 #pragma unroll
     for (int u = 0; u < U; ++u) {
       if (p0 + u < n_pos) {                                 // warp-uniform
         const int rq = t_add * R + a.q;
-        a.add_masked(v[u], rq < n_rows);
+        a.add_masked(v[u], rq < n_rows, s[u]);
         if (++k_add == len) {
           a.store(__shfl_sync(kFull, my_row, rq & 31), __shfl_sync(kFull, my_inv, rq & 31), rq < n_rows);
           k_add = 0;
@@ -772,9 +890,9 @@ aggn_small_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __re
   }
 }
 
-template <typename T, int VB, int G>
+template <typename T, int VB, int G, bool SC>
 static int launch_aggn(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec, const float* row_div,
-                       int acc_rows, float* scratch, int64_t lds, const DropArg& da, cudaStream_t st);
+                       int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st);
 
 // The long-row kernel is bound by instruction issue and L2 bandwidth, the short-row kernel by DRAM latency (it
 // touches the cold sources and writes most of the output): they run side by side, the short rows on a side stream
@@ -798,9 +916,9 @@ static AggSide* agg_side_for(cudaStream_t st) {
   return &e;
 }
 
-template <typename T, int VB, int VPL, bool HINT>
+template <typename T, int VB, int VPL, bool HINT, bool SC>
 static int launch_agg2h(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec,
-                        const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, cudaStream_t st) {
+                        const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st) {
   constexpr int U = (VPL >= 4) ? 2 : (VPL == 2 ? 4 : 8);
   const uint32_t ldxb = static_cast<uint32_t>(ldx * sizeof(T));
   AggSide* side = nullptr;
@@ -812,7 +930,7 @@ static int launch_agg2h(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_
       PG_CHECK_CUDA(cudaStreamWaitEvent(side->side, side->fork, 0));
       ss = side->side;
     }
-    agg2_small_kernel<T, VB, VPL, U, HINT><<<blocks, 256, 0, ss>>>(g, x, ldxb, out, ldo, nvec, row_div, acc_rows, da);
+    agg2_small_kernel<T, VB, VPL, U, HINT, SC><<<blocks, 256, 0, ss>>>(g, x, ldxb, out, ldo, nvec, row_div, acc_rows, da, sc);
     PG_LAUNCH_CHECK();
     if (side != nullptr) PG_CHECK_CUDA(cudaEventRecord(side->join, ss));
   }
@@ -822,31 +940,31 @@ static int launch_agg2h(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_
     const size_t smem = static_cast<size_t>(8) * D * VPL * 512;
     static bool attr_done = false;
     if (!attr_done) {
-      PG_CHECK_CUDA(cudaFuncSetAttribute(agg3_long_kernel<T, VPL, D, HINT>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
-      PG_CHECK_CUDA(cudaFuncSetAttribute(agg3_long_kernel<T, VPL, D, HINT>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
+      PG_CHECK_CUDA(cudaFuncSetAttribute(agg3_long_kernel<T, VPL, D, HINT, SC>, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+      PG_CHECK_CUDA(cudaFuncSetAttribute(agg3_long_kernel<T, VPL, D, HINT, SC>, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
       attr_done = true;
     }
-    agg3_long_kernel<T, VPL, D, HINT><<<blocks, 256, smem, st>>>(g, x, ldxb, out, ldo, nvec, row_div, acc_rows, scratch, lds, da);
+    agg3_long_kernel<T, VPL, D, HINT, SC><<<blocks, 256, smem, st>>>(g, x, ldxb, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc);
     PG_LAUNCH_CHECK();
   } else if (g.n_chunks_long > 0) {
     const unsigned blocks = static_cast<unsigned>((g.n_chunks_long + 7) / 8);
     if (VPL == 1 && g_agg_occ == 5)
-      agg2_long_kernel<T, VB, VPL, U, HINT, (VPL == 1 ? 5 : 4)><<<blocks, 256, 0, st>>>(g, x, ldxb, out, ldo, nvec, row_div, acc_rows, scratch, lds, da);
+      agg2_long_kernel<T, VB, VPL, U, HINT, (VPL == 1 && !SC ? 5 : 4), SC><<<blocks, 256, 0, st>>>(g, x, ldxb, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc);
     else
-      agg2_long_kernel<T, VB, VPL, U, HINT, 4><<<blocks, 256, 0, st>>>(g, x, ldxb, out, ldo, nvec, row_div, acc_rows, scratch, lds, da);
+      agg2_long_kernel<T, VB, VPL, U, HINT, 4, SC><<<blocks, 256, 0, st>>>(g, x, ldxb, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc);
     PG_LAUNCH_CHECK();
   }
   if (g.n_long > 0) {
-    agg_fixup_kernel<T, VB><<<g.n_long, 256, 0, st>>>(g, out, ldo, nvec, row_div, acc_rows, scratch, lds, da);
+    agg_fixup_kernel<T, VB, SC><<<g.n_long, 256, 0, st>>>(g, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc);
     PG_LAUNCH_CHECK();
   }
   if (side != nullptr) PG_CHECK_CUDA(cudaStreamWaitEvent(st, side->join, 0));
   return PG_OK;
 }
 
-template <typename T, int VB, int G>
+template <typename T, int VB, int G, bool SC>
 static int launch_aggn(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec, const float* row_div,
-                       int acc_rows, float* scratch, int64_t lds, const DropArg& da, cudaStream_t st) {
+                       int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st) {
   const uint32_t ldxb = static_cast<uint32_t>(ldx * sizeof(T));
   AggSide* side = nullptr;
   if (g.n_chunks > g.n_chunks_long) {
@@ -857,77 +975,77 @@ static int launch_aggn(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t
       PG_CHECK_CUDA(cudaStreamWaitEvent(side->side, side->fork, 0));
       ss = side->side;
     }
-    aggn_small_kernel<T, VB, G><<<blocks, 256, 0, ss>>>(g, x, ldxb, out, ldo, nvec, row_div, acc_rows, da);
+    aggn_small_kernel<T, VB, G, SC><<<blocks, 256, 0, ss>>>(g, x, ldxb, out, ldo, nvec, row_div, acc_rows, da, sc);
     PG_LAUNCH_CHECK();
     if (side != nullptr) PG_CHECK_CUDA(cudaEventRecord(side->join, ss));
   }
   if (g.n_chunks_long > 0) {
     const unsigned blocks = static_cast<unsigned>((g.n_chunks_long + 7) / 8);
-    aggn_long_kernel<T, VB, G><<<blocks, 256, 0, st>>>(g, x, ldxb, out, ldo, nvec, row_div, acc_rows, scratch, lds, da);
+    aggn_long_kernel<T, VB, G, SC><<<blocks, 256, 0, st>>>(g, x, ldxb, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc);
     PG_LAUNCH_CHECK();
   }
   if (g.n_long > 0) {
-    agg_fixup_kernel<T, VB><<<g.n_long, 256, 0, st>>>(g, out, ldo, nvec, row_div, acc_rows, scratch, lds, da);
+    agg_fixup_kernel<T, VB, SC><<<g.n_long, 256, 0, st>>>(g, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc);
     PG_LAUNCH_CHECK();
   }
   if (side != nullptr) PG_CHECK_CUDA(cudaStreamWaitEvent(st, side->join, 0));
   return PG_OK;
 }
 
-template <typename T, int VB, int VPL>
+template <typename T, int VB, int VPL, bool SC>
 static int launch_agg2(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec,
-                       const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, cudaStream_t st) {
-  if (g_agg_l2_hint) return launch_agg2h<T, VB, VPL, true>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, st);
-  return launch_agg2h<T, VB, VPL, false>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, st);
+                       const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st) {
+  if (g_agg_l2_hint) return launch_agg2h<T, VB, VPL, true, SC>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st);
+  return launch_agg2h<T, VB, VPL, false, SC>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st);
 }
 
 int g_agg_pack_short = 0;   // pg_set_option("agg_pack_short", 0|1): 16 lanes x 2 vectors per row when rows are short.
                             // OFF by default; not measured on H100
 
-template <typename T, int VB, int G, int VPL, int U>
+template <typename T, int VB, int G, int VPL, int U, bool SC>
 static int launch_agg_u(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec,
-                        const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, cudaStream_t st);
+                        const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st);
 
-template <typename T, int VB, int G, int VPL>
+template <typename T, int VB, int G, int VPL, bool SC>
 static int launch_agg(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec,
-                      const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, cudaStream_t st) {
+                      const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st) {
   if (VPL == 1 && g_agg_unroll == 4)
-    return launch_agg_u<T, VB, G, VPL, 4>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, st);
+    return launch_agg_u<T, VB, G, VPL, 4, SC>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st);
   constexpr int U = (VPL >= 4) ? 2 : (VPL == 2 ? 4 : 8);
-  return launch_agg_u<T, VB, G, VPL, U>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, st);
+  return launch_agg_u<T, VB, G, VPL, U, SC>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st);
 }
 
-template <typename T, int VB, int G, int VPL, int U>
+template <typename T, int VB, int G, int VPL, int U, bool SC>
 static int launch_agg_u(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec,
-                        const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, cudaStream_t st) {
+                        const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st) {
   constexpr int GROUPS = 256 / G;
   const int64_t n_items = static_cast<int64_t>(g.n_rows) + g.n_seg;
   if (n_items > 0) {
     const int64_t blocks = (n_items + GROUPS - 1) / GROUPS;
-    agg_kernel<T, VB, G, VPL, U><<<static_cast<unsigned>(blocks), 256, 0, st>>>(g, x, static_cast<uint32_t>(ldx * sizeof(T)), out, ldo, nvec, row_div,
-                                                                                acc_rows, scratch, lds, da);
+    agg_kernel<T, VB, G, VPL, U, SC><<<static_cast<unsigned>(blocks), 256, 0, st>>>(g, x, static_cast<uint32_t>(ldx * sizeof(T)), out, ldo, nvec, row_div,
+                                                                                acc_rows, scratch, lds, da, sc);
     PG_LAUNCH_CHECK();
   }
   if (g.n_long > 0) {
-    agg_fixup_kernel<T, VB><<<g.n_long, 256, 0, st>>>(g, out, ldo, nvec, row_div, acc_rows, scratch, lds, da);
+    agg_fixup_kernel<T, VB, SC><<<g.n_long, 256, 0, st>>>(g, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc);
     PG_LAUNCH_CHECK();
   }
   return PG_OK;
 }
 
-template <typename T, int VB>
+template <typename T, int VB, bool SC>
 static int dispatch_agg(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec,
-                        const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, cudaStream_t st) {
-#define PG_AGG(G_, VPL_) return launch_agg<T, VB, G_, VPL_>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, st)
+                        const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st) {
+#define PG_AGG(G_, VPL_) return launch_agg<T, VB, G_, VPL_, SC>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st)
   if (g_agg_impl >= 2 && g.chunks != nullptr && nvec > 16) {
-    if (nvec <= 32) return launch_agg2<T, VB, 1>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, st);
-    if (nvec <= 64) return launch_agg2<T, VB, 2>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, st);
-    return launch_agg2<T, VB, 4>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, st);
+    if (nvec <= 32) return launch_agg2<T, VB, 1, SC>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st);
+    if (nvec <= 64) return launch_agg2<T, VB, 2, SC>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st);
+    return launch_agg2<T, VB, 4, SC>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st);
   }
   if (g_agg_impl >= 2 && g.chunks != nullptr && g_agg_narrow) {
-    if (nvec <= 4) return launch_aggn<T, VB, 4>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, st);
-    if (nvec <= 8) return launch_aggn<T, VB, 8>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, st);
-    return launch_aggn<T, VB, 16>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, st);
+    if (nvec <= 4) return launch_aggn<T, VB, 4, SC>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st);
+    if (nvec <= 8) return launch_aggn<T, VB, 8, SC>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st);
+    return launch_aggn<T, VB, 16, SC>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st);
   }
   if (nvec <= 4) PG_AGG(4, 1);
   if (nvec <= 8) PG_AGG(8, 1);
@@ -941,9 +1059,9 @@ static int dispatch_agg(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_
 #undef PG_AGG
 }
 
-template <typename T>
+template <typename T, bool SC>
 static int aggregate_t(const pg_csr& g, const void* x, int64_t ldx, void* out, int64_t ldo, int d,
-                       const float* row_div, int acc_rows, float* scratch, const DropArg& da, cudaStream_t st) {
+                       const float* row_div, int acc_rows, float* scratch, const DropArg& da, const ScaleArg& sc, cudaStream_t st) {
   const int es = sizeof(T);
   int vb = min(vec_bytes(x, ldx, es), vec_bytes(out, ldo, es));
   // a vector must not straddle two rows: either d is a multiple of the vector or both strides leave room
@@ -961,9 +1079,9 @@ static int aggregate_t(const pg_csr& g, const void* x, int64_t ldx, void* out, i
   const T* xp = static_cast<const T*>(x);
   T* op = static_cast<T*>(out);
   switch (vb) {
-    case 16: return dispatch_agg<T, 16>(g, xp, ldx, op, ldo, nvec, row_div, acc_rows, scratch, lds, da, st);
-    case 8: return dispatch_agg<T, 8>(g, xp, ldx, op, ldo, nvec, row_div, acc_rows, scratch, lds, da, st);
-    case 4: return dispatch_agg<T, 4>(g, xp, ldx, op, ldo, nvec, row_div, acc_rows, scratch, lds, da, st);
+    case 16: return dispatch_agg<T, 16, SC>(g, xp, ldx, op, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st);
+    case 8: return dispatch_agg<T, 8, SC>(g, xp, ldx, op, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st);
+    case 4: return dispatch_agg<T, 4, SC>(g, xp, ldx, op, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st);
     default:
       set_error("pg_aggregate: rows must be at least 4-byte aligned (vector width %d)", vb);
       return PG_ERR_INVALID;
@@ -1017,6 +1135,49 @@ static int row_div_t(const void* x, int64_t ldx, void* out, int64_t ldo, int n_r
   }
   PG_LAUNCH_CHECK();
   return PG_OK;
+}
+
+// CUDA loads kernels lazily, and loading one may wait for the device: every SC instantiation is loaded at the first
+// pg_aggregate_scaled call (or pg_aggregate_scaled_preload), before a halo wait of a simulated rank can spin
+template <typename T, int VB, int VPL, bool HINT>
+static void preload_agg2(cudaFuncAttributes* a) {
+  constexpr int U = (VPL >= 4) ? 2 : (VPL == 2 ? 4 : 8);
+  constexpr int D = (VPL >= 4) ? 4 : 8;
+  cudaFuncGetAttributes(a, agg2_small_kernel<T, VB, VPL, U, HINT, true>);
+  cudaFuncGetAttributes(a, agg2_long_kernel<T, VB, VPL, U, HINT, 4, true>);
+  cudaFuncGetAttributes(a, agg3_long_kernel<T, VPL, D, HINT, true>);
+}
+template <typename T, int VB>
+static void preload_vb(cudaFuncAttributes* a) {
+  preload_agg2<T, VB, 1, false>(a); preload_agg2<T, VB, 2, false>(a); preload_agg2<T, VB, 4, false>(a);
+  preload_agg2<T, VB, 1, true>(a); preload_agg2<T, VB, 2, true>(a); preload_agg2<T, VB, 4, true>(a);
+  cudaFuncGetAttributes(a, aggn_small_kernel<T, VB, 4, true>);
+  cudaFuncGetAttributes(a, aggn_small_kernel<T, VB, 8, true>);
+  cudaFuncGetAttributes(a, aggn_small_kernel<T, VB, 16, true>);
+  cudaFuncGetAttributes(a, aggn_long_kernel<T, VB, 4, true>);
+  cudaFuncGetAttributes(a, aggn_long_kernel<T, VB, 8, true>);
+  cudaFuncGetAttributes(a, aggn_long_kernel<T, VB, 16, true>);
+  cudaFuncGetAttributes(a, agg_fixup_kernel<T, VB, true>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 4, 1, 8, true>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 4, 1, 4, true>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 8, 1, 8, true>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 8, 1, 4, true>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 16, 1, 8, true>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 16, 1, 4, true>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 16, 2, 4, true>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 32, 1, 8, true>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 32, 1, 4, true>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 32, 2, 4, true>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 32, 4, 2, true>);
+}
+static void aggregate_scaled_preload() {
+  static std::once_flag once;
+  std::call_once(once, [] {
+    cudaFuncAttributes a;
+    preload_vb<float, 16>(&a); preload_vb<float, 8>(&a); preload_vb<float, 4>(&a);
+    preload_vb<__nv_bfloat16, 16>(&a); preload_vb<__nv_bfloat16, 8>(&a); preload_vb<__nv_bfloat16, 4>(&a);
+    cudaGetLastError();
+  });
 }
 
 }  // namespace pg
@@ -1084,10 +1245,35 @@ extern "C" int pg_aggregate_drop(const pg_csr* g, const void* x, int64_t ldx, vo
   PG_REQUIRE(g->n_rows >= 0 && g->seg_len > 0 && d > 0, "pg_aggregate: bad sizes (n_rows=%d seg_len=%d d=%d)", g->n_rows, g->seg_len, d);
   PG_REQUIRE(ldx >= d && ldo >= d && ldx < (1ll << 29), "pg_aggregate: row stride smaller than d (or >= 2^29 elements)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (dtype == PG_F32) return pg::aggregate_t<float>(*g, x, ldx, out, ldo, d, row_div, acc_rows, scratch, da, st);
-  if (dtype == PG_BF16) return pg::aggregate_t<__nv_bfloat16>(*g, x, ldx, out, ldo, d, row_div, acc_rows, scratch, da, st);
+  const pg::ScaleArg sc{nullptr, nullptr, 0};
+  if (dtype == PG_F32) return pg::aggregate_t<float, false>(*g, x, ldx, out, ldo, d, row_div, acc_rows, scratch, da, sc, st);
+  if (dtype == PG_BF16)
+    return pg::aggregate_t<__nv_bfloat16, false>(*g, x, ldx, out, ldo, d, row_div, acc_rows, scratch, da, sc, st);
   pg::set_error("pg_aggregate: unknown dtype %d", dtype);
   return PG_ERR_INVALID;
+}
+
+extern "C" int pg_aggregate_scaled(const pg_csr* g, const void* x, int64_t ldx, void* out, int64_t ldo, int32_t d,
+                                   int dtype, const float* src_scale, const float* dst_scale, const float* bias,
+                                   float* scratch, const pg_drop* drop, void* stream) {
+  const pg::DropArg da = pg::make_drop(drop);
+  PG_REQUIRE(g && x && out && src_scale && dst_scale, "pg_aggregate_scaled: null argument");
+  PG_REQUIRE(g->n_rows >= 0 && g->seg_len > 0 && d > 0, "pg_aggregate_scaled: bad sizes (n_rows=%d seg_len=%d d=%d)",
+             g->n_rows, g->seg_len, d);
+  PG_REQUIRE(ldx >= d && ldo >= d && ldx < (1ll << 29), "pg_aggregate_scaled: row stride smaller than d (or >= 2^29 elements)");
+  pg::aggregate_scaled_preload();
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const pg::ScaleArg sc{src_scale, bias, d};
+  if (dtype == PG_F32) return pg::aggregate_t<float, true>(*g, x, ldx, out, ldo, d, dst_scale, 0, scratch, da, sc, st);
+  if (dtype == PG_BF16)
+    return pg::aggregate_t<__nv_bfloat16, true>(*g, x, ldx, out, ldo, d, dst_scale, 0, scratch, da, sc, st);
+  pg::set_error("pg_aggregate_scaled: unknown dtype %d", dtype);
+  return PG_ERR_INVALID;
+}
+
+extern "C" int pg_aggregate_scaled_preload(void) {
+  pg::aggregate_scaled_preload();
+  return PG_OK;
 }
 
 extern "C" int pg_row_div(const void* x, int64_t ldx, void* out, int64_t ldo, int32_t n_rows, int32_t d, int dtype,

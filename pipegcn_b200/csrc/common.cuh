@@ -94,6 +94,16 @@ template <int VB> struct Pack<float, VB> {
       for (int i = 0; i < NA; ++i) acc[i] = add2(acc[i], make_float2(p[2 * i], p[2 * i + 1]));
     }
   }
+  // acc += s * r, one rounding per element (s == 1 gives the bits of `add`)
+  __device__ __forceinline__ static void fma(float2* acc, const Raw& r, float s) {
+    const float* p = reinterpret_cast<const float*>(&r);
+    if constexpr (V == 1) {
+      acc[0].x = __fmaf_rn(s, p[0], acc[0].x);
+    } else {
+#pragma unroll
+      for (int i = 0; i < NA; ++i) acc[i] = fma2(make_float2(s, s), make_float2(p[2 * i], p[2 * i + 1]), acc[i]);
+    }
+  }
 };
 
 template <int VB> struct Pack<__nv_bfloat16, VB> {
@@ -127,6 +137,16 @@ template <int VB> struct Pack<__nv_bfloat16, VB> {
 #pragma unroll
       for (int i = 0; i < NA; ++i)
         acc[i] = add2(acc[i], make_float2(__uint_as_float(w[i] << 16), __uint_as_float(w[i] & 0xffff0000u)));
+    }
+  }
+  __device__ __forceinline__ static void fma(float2* acc, const Raw& r, float s) {
+    if constexpr (V == 1) {
+      acc[0].x = __fmaf_rn(s, __uint_as_float(static_cast<uint32_t>(*reinterpret_cast<const uint16_t*>(&r)) << 16), acc[0].x);
+    } else {
+      const uint32_t* w = reinterpret_cast<const uint32_t*>(&r);
+#pragma unroll
+      for (int i = 0; i < NA; ++i)
+        acc[i] = fma2(make_float2(s, s), make_float2(__uint_as_float(w[i] << 16), __uint_as_float(w[i] & 0xffff0000u)), acc[i]);
     }
   }
 };

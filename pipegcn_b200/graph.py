@@ -174,6 +174,24 @@ class PartGraph:
             self._row_deg_f = (self.fwd.indptr[1:] - self.fwd.indptr[:-1]).to(torch.float32).contiguous()
         return self._row_deg_f
 
+    def set_sym_norm(self, c: torch.Tensor):
+        """GraphConv's c = deg^-1/2 of every [inner | halo] row: fp32 [num_all], the halo rows' values from their
+        owners (`train._sym_norm_steps`).  Set once; captured CUDA graphs read it at this address."""
+        assert c.dtype == torch.float32 and c.is_contiguous() and c.numel() == self.num_all
+        self._sym_c = c
+
+    def sym_norm(self) -> torch.Tensor:
+        """c [num_all] of GraphConv.  A partition's halo rows need their owners' degrees (`set_sym_norm`); a whole
+        graph (num_in == num_all, whole-graph evaluation) takes them from its row degrees."""
+        c = getattr(self, "_sym_c", None)
+        if c is None:
+            if self.num_in != self.num_all:
+                raise RuntimeError("GraphConv on a partition: the halo rows' degrees come from their owners "
+                                   "(train._sym_norm_steps) and have not been exchanged")
+            from .ops import sym_norm
+            c = self._sym_c = sym_norm(self.row_degrees())
+        return c
+
     def num_nodes(self, ntype: str = "_U") -> int:
         if ntype == "_U":
             return self.num_all

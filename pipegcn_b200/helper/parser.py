@@ -21,6 +21,10 @@ that epoch, so the halo exchange moves p times the bytes.  Evaluation always use
 (DGL's GATv2Conv); `--n-heads k` (not in the reference, default 4, suppressed like `--sampling-rate`: read it with
 getattr(args, 'n_heads', 4)) sets the heads per hidden layer of either.
 
+`--model graphconv` (not in the reference) trains Kipf & Welling's graph convolution (DGL's GraphConv, norm='both'):
+every layer aggregates c_v sum_u c_u h_u with c = deg^-1/2, the halo rows' degrees supplied by their owners.  `--model
+gcn` stays the reference's name for GraphSAGE.  It cannot be combined with --aggregator pool or --sampling-rate < 1.
+
 `--halo-bits b` (8 or 4; not in the reference) quantises the per-epoch halo messages of graph layers >= 1, features
 forward and gradients backward: every row travels as b-bit codes with an fp32 (lo, scale), stochastically rounded so
 the message stays unbiased, and the receiver decodes it before anything reads it.  Layer 0, --use-pp and the
@@ -38,7 +42,8 @@ import argparse
 _FLAGS = [
     ("dataset", dict(type=str, default='reddit', help="the input dataset (or synthetic:<shape>)")),
     ("graph-name", dict(type=str, default='')),
-    ("model", dict(type=str, default='graphsage', help="model for training (graphsage | gcn | gat | gatv2)")),
+    ("model", dict(type=str, default='graphsage', help="model for training (graphsage | gcn | gat | gatv2 | graphconv; "
+                                                              "gcn is GraphSAGE)")),
     ("dropout", dict(type=float, default=0.5, help="dropout probability")),
     ("lr", dict(type=float, default=1e-2, help="learning rate")),
     ("n-epochs", dict(type=int, default=200, help="the number of training epochs")),

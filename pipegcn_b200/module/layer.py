@@ -35,6 +35,18 @@ State-dict keys are GATv2Conv's: `fc_src.weight` / `fc_dst.weight` [H*D, d_in], 
 `attn` [1, H, D].  Initialisation is GATv2Conv.reset_parameters, in this draw order, with
 gain = calculate_gain('relu'): xavier_normal_(fc_src.weight), fc_src.bias = 0, xavier_normal_(fc_dst.weight),
 fc_dst.bias = 0, xavier_normal_(attn).
+
+`GraphConvLayer` (not in the reference): DGL's `GraphConv(in, out, norm='both', weight=True, bias=True)` (Kipf & Welling,
+"Semi-Supervised Classification with Graph Convolutional Networks", ICLR 2017), no activation inside, over the same
+rows, with c = clamp(deg, min=1)^(-1/2) of every [inner | halo] row (deg: in-degree with the self loop in the whole
+graph; the halo rows' values come from their owners, `PartGraph.sym_norm`):
+
+    out[v] = c[v] * sum_{u -> v} c[u] h[u] @ W + b
+
+aggregating first when d_in <= d_out, transforming first otherwise (DGL's rule; PG_NARROW=0 always aggregates first).
+State-dict keys are GraphConv's: `weight` [d_in, d_out] (not transposed like nn.Linear), `bias` [d_out].
+Initialisation is GraphConv.reset_parameters, in this draw order: xavier_uniform_(weight), then bias = 0.
+With --use-pp layer 0 multiplies the precomputed rows c[v] * sum_u c[u] x[u] by the same weight.
 """
 import math
 
@@ -99,6 +111,34 @@ class GraphSAGELayer(nn.Module):
             return ops.linear(torch.cat((x, ah), dim=1), self.linear.weight, self.linear.bias)
         return ops.sage_linear(x, ah, self.linear1.weight, self.linear1.bias,
                                self.linear2.weight, self.linear2.bias)
+
+
+class GraphConvLayer(nn.Module):
+    """GraphConv(in_feats, out_feats, norm='both', weight=True, bias=True), no activation inside: module docstring."""
+
+    def __init__(self, in_feats, out_feats, use_pp=False):
+        super().__init__()
+        self.in_feats, self.out_feats, self.use_pp = in_feats, out_feats, use_pp
+        self.weight = nn.Parameter(torch.empty(in_feats, out_feats))
+        self.bias = nn.Parameter(torch.empty(out_feats))
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        """GraphConv.reset_parameters."""
+        nn.init.xavier_uniform_(self.weight)
+        nn.init.zeros_(self.bias)
+
+    def pp_linear(self, pp_feat):
+        """--use-pp layer 0: the precomputed c_v sum_u c_u x_u rows times W, plus b."""
+        return ops.linear(pp_feat, self.weight.t(), self.bias)
+
+    def forward(self, graph, feat, in_deg=None, drop_bwd=None):
+        """`feat`: the [num_all, d_in] rows of `graph`, or with --use-pp (layer 0, training) the precomputed rows;
+        returns the [N_in, d_out] inner rows.  `in_deg` is unused: the norm is `graph.sym_norm()`.  `drop_bwd` as
+        GraphSAGELayer.forward."""
+        if self.use_pp and self.training:
+            return self.pp_linear(feat)
+        return ops.graphconv_layer(feat, graph, graph.sym_norm(), self.weight, self.bias, drop_bwd)
 
 
 class GATLayer(nn.Module):

@@ -22,13 +22,17 @@ and unkept rows are absent from every softmax.
 
 `GATv2(GAT)` (not in the reference) is `GAT` with `GATv2Layer`s (DGL's GATv2Conv): the same heads, keep mask and
 partitioned evaluation; only the graph layers and the kernels they load differ.
+
+`GraphConv(GraphSAGE)` (not in the reference) is the same layer loop with `GraphConvLayer`s (DGL's GraphConv,
+norm='both'): the layers read the symmetric norm from the graph (`PartGraph.sym_norm`) instead of the in-degrees.
+`GCN` stays the reference's name for GraphSAGE.
 """
 import torch
 from torch import nn
 import torch.nn.functional as F
 
 from ..helper import context as ctx
-from .layer import GATLayer, GATv2Layer, GraphSAGELayer
+from .layer import GATLayer, GATv2Layer, GraphConvLayer, GraphSAGELayer
 
 
 class GNNBase(nn.Module):
@@ -167,7 +171,7 @@ class GraphSAGE(GNNBase):
         for i, layer in enumerate(self.layers):
             if i < self.n_graph_layers:
                 if i == 0 and self.use_pp:
-                    h = ops.linear(pp_feat, layer.linear.weight, layer.linear.bias)
+                    h = self._pp_layer0(layer, pp_feat)
                 else:
                     d = layer.in_feats
                     if i > 0 or push0:
@@ -185,8 +189,38 @@ class GraphSAGE(GNNBase):
                 h = out
         return h
 
+    def _pp_layer0(self, layer, pp_feat):
+        """--use-pp layer 0 on its precomputed input rows (partitioned evaluation)."""
+        from .. import ops
+        return ops.linear(pp_feat, layer.linear.weight, layer.linear.bias)
+
 
 GCN = GraphSAGE
+
+
+class GraphConv(GraphSAGE):
+
+    def _graph_layer(self, i, d_in, d_out):
+        return GraphConvLayer(d_in, d_out, use_pp=(self.use_pp and i == 0))
+
+    def _layer_arg(self, in_deg):
+        """GraphConv layers take no degrees: the norm lives on the graph."""
+        return None
+
+    def _pp_layer0(self, layer, pp_feat):
+        return layer.pp_linear(pp_feat)
+
+    def _preload(self):
+        from .. import ops
+        ops.graphconv_preload()
+
+    def forward(self, g, feat, in_deg=None):
+        self._preload()
+        return super().forward(g, feat, in_deg)
+
+    def forward_partitioned(self, g, xch, pp_feat=None, push0=False):
+        self._preload()
+        return (yield from super().forward_partitioned(g, xch, pp_feat, push0))
 
 
 class GAT(GraphSAGE):

@@ -718,6 +718,140 @@ def sage_linear(x, ah, w1, b1, w2, b2) -> torch.Tensor:
     return linear(x, w1, b1) + linear(ah, w2, b2)
 
 
+# ---- graph convolution (GraphConv, norm='both'): the scaled aggregate of csrc/aggregate.cu --------------------------
+def sym_norm(deg: torch.Tensor) -> torch.Tensor:
+    """c = clamp(deg, min=1)^(-1/2) in fp32 as 1 / sqrt(deg): two correctly rounded operations, so every device and
+    the host give the same bits."""
+    d = torch.clamp(deg.to(torch.float32), min=1.0)
+    return torch.div(1.0, torch.sqrt(d)).contiguous()
+
+
+def graphconv_preload():
+    """Load every scaled-aggregate kernel now (see gat_preload)."""
+    _C.check(_C.lib.pg_aggregate_scaled_preload(), "pg_aggregate_scaled_preload")
+
+
+def aggregate_scaled(plan: CsrPlan, x: torch.Tensor, src: torch.Tensor, dst: torch.Tensor, bias: torch.Tensor = None,
+                     drop: DropSpec = None, out: torch.Tensor = None) -> torch.Tensor:
+    """out[r] = dst[r] * sum_{e in row r} src[indices[e]] * x[indices[e]] (+ bias); with `drop` the mask of that key is
+    applied to every row as it is written (pg_aggregate_scaled)."""
+    _rows(x)
+    d = x.shape[1]
+    if out is None:
+        out = alloc_rows(plan.n_rows, d, x.dtype, x.device)
+    _rows(out)
+    assert out.shape[0] == plan.n_rows and out.shape[1] == d and out.dtype == x.dtype
+    assert src.dtype == dst.dtype == torch.float32 and src.is_contiguous() and dst.is_contiguous()
+    assert src.numel() >= x.shape[0] and dst.numel() >= plan.n_rows
+    if bias is not None:
+        bias = bias.detach()
+        assert bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == d and bias.is_cuda
+    scratch = plan.scratch(d)
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_aggregate_scaled(C.byref(plan.c), x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0), d,
+                                        _C.dtype_code(x.dtype), src.data_ptr(), dst.data_ptr(),
+                                        bias.data_ptr() if bias is not None else None,
+                                        scratch.data_ptr() if scratch is not None else None,
+                                        C.byref(drop.c()) if drop is not None and drop.p > 0 else None,
+                                        _C.stream_ptr()), "pg_aggregate_scaled")
+    return out
+
+
+def _graphconv_wgrad(g, x, weight):
+    """dW [in, out] of `x @ W` from wgrad's [out, in]."""
+    return wgrad(g, x).t().contiguous().to(weight.dtype)
+
+
+class GraphConvLayerFn(torch.autograd.Function):
+    """GraphConv (norm='both') aggregating first, d_in <= d_out; c = deg^-1/2 over the [inner | halo] rows:
+
+        ah  = c[:N_in] * (A @ (c * feat))           pg_aggregate_scaled over the CSR
+        out = ah @ W + b                            pg_linear
+
+        g_ah = g @ W^T                              pg_linear
+        g_feat = c * (A^T @ (c[:N_in] * g_ah))      pg_aggregate_scaled over the CSC, dropout backward in its store
+        gW = ah^T g, gb = sum g
+    """
+
+    @staticmethod
+    def forward(ctx, feat, graph, c, weight, bias, drop_bwd=None):
+        if feat.stride(1) != 1:
+            feat = feat.contiguous()
+        n_in = graph.num_in
+        ah = aggregate_scaled(graph.fwd, feat, c, c[:n_in])
+        out = gemm_nt(ah, padded_weight(weight, feat.dtype, transpose=True), bias=bias)
+        ctx.graph, ctx.c, ctx.drop_bwd = graph, c, drop_bwd
+        ctx.has_bias = bias is not None
+        ctx.save_for_backward(ah, weight)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        ah, weight = ctx.saved_tensors
+        graph, c = ctx.graph, ctx.c
+        colsum = _take_colsum(g)
+        g = _tma_ready(g if g.dtype == ah.dtype else g.to(ah.dtype))
+        gsp = presplit(g)
+        g_feat = None
+        if ctx.needs_input_grad[0]:
+            g_ah = gemm_nt(gsp, padded_weight(weight, ah.dtype))
+            g_feat = aggregate_scaled(graph.bwd, g_ah, c, c, drop=ctx.drop_bwd)
+        gw = _graphconv_wgrad(gsp, ah, weight)
+        gb = (colsum if colsum is not None else g.float().sum(0)) if ctx.has_bias else None
+        return g_feat, None, None, gw, gb, None
+
+
+class GraphConvLayerNarrowFn(torch.autograd.Function):
+    """The same function transform-first when the layer narrows (d_out < d_in), as `SageLayerNarrowFn`:
+
+        z   = feat @ W                              [num_all, d_out]   pg_linear over the inner and halo rows
+        out = c[:N_in] * (A @ (c * z)) + b                             pg_aggregate_scaled, bias in its store
+
+        dz = c * (A^T @ (c[:N_in] * g))            [num_all, d_out]   pg_aggregate_scaled over the CSC
+        g_feat = dz @ W^T                                              pg_linear, dropout backward in its epilogue
+        gW = feat^T dz, gb = sum g
+    """
+
+    @staticmethod
+    def forward(ctx, feat, graph, c, weight, bias, drop_bwd=None):
+        if feat.stride(1) != 1:
+            feat = feat.contiguous()
+        z = gemm_nt(feat, padded_weight(weight, feat.dtype, transpose=True))
+        out = aggregate_scaled(graph.fwd, z, c, c[:graph.num_in], bias=bias)
+        ctx.graph, ctx.c, ctx.drop_bwd = graph, c, drop_bwd
+        ctx.has_bias = bias is not None
+        ctx.save_for_backward(feat, weight)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        feat, weight = ctx.saved_tensors
+        graph, c = ctx.graph, ctx.c
+        colsum = _take_colsum(g)
+        g = _tma_ready(g if g.dtype == feat.dtype else g.to(feat.dtype))
+        dz = aggregate_scaled(graph.bwd, g, c, c)                       # [num_all, d_out]
+        dzsp = presplit(dz)
+        g_feat = None
+        if ctx.needs_input_grad[0]:
+            g_feat = alloc_rows(feat.shape[0], feat.shape[1], feat.dtype, feat.device)
+            db = ctx.drop_bwd if (ctx.drop_bwd is not None and ctx.drop_bwd.p > 0 and feat.shape[1] <= 256
+                                  and _drop_ok(g_feat)) else None   # dropout backward in the GEMM's epilogue
+            gemm_nt(dzsp, padded_weight(weight, feat.dtype), out=g_feat, drop=db)
+            if db is None and ctx.drop_bwd is not None and ctx.drop_bwd.p > 0:
+                dropout_rows(g_feat, ctx.drop_bwd, out=g_feat)
+        gw = _graphconv_wgrad(dzsp, feat, weight)
+        gb = (colsum if colsum is not None else g.float().sum(0)) if ctx.has_bias else None
+        return g_feat, None, None, gw, gb, None
+
+
+def graphconv_layer(feat, graph, c, weight, bias, drop_bwd=None) -> torch.Tensor:
+    """GraphConv(norm='both') over the [num_all, d_in] rows `feat` of `graph` with the norm vector c [num_all];
+    weight [d_in, d_out] (DGL's layout), bias [d_out] or None.  Returns the [N_in, d_out] inner rows."""
+    if NARROW and weight.shape[1] < feat.shape[1]:
+        return GraphConvLayerNarrowFn.apply(feat, graph, c, weight, bias, drop_bwd)
+    return GraphConvLayerFn.apply(feat, graph, c, weight, bias, drop_bwd)
+
+
 # ---- graph attention (csrc/attention.cu) -------------------------------------------------------------------
 def gat_preload():
     """Load every attention kernel now: a first launch may wait for the device, so it must not happen while a halo

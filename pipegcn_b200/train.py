@@ -32,7 +32,7 @@ from .helper import context as ctx
 from .helper.feature_buffer import Buffer, EvalExchange, OneShotExchange, check_halo_bits, check_sampling
 from .helper.reducer import Reducer
 from .helper.timer.comm_timer import CommTimer
-from .module.model import GAT, GATv2, GraphSAGE
+from .module.model import GAT, GATv2, GraphConv, GraphSAGE
 from .partition import PartitionLayout, get_layer_size
 
 
@@ -50,11 +50,19 @@ def check_model(args):
     """Refuses, before anything is allocated, a configuration that is not implemented: --model gat or gatv2 with
     --use-pp (the precompute is GraphSAGE's neighbour mean) or with a hidden width that does not split into --n-heads
     heads, and --aggregator pool with an attention model (an attention layer has no aggregator) or with --use-pp (a
-    neighbour mean)."""
+    neighbour mean).  --model graphconv refuses --aggregator pool (it has no aggregator) and --sampling-rate < 1 (the
+    symmetric norm of a sampled graph needs every source's sampled out-degree, which depends on every peer's sample)."""
     attention = args.model in ('gat', 'gatv2')
     aggregator = getattr(args, 'aggregator', 'mean')
     if aggregator not in ('mean', 'pool'):
         raise ValueError(f"--aggregator {aggregator}: expected mean or pool")
+    if args.model == 'graphconv':
+        if aggregator == 'pool':
+            raise ValueError("--aggregator pool is a GraphSAGE aggregator; --model graphconv has none")
+        if getattr(args, 'sampling_rate', 1.0) < 1.0:
+            raise NotImplementedError("--model graphconv with --sampling-rate < 1: the symmetric norm of the sampled "
+                                      "graph needs every source's sampled out-degree")
+        return
     if aggregator == 'pool':
         if attention:
             raise ValueError(f"--aggregator pool is a GraphSAGE aggregator; --model {args.model} has none")
@@ -77,6 +85,9 @@ def create_model(layer_size, args, buffer=None, dtype=torch.float32):
         kw = {} if aggregator == 'mean' else dict(aggregator=aggregator)
         return GraphSAGE(layer_size, F.relu, args.use_pp, norm=args.norm, dropout=args.dropout,
                          n_linear=args.n_linear, train_size=args.n_train, buffer=buffer, dtype=dtype, **kw)
+    if args.model == 'graphconv':
+        return GraphConv(layer_size, F.relu, args.use_pp, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
+                         train_size=args.n_train, buffer=buffer, dtype=dtype)
     if args.model in ('gat', 'gatv2'):
         cls = GAT if args.model == 'gat' else GATv2
         return cls(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
@@ -84,11 +95,15 @@ def create_model(layer_size, args, buffer=None, dtype=torch.float32):
     raise NotImplementedError(args.model)
 
 
-def pp_input(graph, feat, rows):
+def pp_input(graph, feat, rows, sym=False):
     """--use-pp layer-0 input of the inner rows: cat(feat, neighbour mean) (second half of `precompute`,
-    PipeGCN/train.py:169-189); `rows` [num_all, d] holds the raw features of the inner and the halo rows."""
+    PipeGCN/train.py:169-189); `rows` [num_all, d] holds the raw features of the inner and the halo rows.
+    `sym` (--model graphconv): the symmetric-normalised aggregate c_v sum_u c_u x_u instead."""
     from . import ops
     from .graph import alloc_rows
+    if sym:
+        c = graph.sym_norm()
+        return ops.aggregate_scaled(graph.fwd, rows, c, c[:graph.num_in])
     d = feat.shape[1]
     mean = ops.aggregate(graph.fwd, rows, row_div=graph.in_deg_f)
     both = alloc_rows(graph.num_in, 2 * d, feat.dtype, feat.device)
@@ -192,12 +207,16 @@ class RankEngine:
         return getattr(self.world, 'is_local', False) and self.world.size > 1
 
     def _setup_steps(self, layout):
-        """Collective set-up (generator): the --use-pp precompute (train.py:169-189), cat(feat, neighbour mean) over
-        the raw features' halo rows, or else the one-shot exchange of the static layer-0 halo rows (SURVEY.md §8f-2)."""
+        """Collective set-up (generator): --model graphconv first exchanges the halo rows' degrees; then the --use-pp
+        precompute (train.py:169-189), cat(feat, neighbour mean) over the raw features' halo rows, or else the
+        one-shot exchange of the static layer-0 halo rows (SURVEY.md §8f-2)."""
+        sym = self.args.model == 'graphconv'
+        if sym:
+            yield from _sym_norm_steps(self.world, layout, self.graph, 'pipegcn.buffer.norm', self.buffer.timeout_ms)
         if self.args.use_pp:
             self.feat = yield from _raw_halo_steps(self.world, layout, self.feat, self.args.n_feat, 'pipegcn.buffer.pp',
                                                    self.buffer.timeout_ms,
-                                                   lambda rows: pp_input(self.graph, self.feat, rows))
+                                                   lambda rows: pp_input(self.graph, self.feat, rows, sym))
             return
         # the static input features live in the exchange buffer of layer 0 (all versions): update(0, .) copies nothing
         self.buffer.load_inner(0, self.feat)
@@ -243,6 +262,9 @@ class RankEngine:
             return
         # --use-pp: `self.feat` is cat(feat, neighbour mean) (train.py:169-189); the raw half is refreshed, the mean is
         # set-up work of the reference (precompute runs once, train.py:287-288) and is not recomputed per step
+        if self.args.model == 'graphconv':
+            raise NotImplementedError("set_features with --model graphconv --use-pp: layer 0's input is the "
+                                      "precomputed aggregate, which has no raw half to refresh")
         dst = self.feat[:, :feat.shape[1]]
         if feat.is_cuda and feat.dtype == dst.dtype:
             torch.mul(feat, 1, out=dst)
@@ -361,6 +383,7 @@ class RankEngine:
             # one key per evaluation layout (every rank opens them in the same order): several may be alive at once
             self._n_eval_layouts = getattr(self, '_n_eval_layouts', 0) + 1
             key = 'pipegcn.eval.layout%d' % self._n_eval_layouts
+        sym = args.model == 'graphconv'
         st.xch = EvalExchange(self.world, lay.num_in, lay.num_all, lay.boundary, lay.recv_shape, widths, n_graph,
                               self.dtype, key=key, timeout_ms=self.buffer.timeout_ms)
         self.last_eval_exchange = st.xch
@@ -378,9 +401,12 @@ class RankEngine:
         # an evaluation layout: its features are those of the graph it was built from, static for the run
         feat = eval_layout.feat.to(dev).to(self.dtype)
 
+        if sym:         # the degrees of this layout's own graph, next to its layer-0 feature exchange
+            yield from _sym_norm_steps(self.world, lay, st.graph, key + '.norm', self.buffer.timeout_ms)
+
         def use(rows):
             if args.use_pp:
-                st.pp_feat = pp_input(st.graph, feat, rows)    # recomputed over this layout's graph
+                st.pp_feat = pp_input(st.graph, feat, rows, sym)    # recomputed over this layout's graph
             else:
                 st.feat = feat
                 st.x0 = rows[lay.num_in:].clone()
@@ -461,6 +487,19 @@ def _raw_halo_steps(world, lay, feat, d, key, timeout_ms, use):
     one.check_status()
     one.release()
     return out
+
+
+def _sym_norm_steps(world, lay, graph, key, timeout_ms):
+    """--model graphconv (generator): GraphConv's c = deg^-1/2 of every [inner | halo] row of `graph`, stored with
+    `graph.set_sym_norm`.  The inner rows' degrees are their CSR row lengths (a partition holds every in-edge of its
+    inner rows).  A halo row's degree is not its CSC row length here (that counts only the edges into this partition):
+    its owner's c arrives over a one-shot exchange, the same bits on every rank that holds the row."""
+    from . import ops
+    from .graph import alloc_rows
+    col = alloc_rows(lay.num_in, 1, torch.float32, graph.device)
+    col.copy_(ops.sym_norm(graph.row_degrees())[:, None])
+    yield from _raw_halo_steps(world, lay, col, 1, key, timeout_ms,
+                               lambda rows: graph.set_sym_norm(rows[:, 0].clone()))
 
 
 def _lockstep(gens, streams=None):
