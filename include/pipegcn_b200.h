@@ -127,6 +127,36 @@ int pg_aggregate_scaled(const pg_csr* g, const void* x, int64_t ldx, void* out, 
 /* loads every pg_aggregate_scaled kernel (call it before any halo wait can spin: a first launch may wait for the device) */
 int pg_aggregate_scaled_preload(void);
 
+/*
+ * pg_aggregate_scaled with an initial residual (GCNII):
+ *   out[r, 0:d] = dst_scale[r] * ( sum_{e in row r} src_scale[indices[e]] * x[indices[e], 0:d] ) + alpha * res[r, 0:d]
+ *                 ( + bias[0:d] )
+ * The sum is that of pg_aggregate_scaled; after the multiply by dst_scale each element takes one fp32 multiply-add of
+ * alpha * res, then the bias, then one rounding to `dtype`.  A long row gets the residual once, in its fix-up.
+ * res: [n_rows, ldr] of `dtype`, ldr >= d; res == NULL is pg_aggregate_scaled (the same kernels and bits).
+ * Dropout, scratch and determinism as pg_aggregate_scaled.
+ */
+int pg_aggregate_scaled_res(const pg_csr* g, const void* x, int64_t ldx, void* out, int64_t ldo, int32_t d, int dtype,
+                            const float* src_scale, const float* dst_scale, const void* res, int64_t ldr, float alpha,
+                            const float* bias, float* scratch, const pg_drop* drop, void* stream);
+/* loads every pg_aggregate_scaled_res kernel (as pg_aggregate_scaled_preload) */
+int pg_aggregate_scaled_res_preload(void);
+
+/*
+ * GCNII row kernels (csrc/gcnii.cu).  Rows of `dtype` are 16-byte aligned and padded to the 16-byte vector (as the
+ * dropout kernels); the pad columns of every output are written as 0.  No atomics: the same bits from run to run.
+ *   pg_gcnii_relu_drop: h0 = ReLU(z); if hd != NULL, hd = dropout(h0) under `drop` (element (r, c) keyed as
+ *                       pg_dropout_rows with row0 = 0; drop NULL or p = 0: hd = h0).
+ *   pg_gcnii_teleport:  acc[r, c] = alpha * ds[r, c] (accumulate = 0) or fma(alpha, ds[r, c], acc[r, c]), fp32 acc.
+ *   pg_gcnii_relu_bwd:  dz[r, c] = h0[r, c] > 0 ? g[r, c] + (r < n_acc ? acc[r, c] : 0) : 0, the sum in fp32, one rounding.
+ */
+int pg_gcnii_relu_drop(const void* z, int64_t ldz, void* h0, int64_t ldh, void* hd, int64_t ldd, int32_t n_rows,
+                       int32_t d, int dtype, const pg_drop* drop, void* stream);
+int pg_gcnii_teleport(const void* ds, int64_t ldd, float* acc, int64_t lda, int32_t n_rows, int32_t d, int dtype,
+                      float alpha, int accumulate, void* stream);
+int pg_gcnii_relu_bwd(const void* g, int64_t ldg, const void* h0, int64_t ldh, const float* acc, int64_t lda,
+                      int32_t n_acc, void* dz, int64_t ldz, int32_t n_rows, int32_t d, int dtype, void* stream);
+
 /* out[r, 0:d] = x[r, 0:d] / row_div[r]   (gradient of `/ degs`, layer.py:50) */
 int pg_row_div(const void* x, int64_t ldx, void* out, int64_t ldo, int32_t n_rows, int32_t d, int dtype,
                const float* row_div, void* stream);

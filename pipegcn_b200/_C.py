@@ -71,6 +71,12 @@ def _load():
         "pg_aggregate_scaled": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, i32, C.c_int, vp, vp, vp, vp,
                                           C.POINTER(pg_drop), vp]),
         "pg_aggregate_scaled_preload": (C.c_int, []),
+        "pg_aggregate_scaled_res": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, i32, C.c_int, vp, vp, vp, i64, f32,
+                                              vp, vp, C.POINTER(pg_drop), vp]),
+        "pg_aggregate_scaled_res_preload": (C.c_int, []),
+        "pg_gcnii_relu_drop": (C.c_int, [vp, i64, vp, i64, vp, i64, i32, i32, C.c_int, C.POINTER(pg_drop), vp]),
+        "pg_gcnii_teleport": (C.c_int, [vp, i64, vp, i64, i32, i32, C.c_int, f32, C.c_int, vp]),
+        "pg_gcnii_relu_bwd": (C.c_int, [vp, i64, vp, i64, vp, i64, i32, vp, i64, i32, i32, C.c_int, vp]),
         "pg_row_div": (C.c_int, [vp, i64, vp, i64, i32, i32, C.c_int, vp, vp]),
         "pg_linear": (C.c_int, [C.c_int, C.c_int, C.POINTER(pg_gemm_src), i32, vp, vp, vp, i64, i32, i32, vp]),
         "pg_linear_drop": (C.c_int, [C.c_int, C.c_int, C.POINTER(pg_gemm_src), i32, vp, vp, vp, i64, i32, i32,

@@ -14,9 +14,14 @@
 //   out[r,:] = dst_scale[r] * ( sum_{e in row r} src_scale[indices[e]] * x[indices[e],:] )  (+ bias)
 // The lane that loads a column id also loads its source scale; the scale travels with the id (one more shuffle per
 // edge) and is applied as a multiply-add per element.  dst_scale arrives in the row_div slot and is a multiplier.
-// SC = false instantiations are the plain aggregate, instruction for instruction.  The SC kernels hold the scales of
+// SC = 0 instantiations are the plain aggregate, instruction for instruction.  The SC kernels hold the scales of
 // the rows in flight as well: they are compiled for one resident CTA per SM fewer (agg_occ does not apply), which
 // keeps every one of them free of local-memory spills.
+//
+// SC = 2 (pg_aggregate_scaled_res, GCNII's initial residual) is SC = 1 plus, wherever a finished row is stored,
+//   out[r,:] = dst_scale[r] * ( ... ) + alpha * res[r,:]  (+ bias)
+// one fp32 multiply-add per element after the row scale, before the single rounding to the output type.  A long row
+// gets it in the fix-up only: its segment partials carry the bare sums.  SC = 0 and 1 compile to the code they had.
 #include <algorithm>
 #include <mutex>
 #include <type_traits>
@@ -26,27 +31,41 @@
 namespace pg {
 
 // the operands of the SC instantiations that have no slot in the plain aggregate's arguments
-struct ScaleArg {
+struct ScaleCore {
   const float* src;    // [source rows] multiplier of every gathered row
   const float* bias;   // [d] added after the row scale, or NULL
-  int d;               // columns of the bias (the pad columns of a vector get none)
+  int d;               // columns of the bias and the residual (the pad columns of a vector get none)
+};
+struct ScaleArg : ScaleCore {
+  const void* res;     // SC = 2: [n_rows, ldr] rows of the output type, added times alpha
+  int64_t ldr;
+  float alpha;
 };
 
 // the factor every output row is multiplied by: dst_scale[row] (SC), else the IEEE reciprocal of row_div[row]
-template <bool SC>
+template <int SC>
 __device__ __forceinline__ float row_scale(const float* __restrict__ row_div, int row) {
-  if constexpr (SC) return __ldg(row_div + row);
+  if constexpr (SC != 0) return __ldg(row_div + row);
   return row_div != nullptr ? 1.f / __ldg(row_div + row) : 1.f;
 }
-// the scale operands a walker holds: none in the plain instantiations, so their code is that of pg_aggregate
+// the scale operands a walker holds: none in the plain instantiations, so their code is that of pg_aggregate, and no
+// residual operands in the SC = 1 ones, so theirs is that of pg_aggregate_scaled
 struct NoScale {};
-template <bool SC> using ScaleOf = std::conditional_t<SC, ScaleArg, NoScale>;
+template <int SC> using ScaleOf = std::conditional_t<SC == 0, NoScale, std::conditional_t<SC == 1, ScaleCore, ScaleArg>>;
 
-// r[0:V] += bias[o:o+V] (SC with a bias; columns past d add nothing)
-
-template <bool SC, int V, typename S>
-__device__ __forceinline__ void add_bias(float* r, const S& sc, int64_t o) {
-  if constexpr (SC) {
+// r[0:V] holds columns o .. o+V of the scaled output row `row`: SC = 2 adds alpha * res[row, o:o+V] (one multiply-add),
+// then SC with a bias adds bias[o:o+V]; columns past d add nothing
+template <int SC, typename P, typename S>
+__device__ __forceinline__ void row_epilogue(float* r, const S& sc, int row, int64_t o) {
+  constexpr int V = P::V;
+  if constexpr (SC == 2) {
+    float rv[V];
+    P::unpack(*reinterpret_cast<const typename P::Raw*>(static_cast<const typename P::Elem*>(sc.res) + static_cast<int64_t>(row) * sc.ldr + o), rv);
+#pragma unroll
+    for (int i = 0; i < V; ++i)
+      if (o + i < sc.d) r[i] = __fmaf_rn(sc.alpha, rv[i], r[i]);
+  }
+  if constexpr (SC != 0) {
     if (sc.bias != nullptr) {
 #pragma unroll
       for (int i = 0; i < V; ++i)
@@ -55,7 +74,7 @@ __device__ __forceinline__ void add_bias(float* r, const S& sc, int64_t o) {
   }
 }
 
-template <typename T, int VB, int G, int VPL, int U, bool SC>
+template <typename T, int VB, int G, int VPL, int U, int SC>
 __global__ void __launch_bounds__(256)
 agg_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict__ out, int64_t ldo, int nvec,
            const float* __restrict__ row_div, int acc_rows, float* __restrict__ scratch, int64_t lds, DropArg drop,
@@ -116,7 +135,7 @@ agg_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict_
         for (int j = 0; j < VPL; ++j)
           if (act[j]) v[u][j] = ld_vec<VB>(xc[j] + static_cast<uint64_t>(src[u]) * ldx_bytes);
       float ss[U];
-      if constexpr (SC) {
+      if constexpr (SC != 0) {
 #pragma unroll
         for (int u = 0; u < U; ++u) ss[u] = __ldg(sc.src + src[u]);
       }
@@ -124,7 +143,7 @@ agg_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict_
       for (int u = 0; u < U; ++u)
 #pragma unroll
         for (int j = 0; j < VPL; ++j) {
-          if constexpr (SC) {
+          if constexpr (SC != 0) {
             if (act[j]) P::fma(acc[j], v[u][j], ss[u]);
           } else {
             if (act[j]) P::add(acc[j], v[u][j]);
@@ -133,7 +152,7 @@ agg_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict_
     }
     for (; e < end; ++e) {
       const uint32_t s = static_cast<uint32_t>(__ldg(g.indices + e));
-      if constexpr (SC) {
+      if constexpr (SC != 0) {
         const float s1 = __ldg(sc.src + s);
 #pragma unroll
         for (int j = 0; j < VPL; ++j)
@@ -170,7 +189,7 @@ agg_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict_
           const float a = (i & 1) ? acc[j][i / 2].y : acc[j][i / 2].x;
           r[i] = a * inv;
         }
-        add_bias<SC, V>(r, sc, o);
+        row_epilogue<SC, P>(r, sc, row, o);
         if (row < acc_rows) {
           float ov[V];
           P::unpack(*reinterpret_cast<const Raw*>(op + o), ov);
@@ -188,7 +207,7 @@ agg_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict_
 // sums the fp32 partials of every long row and writes the row: one CTA per long row, warp w adds the segments
 // s0 + w, s0 + w + 8, ... (four in flight), then the eight warp sums are added in warp order -- a fixed order, so the
 // result does not depend on scheduling
-template <typename T, int VB, bool SC>
+template <typename T, int VB, int SC>
 __global__ void __launch_bounds__(256)
 agg_fixup_kernel(pg_csr g, T* __restrict__ out, int64_t ldo, int nvec, const float* __restrict__ row_div,
                  int acc_rows, const float* __restrict__ scratch, int64_t lds, DropArg drop, ScaleArg sc) {
@@ -235,7 +254,7 @@ agg_fixup_kernel(pg_csr g, T* __restrict__ out, int64_t ldo, int nvec, const flo
         for (int w = 1; w < 8; ++w) a += part[w][lane * V + i];
         r[i] = a * inv;
       }
-      add_bias<SC, V>(r, sc, static_cast<int64_t>(vi) * V);
+      row_epilogue<SC, P>(r, sc, row, static_cast<int64_t>(vi) * V);
       if (row < acc_rows) {
         float o[V];
         P::unpack(*reinterpret_cast<const typename P::Raw*>(op + static_cast<int64_t>(vi) * V), o);
@@ -309,14 +328,14 @@ template <> __device__ __forceinline__ void st_vec_cs<4>(void* p, uint32_t v) { 
 
 struct Chunk { int e_beg, n, item, kind_rows; };   // kind = kind_rows & 3 (0: n_rows rows of n edges, 1: one row, 2: segment)
 
-template <typename T, int VB, int VPL, int U, bool HINT, bool SC>
+template <typename T, int VB, int VPL, int U, bool HINT, int SC>
 struct Agg2 {
   using P = Pack<T, VB>;
   using Raw = typename P::Raw;
   static constexpr int V = P::V;
   static constexpr int NA = P::NA;
   static constexpr int kVPL = VPL;
-  static constexpr bool kSC = SC;
+  static constexpr bool kSC = SC != 0;
   static constexpr unsigned kFull = 0xffffffffu;
 
   const char* xc[VPL];      // this lane's column(s) of source row 0
@@ -350,13 +369,13 @@ struct Agg2 {
   __device__ __forceinline__ void add(const Raw (&v)[VPL], float s) {
 #pragma unroll
     for (int j = 0; j < VPL; ++j) {
-      if constexpr (SC) P::fma(acc[j], v[j], s);
+      if constexpr (SC != 0) P::fma(acc[j], v[j], s);
       else P::add(acc[j], v[j]);
     }
   }
   // source scale of column id `id` (hot flag in bit 31)
   __device__ __forceinline__ float scale_of(uint32_t id) const {
-    if constexpr (SC) return __ldg(sc.src + (id & 0x7fffffffu));
+    if constexpr (SC != 0) return __ldg(sc.src + (id & 0x7fffffffu));
     else return 1.f;
   }
   // the ragged end of a batch: every load is issued (positions past the end fetch a valid row: lanes past the
@@ -386,7 +405,7 @@ struct Agg2 {
         float r[V];
 #pragma unroll
         for (int i = 0; i < V; ++i) r[i] = ((i & 1) ? acc[j][i / 2].y : acc[j][i / 2].x) * inv;
-        add_bias<SC, V>(r, sc, o);
+        row_epilogue<SC, P>(r, sc, row, o);
         if (row < acc_rows) {
           float ov[V];
           P::unpack(*reinterpret_cast<const Raw*>(op + o), ov);
@@ -457,7 +476,7 @@ struct Agg2 {
       const float my_sc = nxt_sc;
       if (base + 32 + lane < n_e) {
         nxt = __ldcs(pidx + base + 32 + lane);
-        if constexpr (SC) nxt_sc = scale_of(nxt);
+        if constexpr (SC != 0) nxt_sc = scale_of(nxt);
       }
       const int n = min(32, n_e - base);
       int u0 = 0;
@@ -497,7 +516,7 @@ __device__ __forceinline__ void agg2_columns(A& a, const T* x, int c0, int lane,
 }
 
 // chunks [0, n_chunks_long): one row (kind 1) or one segment of a long row (kind 2) per warp
-template <typename T, int VB, int VPL, int U, bool HINT, int OCC, bool SC>
+template <typename T, int VB, int VPL, int U, bool HINT, int OCC, int SC>
 __global__ void __launch_bounds__(256, (VPL == 1 ? (SC ? (HINT ? 2 : 3) : OCC) : (VPL == 2 ? 2 : 1)))
 agg2_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict__ out, int64_t ldo, int nvec,
                  const float* __restrict__ row_div, int acc_rows, float* __restrict__ scratch, int64_t lds, DropArg drop,
@@ -552,7 +571,7 @@ template <int N> __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;" ::"n"(N) : "memory");
 }
 
-template <typename T, int VPL, int D, bool HINT, bool SC>
+template <typename T, int VPL, int D, bool HINT, int SC>
 __global__ void __launch_bounds__(256, (VPL == 1 ? (SC ? 4 : 6) : (SC ? 2 : 3)))
 agg3_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict__ out, int64_t ldo, int nvec,
                  const float* __restrict__ row_div, int acc_rows, float* __restrict__ scratch, int64_t lds, DropArg drop,
@@ -616,7 +635,7 @@ agg3_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __res
         a.add(v, SC ? __shfl_sync(kFull, sc_a, u) : 1.f);
       }
       idx_a = idx_b;
-      if constexpr (SC) sc_a = base + 32 + lane < n_e ? a.scale_of(idx_a) : 1.f;
+      if constexpr (SC != 0) sc_a = base + 32 + lane < n_e ? a.scale_of(idx_a) : 1.f;
       idx_b = base + 64 + lane < n_e ? __ldcs(pidx + base + 64 + lane) : 0u;
     }
     if ((c.w & 3) == 2) {
@@ -636,7 +655,7 @@ agg3_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __res
 }
 
 // chunks [n_chunks_long, n_chunks): n_rows whole rows of equal length (<= 32 entries together) per warp
-template <typename T, int VB, int VPL, int U, bool HINT, bool SC>
+template <typename T, int VB, int VPL, int U, bool HINT, int SC>
 __global__ void __launch_bounds__(256, (VPL == 1 ? (SC ? (HINT ? 2 : 3) : 4) : (VPL == 2 ? 2 : 1)))
 agg2_small_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict__ out, int64_t ldo, int nvec,
                   const float* __restrict__ row_div, int acc_rows, DropArg drop, ScaleArg sc) {
@@ -652,7 +671,7 @@ agg2_small_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __re
   float my_inv = 1.f;
   if (lane < n_rows) {
     my_row = __ldg(g.prow + c.z + lane);
-    if constexpr (SC) my_inv = __ldg(row_div + my_row);
+    if constexpr (SC != 0) my_inv = __ldg(row_div + my_row);
     else if (row_div != nullptr) my_inv = 1.f / __ldg(row_div + my_row);
   }
   A a;
@@ -675,7 +694,7 @@ agg2_small_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __re
 //   chunks of short rows : lane group q takes the rows q, q + R, ... of the chunk; all groups walk rows of the same
 //                          length, so the flush points are warp-uniform and only the stores are predicated
 // Same chunk plan, same coalesced index loads + shuffles as the full-width kernels.
-template <typename T, int VB, int G, bool SC>
+template <typename T, int VB, int G, int SC>
 struct AggN {
   using P = Pack<T, VB>;
   using Raw = typename P::Raw;
@@ -683,7 +702,7 @@ struct AggN {
   static constexpr int NA = P::NA;
   static constexpr int R = 32 / G;
   static constexpr int U = 8;
-  static constexpr bool kSC = SC;
+  static constexpr bool kSC = SC != 0;
   static constexpr unsigned kFull = 0xffffffffu;
   const char* xc;           // this lane's column of source row 0
   bool act;                 // lane's column exists
@@ -704,7 +723,7 @@ struct AggN {
     return ld_vec<VB>(xc + static_cast<uint64_t>(s & 0x7fffffffu) * ldx_bytes);
   }
   __device__ __forceinline__ void add(const Raw& t, float s) {
-    if constexpr (SC) P::fma(acc, t, s);
+    if constexpr (SC != 0) P::fma(acc, t, s);
     else P::add(acc, t);
   }
   __device__ __forceinline__ void add_masked(Raw t, bool keep, float s) {
@@ -715,7 +734,7 @@ struct AggN {
     add(t, s);
   }
   __device__ __forceinline__ float scale_of(uint32_t id) const {
-    if constexpr (SC) return __ldg(sc.src + (id & 0x7fffffffu));
+    if constexpr (SC != 0) return __ldg(sc.src + (id & 0x7fffffffu));
     else return 1.f;
   }
   __device__ __forceinline__ void store(int row, float inv, bool valid) {
@@ -724,7 +743,7 @@ struct AggN {
       float r[V];
 #pragma unroll
       for (int i = 0; i < V; ++i) r[i] = ((i & 1) ? acc[i / 2].y : acc[i / 2].x) * inv;
-      add_bias<SC, V>(r, sc, static_cast<int64_t>(col) * V);
+      row_epilogue<SC, P>(r, sc, row, static_cast<int64_t>(col) * V);
       if (row < acc_rows) {
         float ov[V];
         P::unpack(*reinterpret_cast<const Raw*>(op), ov);
@@ -768,7 +787,7 @@ __device__ __forceinline__ void aggn_setup(A& a, const T* x, uint32_t ldx_bytes,
   a.zero();
 }
 
-template <typename T, int VB, int G, bool SC>
+template <typename T, int VB, int G, int SC>
 __global__ void __launch_bounds__(256, SC ? (G == 16 ? 2 : 3) : 4)
 aggn_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict__ out, int64_t ldo, int nvec,
                  const float* __restrict__ row_div, int acc_rows, float* __restrict__ scratch, int64_t lds, DropArg drop,
@@ -793,7 +812,7 @@ aggn_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __res
     const float my_sc = nxt_sc;
     if (base + 32 + lane < n_e) {
       nxt = __ldcs(pidx + base + 32 + lane);
-      if constexpr (SC) nxt_sc = a.scale_of(nxt);
+      if constexpr (SC != 0) nxt_sc = a.scale_of(nxt);
     }
     const int n = min(32, n_e - base);
     // step u of this block: group q fetches entry u * R + q
@@ -828,7 +847,7 @@ aggn_long_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __res
   }
 }
 
-template <typename T, int VB, int G, bool SC>
+template <typename T, int VB, int G, int SC>
 __global__ void __launch_bounds__(256, SC ? (G == 16 ? 2 : 3) : 4)
 aggn_small_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __restrict__ out, int64_t ldo, int nvec,
                   const float* __restrict__ row_div, int acc_rows, DropArg drop, ScaleArg sc) {
@@ -847,7 +866,7 @@ aggn_small_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __re
   float my_inv = 1.f;
   if (lane < n_rows) {
     my_row = __ldg(g.prow + c.z + lane);
-    if constexpr (SC) my_inv = __ldg(row_div + my_row);
+    if constexpr (SC != 0) my_inv = __ldg(row_div + my_row);
     else if (row_div != nullptr) my_inv = 1.f / __ldg(row_div + my_row);
   }
   A a;
@@ -890,7 +909,7 @@ aggn_small_kernel(pg_csr g, const T* __restrict__ x, uint32_t ldx_bytes, T* __re
   }
 }
 
-template <typename T, int VB, int G, bool SC>
+template <typename T, int VB, int G, int SC>
 static int launch_aggn(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec, const float* row_div,
                        int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st);
 
@@ -916,7 +935,7 @@ static AggSide* agg_side_for(cudaStream_t st) {
   return &e;
 }
 
-template <typename T, int VB, int VPL, bool HINT, bool SC>
+template <typename T, int VB, int VPL, bool HINT, int SC>
 static int launch_agg2h(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec,
                         const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st) {
   constexpr int U = (VPL >= 4) ? 2 : (VPL == 2 ? 4 : 8);
@@ -962,7 +981,7 @@ static int launch_agg2h(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_
   return PG_OK;
 }
 
-template <typename T, int VB, int G, bool SC>
+template <typename T, int VB, int G, int SC>
 static int launch_aggn(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec, const float* row_div,
                        int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st) {
   const uint32_t ldxb = static_cast<uint32_t>(ldx * sizeof(T));
@@ -992,7 +1011,7 @@ static int launch_aggn(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t
   return PG_OK;
 }
 
-template <typename T, int VB, int VPL, bool SC>
+template <typename T, int VB, int VPL, int SC>
 static int launch_agg2(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec,
                        const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st) {
   if (g_agg_l2_hint) return launch_agg2h<T, VB, VPL, true, SC>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st);
@@ -1002,11 +1021,11 @@ static int launch_agg2(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t
 int g_agg_pack_short = 0;   // pg_set_option("agg_pack_short", 0|1): 16 lanes x 2 vectors per row when rows are short.
                             // OFF by default; not measured on H100
 
-template <typename T, int VB, int G, int VPL, int U, bool SC>
+template <typename T, int VB, int G, int VPL, int U, int SC>
 static int launch_agg_u(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec,
                         const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st);
 
-template <typename T, int VB, int G, int VPL, bool SC>
+template <typename T, int VB, int G, int VPL, int SC>
 static int launch_agg(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec,
                       const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st) {
   if (VPL == 1 && g_agg_unroll == 4)
@@ -1015,7 +1034,7 @@ static int launch_agg(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t 
   return launch_agg_u<T, VB, G, VPL, U, SC>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st);
 }
 
-template <typename T, int VB, int G, int VPL, int U, bool SC>
+template <typename T, int VB, int G, int VPL, int U, int SC>
 static int launch_agg_u(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec,
                         const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st) {
   constexpr int GROUPS = 256 / G;
@@ -1033,7 +1052,7 @@ static int launch_agg_u(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_
   return PG_OK;
 }
 
-template <typename T, int VB, bool SC>
+template <typename T, int VB, int SC>
 static int dispatch_agg(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_t ldo, int nvec,
                         const float* row_div, int acc_rows, float* scratch, int64_t lds, const DropArg& da, const ScaleArg& sc, cudaStream_t st) {
 #define PG_AGG(G_, VPL_) return launch_agg<T, VB, G_, VPL_, SC>(g, x, ldx, out, ldo, nvec, row_div, acc_rows, scratch, lds, da, sc, st)
@@ -1059,16 +1078,17 @@ static int dispatch_agg(const pg_csr& g, const T* x, int64_t ldx, T* out, int64_
 #undef PG_AGG
 }
 
-template <typename T, bool SC>
+template <typename T, int SC>
 static int aggregate_t(const pg_csr& g, const void* x, int64_t ldx, void* out, int64_t ldo, int d,
                        const float* row_div, int acc_rows, float* scratch, const DropArg& da, const ScaleArg& sc, cudaStream_t st) {
   const int es = sizeof(T);
   int vb = min(vec_bytes(x, ldx, es), vec_bytes(out, ldo, es));
-  // a vector must not straddle two rows: either d is a multiple of the vector or both strides leave room
+  if constexpr (SC == 2) vb = min(vb, vec_bytes(sc.res, sc.ldr, es));
+  // a vector must not straddle two rows: either d is a multiple of the vector or every stride leaves room
   while (vb > es) {
     const int v = vb / es;
     const int64_t dp = round_up(d, v);
-    if (d % v == 0 || (dp <= ldx && dp <= ldo)) break;
+    if (d % v == 0 || (dp <= ldx && dp <= ldo && (SC != 2 || dp <= sc.ldr))) break;
     vb >>= 1;
   }
   const int v = vb / es;
@@ -1138,44 +1158,46 @@ static int row_div_t(const void* x, int64_t ldx, void* out, int64_t ldo, int n_r
 }
 
 // CUDA loads kernels lazily, and loading one may wait for the device: every SC instantiation is loaded at the first
-// pg_aggregate_scaled call (or pg_aggregate_scaled_preload), before a halo wait of a simulated rank can spin
-template <typename T, int VB, int VPL, bool HINT>
+// pg_aggregate_scaled call (or pg_aggregate_scaled_preload), before a halo wait of a simulated rank can spin; the SC = 2
+// ones likewise at the first pg_aggregate_scaled_res call (or pg_aggregate_scaled_res_preload)
+template <typename T, int VB, int VPL, bool HINT, int SC>
 static void preload_agg2(cudaFuncAttributes* a) {
   constexpr int U = (VPL >= 4) ? 2 : (VPL == 2 ? 4 : 8);
   constexpr int D = (VPL >= 4) ? 4 : 8;
-  cudaFuncGetAttributes(a, agg2_small_kernel<T, VB, VPL, U, HINT, true>);
-  cudaFuncGetAttributes(a, agg2_long_kernel<T, VB, VPL, U, HINT, 4, true>);
-  cudaFuncGetAttributes(a, agg3_long_kernel<T, VPL, D, HINT, true>);
+  cudaFuncGetAttributes(a, agg2_small_kernel<T, VB, VPL, U, HINT, SC>);
+  cudaFuncGetAttributes(a, agg2_long_kernel<T, VB, VPL, U, HINT, 4, SC>);
+  cudaFuncGetAttributes(a, agg3_long_kernel<T, VPL, D, HINT, SC>);
 }
-template <typename T, int VB>
+template <typename T, int VB, int SC>
 static void preload_vb(cudaFuncAttributes* a) {
-  preload_agg2<T, VB, 1, false>(a); preload_agg2<T, VB, 2, false>(a); preload_agg2<T, VB, 4, false>(a);
-  preload_agg2<T, VB, 1, true>(a); preload_agg2<T, VB, 2, true>(a); preload_agg2<T, VB, 4, true>(a);
-  cudaFuncGetAttributes(a, aggn_small_kernel<T, VB, 4, true>);
-  cudaFuncGetAttributes(a, aggn_small_kernel<T, VB, 8, true>);
-  cudaFuncGetAttributes(a, aggn_small_kernel<T, VB, 16, true>);
-  cudaFuncGetAttributes(a, aggn_long_kernel<T, VB, 4, true>);
-  cudaFuncGetAttributes(a, aggn_long_kernel<T, VB, 8, true>);
-  cudaFuncGetAttributes(a, aggn_long_kernel<T, VB, 16, true>);
-  cudaFuncGetAttributes(a, agg_fixup_kernel<T, VB, true>);
-  cudaFuncGetAttributes(a, agg_kernel<T, VB, 4, 1, 8, true>);
-  cudaFuncGetAttributes(a, agg_kernel<T, VB, 4, 1, 4, true>);
-  cudaFuncGetAttributes(a, agg_kernel<T, VB, 8, 1, 8, true>);
-  cudaFuncGetAttributes(a, agg_kernel<T, VB, 8, 1, 4, true>);
-  cudaFuncGetAttributes(a, agg_kernel<T, VB, 16, 1, 8, true>);
-  cudaFuncGetAttributes(a, agg_kernel<T, VB, 16, 1, 4, true>);
-  cudaFuncGetAttributes(a, agg_kernel<T, VB, 16, 2, 4, true>);
-  cudaFuncGetAttributes(a, agg_kernel<T, VB, 32, 1, 8, true>);
-  cudaFuncGetAttributes(a, agg_kernel<T, VB, 32, 1, 4, true>);
-  cudaFuncGetAttributes(a, agg_kernel<T, VB, 32, 2, 4, true>);
-  cudaFuncGetAttributes(a, agg_kernel<T, VB, 32, 4, 2, true>);
+  preload_agg2<T, VB, 1, false, SC>(a); preload_agg2<T, VB, 2, false, SC>(a); preload_agg2<T, VB, 4, false, SC>(a);
+  preload_agg2<T, VB, 1, true, SC>(a); preload_agg2<T, VB, 2, true, SC>(a); preload_agg2<T, VB, 4, true, SC>(a);
+  cudaFuncGetAttributes(a, aggn_small_kernel<T, VB, 4, SC>);
+  cudaFuncGetAttributes(a, aggn_small_kernel<T, VB, 8, SC>);
+  cudaFuncGetAttributes(a, aggn_small_kernel<T, VB, 16, SC>);
+  cudaFuncGetAttributes(a, aggn_long_kernel<T, VB, 4, SC>);
+  cudaFuncGetAttributes(a, aggn_long_kernel<T, VB, 8, SC>);
+  cudaFuncGetAttributes(a, aggn_long_kernel<T, VB, 16, SC>);
+  cudaFuncGetAttributes(a, agg_fixup_kernel<T, VB, SC>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 4, 1, 8, SC>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 4, 1, 4, SC>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 8, 1, 8, SC>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 8, 1, 4, SC>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 16, 1, 8, SC>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 16, 1, 4, SC>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 16, 2, 4, SC>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 32, 1, 8, SC>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 32, 1, 4, SC>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 32, 2, 4, SC>);
+  cudaFuncGetAttributes(a, agg_kernel<T, VB, 32, 4, 2, SC>);
 }
+template <int SC>
 static void aggregate_scaled_preload() {
   static std::once_flag once;
   std::call_once(once, [] {
     cudaFuncAttributes a;
-    preload_vb<float, 16>(&a); preload_vb<float, 8>(&a); preload_vb<float, 4>(&a);
-    preload_vb<__nv_bfloat16, 16>(&a); preload_vb<__nv_bfloat16, 8>(&a); preload_vb<__nv_bfloat16, 4>(&a);
+    preload_vb<float, 16, SC>(&a); preload_vb<float, 8, SC>(&a); preload_vb<float, 4, SC>(&a);
+    preload_vb<__nv_bfloat16, 16, SC>(&a); preload_vb<__nv_bfloat16, 8, SC>(&a); preload_vb<__nv_bfloat16, 4, SC>(&a);
     cudaGetLastError();
   });
 }
@@ -1245,10 +1267,10 @@ extern "C" int pg_aggregate_drop(const pg_csr* g, const void* x, int64_t ldx, vo
   PG_REQUIRE(g->n_rows >= 0 && g->seg_len > 0 && d > 0, "pg_aggregate: bad sizes (n_rows=%d seg_len=%d d=%d)", g->n_rows, g->seg_len, d);
   PG_REQUIRE(ldx >= d && ldo >= d && ldx < (1ll << 29), "pg_aggregate: row stride smaller than d (or >= 2^29 elements)");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const pg::ScaleArg sc{nullptr, nullptr, 0};
-  if (dtype == PG_F32) return pg::aggregate_t<float, false>(*g, x, ldx, out, ldo, d, row_div, acc_rows, scratch, da, sc, st);
+  const pg::ScaleArg sc{{nullptr, nullptr, 0}, nullptr, 0, 0.f};
+  if (dtype == PG_F32) return pg::aggregate_t<float, 0>(*g, x, ldx, out, ldo, d, row_div, acc_rows, scratch, da, sc, st);
   if (dtype == PG_BF16)
-    return pg::aggregate_t<__nv_bfloat16, false>(*g, x, ldx, out, ldo, d, row_div, acc_rows, scratch, da, sc, st);
+    return pg::aggregate_t<__nv_bfloat16, 0>(*g, x, ldx, out, ldo, d, row_div, acc_rows, scratch, da, sc, st);
   pg::set_error("pg_aggregate: unknown dtype %d", dtype);
   return PG_ERR_INVALID;
 }
@@ -1261,18 +1283,45 @@ extern "C" int pg_aggregate_scaled(const pg_csr* g, const void* x, int64_t ldx, 
   PG_REQUIRE(g->n_rows >= 0 && g->seg_len > 0 && d > 0, "pg_aggregate_scaled: bad sizes (n_rows=%d seg_len=%d d=%d)",
              g->n_rows, g->seg_len, d);
   PG_REQUIRE(ldx >= d && ldo >= d && ldx < (1ll << 29), "pg_aggregate_scaled: row stride smaller than d (or >= 2^29 elements)");
-  pg::aggregate_scaled_preload();
+  pg::aggregate_scaled_preload<1>();
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  const pg::ScaleArg sc{src_scale, bias, d};
-  if (dtype == PG_F32) return pg::aggregate_t<float, true>(*g, x, ldx, out, ldo, d, dst_scale, 0, scratch, da, sc, st);
+  const pg::ScaleArg sc{{src_scale, bias, d}, nullptr, 0, 0.f};
+  if (dtype == PG_F32) return pg::aggregate_t<float, 1>(*g, x, ldx, out, ldo, d, dst_scale, 0, scratch, da, sc, st);
   if (dtype == PG_BF16)
-    return pg::aggregate_t<__nv_bfloat16, true>(*g, x, ldx, out, ldo, d, dst_scale, 0, scratch, da, sc, st);
+    return pg::aggregate_t<__nv_bfloat16, 1>(*g, x, ldx, out, ldo, d, dst_scale, 0, scratch, da, sc, st);
   pg::set_error("pg_aggregate_scaled: unknown dtype %d", dtype);
   return PG_ERR_INVALID;
 }
 
 extern "C" int pg_aggregate_scaled_preload(void) {
-  pg::aggregate_scaled_preload();
+  pg::aggregate_scaled_preload<1>();
+  return PG_OK;
+}
+
+extern "C" int pg_aggregate_scaled_res(const pg_csr* g, const void* x, int64_t ldx, void* out, int64_t ldo, int32_t d,
+                                       int dtype, const float* src_scale, const float* dst_scale, const void* res,
+                                       int64_t ldr, float alpha, const float* bias, float* scratch, const pg_drop* drop,
+                                       void* stream) {
+  if (res == nullptr)      // no residual: pg_aggregate_scaled, the same kernels and bits
+    return pg_aggregate_scaled(g, x, ldx, out, ldo, d, dtype, src_scale, dst_scale, bias, scratch, drop, stream);
+  const pg::DropArg da = pg::make_drop(drop);
+  PG_REQUIRE(g && x && out && src_scale && dst_scale, "pg_aggregate_scaled_res: null argument");
+  PG_REQUIRE(g->n_rows >= 0 && g->seg_len > 0 && d > 0, "pg_aggregate_scaled_res: bad sizes (n_rows=%d seg_len=%d d=%d)",
+             g->n_rows, g->seg_len, d);
+  PG_REQUIRE(ldx >= d && ldo >= d && ldr >= d && ldx < (1ll << 29),
+             "pg_aggregate_scaled_res: row stride smaller than d (or >= 2^29 elements)");
+  pg::aggregate_scaled_preload<2>();
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const pg::ScaleArg sc{{src_scale, bias, d}, res, ldr, alpha};
+  if (dtype == PG_F32) return pg::aggregate_t<float, 2>(*g, x, ldx, out, ldo, d, dst_scale, 0, scratch, da, sc, st);
+  if (dtype == PG_BF16)
+    return pg::aggregate_t<__nv_bfloat16, 2>(*g, x, ldx, out, ldo, d, dst_scale, 0, scratch, da, sc, st);
+  pg::set_error("pg_aggregate_scaled_res: unknown dtype %d", dtype);
+  return PG_ERR_INVALID;
+}
+
+extern "C" int pg_aggregate_scaled_res_preload(void) {
+  pg::aggregate_scaled_preload<2>();
   return PG_OK;
 }
 

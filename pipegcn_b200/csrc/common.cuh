@@ -70,6 +70,7 @@ __device__ __forceinline__ float2 fma2(float2 a, float2 b, float2 c) {
 template <typename T, int VB> struct Pack;
 
 template <int VB> struct Pack<float, VB> {
+  using Elem = float;
   static constexpr int V = VB / 4;
   static constexpr int NA = (V + 1) / 2;      // float2 accumulators per vector
   using Raw = typename RawVec<VB>::type;
@@ -107,6 +108,7 @@ template <int VB> struct Pack<float, VB> {
 };
 
 template <int VB> struct Pack<__nv_bfloat16, VB> {
+  using Elem = __nv_bfloat16;
   static constexpr int V = VB / 2;
   static constexpr int NA = (V + 1) / 2;
   using Raw = typename RawVec<VB>::type;

@@ -192,6 +192,16 @@ class PartGraph:
             c = self._sym_c = sym_norm(self.row_degrees())
         return c
 
+    def gcnii_norm(self, alpha: float) -> torch.Tensor:
+        """(1 - alpha) * c[:num_in] in fp32 (GCNII's destination scale; (1 - alpha) rounded to fp32 first), computed
+        once per alpha and kept at this address: captured CUDA graphs read it."""
+        cached = getattr(self, "_gcnii_cs", None)
+        if cached is None or cached[0] != float(alpha):
+            c = self.sym_norm()[:self.num_in]
+            cached = self._gcnii_cs = (float(alpha), torch.mul(c, torch.tensor(1.0 - float(alpha), dtype=torch.float32,
+                                                                               device=c.device)).contiguous())
+        return cached[1]
+
     def num_nodes(self, ntype: str = "_U") -> int:
         if ntype == "_U":
             return self.num_all

@@ -35,6 +35,14 @@ read it with getattr(args, 'halo_bits', None).
 reference's) or `pool`, Hamilton et al.'s max-pool aggregator (DGL `SAGEConv(aggregator_type='pool')`): every layer
 takes the element-wise neighbour maximum of ReLU(h Wp^T + bp).  It cannot be combined with --model gat, --model gatv2 or --use-pp.
 Suppressed like `--sampling-rate`: read it with getattr(args, 'aggregator', 'mean').
+
+`--model gcnii` (not in the reference) trains GCNII (Chen et al., ICML 2020; DGL's GCN2Conv): graph layer 0 is a linear
+fc_in in front of its convolution, every convolution adds alpha times the initial representation h0 to its scaled
+aggregate and maps it through (1 - beta_l) I + beta_l W1 with beta_l = ln(lambda / l + 1).  `--n-layers` counts fc_in's
+layer, the convolutions and the `--n-linear` (>= 1) trailing linears.  `--gcnii-alpha a` (0 <= a <= 1, default 0.1)
+and `--gcnii-lambda l` (l > 0, finite, default 0.5) set alpha and lambda; suppressed like `--sampling-rate`: read them
+with getattr(args, 'gcnii_alpha', 0.1) and getattr(args, 'gcnii_lambda', 0.5).  It cannot be combined with --use-pp,
+--aggregator pool or --sampling-rate < 1.
 """
 import argparse
 
@@ -42,8 +50,8 @@ import argparse
 _FLAGS = [
     ("dataset", dict(type=str, default='reddit', help="the input dataset (or synthetic:<shape>)")),
     ("graph-name", dict(type=str, default='')),
-    ("model", dict(type=str, default='graphsage', help="model for training (graphsage | gcn | gat | gatv2 | graphconv; "
-                                                              "gcn is GraphSAGE)")),
+    ("model", dict(type=str, default='graphsage', help="model for training (graphsage | gcn | gat | gatv2 | graphconv | "
+                                                              "gcnii; gcn is GraphSAGE)")),
     ("dropout", dict(type=float, default=0.5, help="dropout probability")),
     ("lr", dict(type=float, default=1e-2, help="learning rate")),
     ("n-epochs", dict(type=int, default=200, help="the number of training epochs")),
@@ -97,6 +105,26 @@ def _n_heads(text):
     return k
 
 
+def _gcnii_alpha(text):
+    try:
+        a = float(text)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"invalid GCNII alpha '{text}'")
+    if not 0.0 <= a <= 1.0:          # also refuses nan
+        raise argparse.ArgumentTypeError(f"--gcnii-alpha {text}: expected 0 <= alpha <= 1")
+    return a
+
+
+def _gcnii_lambda(text):
+    try:
+        lam = float(text)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"invalid GCNII lambda '{text}'")
+    if not 0.0 < lam < float('inf'):   # also refuses nan
+        raise argparse.ArgumentTypeError(f"--gcnii-lambda {text}: expected a finite lambda > 0")
+    return lam
+
+
 def build_parser():
     parser = argparse.ArgumentParser(description='PipeGCN on H100')
     for flag, kw in _FLAGS:
@@ -123,6 +151,10 @@ def build_parser():
                              "(default: exact)")
     parser.add_argument('--aggregator', choices=['mean', 'pool'], default=argparse.SUPPRESS,
                         help="GraphSAGE neighbour aggregator: mean (default) or pool (max over ReLU(h Wp^T + bp))")
+    parser.add_argument('--gcnii-alpha', '--gcnii_alpha', type=_gcnii_alpha, default=argparse.SUPPRESS,
+                        help="--model gcnii: weight of the initial residual (0 <= alpha <= 1, default 0.1)")
+    parser.add_argument('--gcnii-lambda', '--gcnii_lambda', type=_gcnii_lambda, default=argparse.SUPPRESS,
+                        help="--model gcnii: beta_l = ln(lambda / l + 1) (lambda > 0, default 0.5)")
     return parser
 
 

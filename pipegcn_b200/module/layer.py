@@ -47,6 +47,18 @@ aggregating first when d_in <= d_out, transforming first otherwise (DGL's rule; 
 State-dict keys are GraphConv's: `weight` [d_in, d_out] (not transposed like nn.Linear), `bias` [d_out].
 Initialisation is GraphConv.reset_parameters, in this draw order: xavier_uniform_(weight), then bias = 0.
 With --use-pp layer 0 multiplies the precomputed rows c[v] * sum_u c[u] x[u] by the same weight.
+
+`GCNIILayer` (not in the reference): one convolution of GCNII (Chen et al., "Simple and Deep Graph Convolutional
+Networks", ICML 2020), DGL's `GCN2Conv(d, layer=l, alpha, lambda_, project_initial_features=True, bias=True)`, no
+activation inside, over the same rows and with the same c as GraphConvLayer.  Convolution l = i + 1 of graph layer i:
+
+    S   = (1 - alpha) * c[v] * sum_{u -> v} c[u] h[u] + alpha * h0[v]
+    out = (1 - beta_l) * S + beta_l * S @ W1 + b,      beta_l = ln(lambda / l + 1)
+
+h0 = ReLU(fc_in(dropout(x))) is the model's initial representation; graph layer 0 holds `fc_in` (an nn.Linear
+[d, n_feat], default initialisation, drawn first) in front of its convolution and computes it over every [inner | halo]
+row of x.  State-dict keys: `fc_in.weight` / `fc_in.bias` (layer 0 only), `weight1` [d, d] (in x out, DGL's layout),
+`bias` [d].  Initialisation is the GCNII authors': weight1 ~ U(-1/sqrt(d), 1/sqrt(d)), then bias = 0.
 """
 import math
 
@@ -139,6 +151,40 @@ class GraphConvLayer(nn.Module):
         if self.use_pp and self.training:
             return self.pp_linear(feat)
         return ops.graphconv_layer(feat, graph, graph.sym_norm(), self.weight, self.bias, drop_bwd)
+
+
+class GCNIILayer(nn.Module):
+    """GCN2Conv(d, layer=i+1, alpha, lambda_, project_initial_features=True, bias=True), no activation inside, with
+    fc_in in front of it in graph layer 0: module docstring."""
+
+    def __init__(self, in_feats, out_feats, layer, alpha=0.1, lam=0.5):
+        super().__init__()
+        if layer > 0 and in_feats != out_feats:
+            raise ValueError(f"GCNII convolution {layer + 1}: {in_feats} -> {out_feats} is not square")
+        self.in_feats, self.out_feats, self.layer = in_feats, out_feats, layer
+        self.alpha, self.lam = float(alpha), float(lam)
+        self.beta = ops.gcnii_beta(self.lam, layer + 1)
+        if layer == 0:
+            self.fc_in = nn.Linear(in_feats, out_feats)
+        self.weight1 = nn.Parameter(torch.empty(out_feats, out_feats))
+        self.bias = nn.Parameter(torch.empty(out_feats))
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        """The GCNII authors' initialisation of the convolution (fc_in keeps nn.Linear's, drawn at construction)."""
+        stdv = 1.0 / math.sqrt(self.out_feats)
+        nn.init.uniform_(self.weight1, -stdv, stdv)
+        nn.init.zeros_(self.bias)
+
+    def forward(self, graph, feat, state, drop_bwd=None):
+        """`feat`: the [num_all, d_in] rows of `graph` (layer 0: the dropped input features); `state`: the
+        `ops.GCNIIState` of this forward (layer 0 fills its h0).  Returns the [N_in, d] inner rows.  `drop_bwd` as
+        GraphSAGELayer.forward."""
+        c, cs = graph.sym_norm(), graph.gcnii_norm(self.alpha)
+        if self.layer == 0:
+            return ops.gcnii_first(feat, graph, c, cs, self.fc_in.weight, self.fc_in.bias, self.weight1, self.bias,
+                                   self.alpha, self.beta, state)
+        return ops.gcnii_conv(feat, graph, c, cs, self.weight1, self.bias, self.alpha, self.beta, state, drop_bwd)
 
 
 class GATLayer(nn.Module):

@@ -26,13 +26,19 @@ partitioned evaluation; only the graph layers and the kernels they load differ.
 `GraphConv(GraphSAGE)` (not in the reference) is the same layer loop with `GraphConvLayer`s (DGL's GraphConv,
 norm='both'): the layers read the symmetric norm from the graph (`PartGraph.sym_norm`) instead of the in-degrees.
 `GCN` stays the reference's name for GraphSAGE.
+
+`GCNII(GraphSAGE)` (not in the reference) is the same layer loop with `GCNIILayer`s (DGL's GCN2Conv): graph layer 0 is
+fc_in + ReLU + convolution 1 over the exchanged input features, every later graph layer one square convolution, and
+the trailing `n_linear` (>= 1) linears produce the logits.  Every layer reads h0 = ReLU(fc_in(dropout(x))) through
+the `ops.GCNIIState` of the forward; h0 enters convolution 1 through its own keyed dropout and the residuals clean.
+Between the graph layers the loop applies norm, ReLU and dropout as for every other model; the paper has ReLU only.
 """
 import torch
 from torch import nn
 import torch.nn.functional as F
 
 from ..helper import context as ctx
-from .layer import GATLayer, GATv2Layer, GraphConvLayer, GraphSAGELayer
+from .layer import GATLayer, GATv2Layer, GCNIILayer, GraphConvLayer, GraphSAGELayer
 
 
 class GNNBase(nn.Module):
@@ -94,6 +100,10 @@ class GraphSAGE(GNNBase):
         from .. import ops
         return ops.dropout(h, self.dropout.p, self.training)
 
+    def _drop_input(self, i, h):
+        """Dropout of graph layer i's input rows where no fused or keyed path applies."""
+        return self._drop(h)
+
     def _buffer(self):
         return self.buffer if self.buffer is not None else ctx.buffer
 
@@ -146,7 +156,7 @@ class GraphSAGE(GNNBase):
                     # same mask as the fused path, as separate passes (PG_FUSED_DROPOUT=0 / unsupported shapes)
                     h = layer(g, ops.keyed_dropout(h, self._drop_spec(i)), in_deg)
                 else:
-                    h = layer(g, self._drop(h), in_deg)
+                    h = layer(g, self._drop_input(i, h), in_deg)
             else:
                 h = ops.linear(self._drop(h), layer.weight, layer.bias)
             if i < self.n_layers - 1:
@@ -168,6 +178,7 @@ class GraphSAGE(GNNBase):
         if self.aggregator == 'pool':
             ops.pool_preload()
         h = None
+        arg = self._layer_arg(None)
         for i, layer in enumerate(self.layers):
             if i < self.n_graph_layers:
                 if i == 0 and self.use_pp:
@@ -178,7 +189,7 @@ class GraphSAGE(GNNBase):
                         xch.push(i, d)
                         yield i
                         xch.wait(i)
-                    h = layer(g, xch.rows(i, d), None)
+                    h = layer(g, xch.rows(i, d), arg)
             else:
                 h = ops.linear(h, layer.weight, layer.bias)
             if i < self.n_layers - 1:
@@ -213,6 +224,57 @@ class GraphConv(GraphSAGE):
     def _preload(self):
         from .. import ops
         ops.graphconv_preload()
+
+    def forward(self, g, feat, in_deg=None):
+        self._preload()
+        return super().forward(g, feat, in_deg)
+
+    def forward_partitioned(self, g, xch, pp_feat=None, push0=False):
+        self._preload()
+        return (yield from super().forward_partitioned(g, xch, pp_feat, push0))
+
+
+class GCNII(GraphSAGE):
+
+    def __init__(self, layer_size, activation, dropout=0.5, norm='layer', train_size=None, n_linear=1, buffer=None,
+                 dtype=torch.float32, alpha=0.1, lam=0.5):
+        n_graph = len(layer_size) - 1 - n_linear
+        if n_linear < 1:
+            raise ValueError("GCNII needs n_linear >= 1: its last convolution is square, the logits come from a linear")
+        if n_graph < 1:
+            raise ValueError("GCNII needs at least one graph layer")
+        if len(set(layer_size[1:n_graph + 1])) != 1:
+            raise ValueError(f"GCNII: every convolution is square, got widths {layer_size[1:n_graph + 1]}")
+        self.alpha, self.lam = float(alpha), float(lam)
+        super().__init__(layer_size, activation, False, dropout=dropout, norm=norm, train_size=train_size,
+                         n_linear=n_linear, buffer=buffer, dtype=dtype)
+
+    def _graph_layer(self, i, d_in, d_out):
+        return GCNIILayer(d_in, d_out, i, alpha=self.alpha, lam=self.lam)
+
+    def _layer_arg(self, in_deg):
+        """A fresh `ops.GCNIIState` per forward, with the dropout key of h0 in training."""
+        from .. import ops
+        drop = None
+        if self.training and self.dropout.p > 0:
+            drop = ops.DropSpec(self.dropout.p, ops.gcnii_h0_seed(), getattr(self._buffer(), 'epoch_dev', None), 0)
+        return ops.GCNIIState(drop)
+
+    def _drop_input(self, i, h):
+        """Layer 0's input features take a keyed mask too (CUDA-graph replays draw fresh ones)."""
+        from .. import ops
+        if i > 0 or not self.training or self.dropout.p == 0:
+            return super()._drop_input(i, h)
+        if not ops._drop_ok(h):
+            from ..graph import alloc_rows
+            hp = alloc_rows(h.shape[0], h.shape[1], h.dtype, h.device)
+            hp.copy_(h)
+            h = hp
+        return ops.keyed_dropout(h, self._drop_spec(0))
+
+    def _preload(self):
+        from .. import ops
+        ops.gcnii_preload()
 
     def forward(self, g, feat, in_deg=None):
         self._preload()

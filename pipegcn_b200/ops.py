@@ -852,6 +852,227 @@ def graphconv_layer(feat, graph, c, weight, bias, drop_bwd=None) -> torch.Tensor
     return GraphConvLayerFn.apply(feat, graph, c, weight, bias, drop_bwd)
 
 
+# ---- GCNII (--model gcnii): the residual aggregate of csrc/aggregate.cu and the row kernels of csrc/gcnii.cu ------
+def gcnii_preload():
+    """Load every residual-aggregate kernel (and the column sum of fc_in's bias gradient) now (see gat_preload)."""
+    _C.check(_C.lib.pg_aggregate_scaled_res_preload(), "pg_aggregate_scaled_res_preload")
+    graphconv_preload()
+    gat_preload()
+
+
+def gcnii_beta(lam: float, layer: int) -> float:
+    """beta_l = ln(lambda / l + 1) of convolution l (1-based)."""
+    import math
+    return math.log(lam / layer + 1.0)
+
+
+def gcnii_h0_seed() -> int:
+    """Dropout seed of h0 on its way into the first convolution (distinct from every layer_seed)."""
+    return (layer_seed(0) * 0x9E3779B97F4A7C15 + 0x5851F42D4C957F2D) & 0xFFFFFFFFFFFFFFFF
+
+
+def aggregate_scaled_res(plan: CsrPlan, x: torch.Tensor, src: torch.Tensor, dst: torch.Tensor,
+                         res: torch.Tensor = None, alpha: float = 0.0, bias: torch.Tensor = None,
+                         drop: DropSpec = None, out: torch.Tensor = None) -> torch.Tensor:
+    """out[r] = dst[r] * sum_{e in row r} src[indices[e]] * x[indices[e]] + alpha * res[r] (+ bias), one rounding
+    (pg_aggregate_scaled_res); res None is `aggregate_scaled`."""
+    _rows(x)
+    d = x.shape[1]
+    if out is None:
+        out = alloc_rows(plan.n_rows, d, x.dtype, x.device)
+    _rows(out)
+    assert out.shape[0] == plan.n_rows and out.shape[1] == d and out.dtype == x.dtype
+    assert src.dtype == dst.dtype == torch.float32 and src.is_contiguous() and dst.is_contiguous()
+    assert src.numel() >= x.shape[0] and dst.numel() >= plan.n_rows
+    if res is not None:
+        _rows(res)
+        assert res.shape[0] >= plan.n_rows and res.shape[1] == d and res.dtype == x.dtype
+    if bias is not None:
+        bias = bias.detach()
+        assert bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == d and bias.is_cuda
+    scratch = plan.scratch(d)
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_aggregate_scaled_res(C.byref(plan.c), x.data_ptr(), x.stride(0), out.data_ptr(), out.stride(0),
+                                            d, _C.dtype_code(x.dtype), src.data_ptr(), dst.data_ptr(),
+                                            res.data_ptr() if res is not None else None,
+                                            res.stride(0) if res is not None else 0, float(alpha),
+                                            bias.data_ptr() if bias is not None else None,
+                                            scratch.data_ptr() if scratch is not None else None,
+                                            C.byref(drop.c()) if drop is not None and drop.p > 0 else None,
+                                            _C.stream_ptr()), "pg_aggregate_scaled_res")
+    return out
+
+
+def gcnii_relu_drop(z: torch.Tensor, drop: DropSpec = None):
+    """(h0, hd): h0 = ReLU(z) and hd = dropout(h0) under the key `drop` in one pass (pg_gcnii_relu_drop); without a
+    dropout hd is h0."""
+    _rows(z)
+    n, d = z.shape
+    h0 = alloc_rows(n, d, z.dtype, z.device)
+    hd = alloc_rows(n, d, z.dtype, z.device) if drop is not None and drop.p > 0 else None
+    _C.count()
+    _C.check(_C.lib.pg_gcnii_relu_drop(z.data_ptr(), z.stride(0), h0.data_ptr(), h0.stride(0),
+                                       hd.data_ptr() if hd is not None else None, hd.stride(0) if hd is not None else 0,
+                                       n, d, _C.dtype_code(z.dtype), C.byref(drop.c()) if hd is not None else None,
+                                       _C.stream_ptr()), "pg_gcnii_relu_drop")
+    return h0, (hd if hd is not None else h0)
+
+
+def gcnii_teleport(ds: torch.Tensor, acc: torch.Tensor, alpha: float, accumulate: bool):
+    """acc = alpha * ds, or acc = fma(alpha, ds, acc) when `accumulate`, in fp32 (pg_gcnii_teleport)."""
+    _rows(ds)
+    assert acc.dtype == torch.float32 and acc.shape == ds.shape and acc.stride(1) == 1
+    _C.count()
+    _C.check(_C.lib.pg_gcnii_teleport(ds.data_ptr(), ds.stride(0), acc.data_ptr(), acc.stride(0), ds.shape[0],
+                                      ds.shape[1], _C.dtype_code(ds.dtype), float(alpha), int(bool(accumulate)),
+                                      _C.stream_ptr()), "pg_gcnii_teleport")
+
+
+def gcnii_relu_bwd(g: torch.Tensor, h0: torch.Tensor, acc: torch.Tensor = None) -> torch.Tensor:
+    """dz = (h0 > 0) ? g + acc : 0 in fp32, acc on its first acc.shape[0] rows only (pg_gcnii_relu_bwd)."""
+    _rows(g)
+    _rows(h0)
+    n, d = g.shape
+    assert h0.shape == g.shape and h0.dtype == g.dtype
+    n_acc = 0
+    if acc is not None:
+        assert acc.dtype == torch.float32 and acc.shape[1] == d and acc.shape[0] <= n and acc.stride(1) == 1
+        n_acc = acc.shape[0]
+    dz = alloc_rows(n, d, g.dtype, g.device)
+    _C.count()
+    _C.check(_C.lib.pg_gcnii_relu_bwd(g.data_ptr(), g.stride(0), h0.data_ptr(), h0.stride(0),
+                                      acc.data_ptr() if acc is not None else None,
+                                      acc.stride(0) if acc is not None else 0, n_acc, dz.data_ptr(), dz.stride(0), n, d,
+                                      _C.dtype_code(g.dtype), _C.stream_ptr()), "pg_gcnii_relu_bwd")
+    return dz
+
+
+class GCNIIState:
+    """What the convolutions of one GCNII forward share: the clean initial representation h0 [num_all, d] (layer 0
+    writes it, every convolution reads its inner rows), the dropout key of h0 on its way into convolution 0, and the
+    fp32 [N_in, d] sum of the gradients the convolutions send to h0 (the first backward writes it, the later ones add
+    to it: layer L-1 down to 0, the order autograd runs them in)."""
+
+    def __init__(self, drop_h0: DropSpec = None):
+        self.drop_h0 = drop_h0
+        self.h0 = None
+        self.acc = None
+        self.written = False
+
+
+def gcnii_weight(w1: torch.Tensor, beta: float) -> torch.Tensor:
+    """W_eff = (1 - beta) I + beta W1 in fp32 from the master weight ([d, d], in x out)."""
+    w = w1.detach().float() * beta
+    w.diagonal().add_(1.0 - beta)
+    return w
+
+
+def _gcnii_conv_fwd(feat, graph, c, cs, h0_in, alpha, w_eff, bias):
+    """S = (1-a) c[:N_in] * (A @ (c * feat)) + a h0 (the residual aggregate), out = S @ W_eff + b (pg_linear)."""
+    s = aggregate_scaled_res(graph.fwd, feat, c, cs, res=h0_in, alpha=alpha)
+    return s, gemm_nt(s, padded_weight(w_eff, feat.dtype, transpose=True), bias=bias)
+
+
+def _gcnii_conv_bwd(ctx, g, s, w_eff, need_feat, drop_bwd):
+    """Gradients of one convolution: dS = g W_eff^T (pg_linear), alpha dS into the teleport sum, the input gradient
+    c * (A^T @ ((1-a) c[:N_in] * dS)) with the dropout backward in its store, dW1 = beta S^T g (pg_wgrad), db."""
+    graph, c, cs, state = ctx.graph, ctx.c, ctx.cs, ctx.state
+    colsum = _take_colsum(g)
+    g = _tma_ready(g if g.dtype == s.dtype else g.to(s.dtype))
+    gsp = presplit(g)
+    ds = gemm_nt(gsp, padded_weight(w_eff, s.dtype))
+    if state.acc is None:
+        state.acc = alloc_rows(s.shape[0], s.shape[1], torch.float32, s.device)
+    gcnii_teleport(ds, state.acc, ctx.alpha, accumulate=state.written)
+    state.written = True
+    g_feat = aggregate_scaled(graph.bwd, ds, cs, c, drop=drop_bwd) if need_feat else None
+    gw = (wgrad(gsp, s).t() * ctx.beta).contiguous()
+    gb = (colsum if colsum is not None else g.float().sum(0)) if ctx.has_bias else None
+    return g_feat, gw, gb
+
+
+class GCNIIConvFn(torch.autograd.Function):
+    """GCNII convolution l >= 1 (DGL GCN2Conv, project_initial_features=True, no activation) over the [inner | halo]
+    rows `feat`, with h0 the inner rows of state.h0:
+
+        S   = (1-a) c[:N_in] * (A @ (c * feat)) + a h0      pg_aggregate_scaled_res over the CSR
+        out = S @ ((1-b) I + b W1) + bias                   pg_linear
+
+        dS = g W_eff^T                                      pg_linear
+        h0 += a dS                                          pg_gcnii_teleport (fp32 sum, GCNIIState)
+        g_feat = c * (A^T @ ((1-a) c[:N_in] * dS))          pg_aggregate_scaled over the CSC, dropout backward in its store
+        dW1 = b S^T g, d bias = sum g
+    """
+
+    @staticmethod
+    def forward(ctx, feat, weight1, bias, graph, c, cs, alpha, beta, state, drop_bwd=None):
+        if feat.stride(1) != 1:
+            feat = feat.contiguous()
+        w_eff = gcnii_weight(weight1, beta)
+        s, out = _gcnii_conv_fwd(feat, graph, c, cs, state.h0[:graph.num_in], alpha, w_eff, bias)
+        ctx.graph, ctx.c, ctx.cs, ctx.state, ctx.drop_bwd = graph, c, cs, state, drop_bwd
+        ctx.alpha, ctx.beta, ctx.has_bias = alpha, beta, bias is not None
+        ctx.save_for_backward(s, w_eff)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        s, w_eff = ctx.saved_tensors
+        g_feat, gw, gb = _gcnii_conv_bwd(ctx, g, s, w_eff, ctx.needs_input_grad[0], ctx.drop_bwd)
+        return g_feat, gw, gb, None, None, None, None, None, None, None
+
+
+class GCNIIFirstFn(torch.autograd.Function):
+    """Graph layer 0 of GCNII: fc_in over every [inner | halo] row of the (dropped) input features, then convolution 0:
+
+        z = x W_in^T + b_in                                 pg_linear over num_all rows
+        h0 = ReLU(z), hd = dropout(h0)                      pg_gcnii_relu_drop (state.h0 = h0)
+        out = convolution 0 of hd with the residual h0[:N_in]     as GCNIIConvFn
+
+    Backward: convolution 0's gradients (its teleport term last in the sum), then
+        dz = ReLU'(z) * (g_hd + teleport sum on the inner rows)    pg_gcnii_relu_bwd
+        dW_in = dz^T x (pg_wgrad), d b_in = column sum of dz (pg_gat_colsum); no gradient to x.
+    Every rank's dW_in covers the halo rows it used: the all-reduce adds them up to the whole graph's gradient.
+    """
+
+    @staticmethod
+    def forward(ctx, x, fc_weight, fc_bias, weight1, bias, graph, c, cs, alpha, beta, state):
+        if x.stride(1) != 1:
+            x = x.contiguous()
+        z = gemm_nt(x, padded_weight(fc_weight, x.dtype), bias=fc_bias)
+        h0, hd = gcnii_relu_drop(z, state.drop_h0)
+        del z
+        state.h0, state.acc, state.written = h0, None, False
+        w_eff = gcnii_weight(weight1, beta)
+        s, out = _gcnii_conv_fwd(hd, graph, c, cs, h0[:graph.num_in], alpha, w_eff, bias)
+        ctx.graph, ctx.c, ctx.cs, ctx.state = graph, c, cs, state
+        ctx.alpha, ctx.beta, ctx.has_bias = alpha, beta, bias is not None
+        ctx.has_fc_bias = fc_bias is not None
+        ctx.save_for_backward(x, h0, s, w_eff)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        x, h0, s, w_eff = ctx.saved_tensors
+        state = ctx.state
+        g_hd, gw, gb = _gcnii_conv_bwd(ctx, g, s, w_eff, True, state.drop_h0)
+        dz = gcnii_relu_bwd(g_hd, h0, state.acc)
+        dzsp = presplit(dz)
+        g_fc_w = wgrad(dzsp, x)
+        g_fc_b = gat_colsum(dz) if ctx.has_fc_bias else None
+        return None, g_fc_w, g_fc_b, gw, gb, None, None, None, None, None, None
+
+
+def gcnii_first(x, graph, c, cs, fc_weight, fc_bias, weight1, bias, alpha, beta, state) -> torch.Tensor:
+    """Graph layer 0 of GCNII (GCNIIFirstFn): fc_in, ReLU and convolution 0; fills state.h0."""
+    return GCNIIFirstFn.apply(x, fc_weight, fc_bias, weight1, bias, graph, c, cs, alpha, beta, state)
+
+
+def gcnii_conv(feat, graph, c, cs, weight1, bias, alpha, beta, state, drop_bwd=None) -> torch.Tensor:
+    """GCNII convolution l >= 1 (GCNIIConvFn) over the [num_all, d] rows `feat`; returns the [N_in, d] inner rows."""
+    return GCNIIConvFn.apply(feat, weight1, bias, graph, c, cs, alpha, beta, state, drop_bwd)
+
+
 # ---- graph attention (csrc/attention.cu) -------------------------------------------------------------------
 def gat_preload():
     """Load every attention kernel now: a first launch may wait for the device, so it must not happen while a halo

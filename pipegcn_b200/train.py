@@ -32,7 +32,7 @@ from .helper import context as ctx
 from .helper.feature_buffer import Buffer, EvalExchange, OneShotExchange, check_halo_bits, check_sampling
 from .helper.reducer import Reducer
 from .helper.timer.comm_timer import CommTimer
-from .module.model import GAT, GATv2, GraphConv, GraphSAGE
+from .module.model import GAT, GATv2, GCNII, GraphConv, GraphSAGE
 from .partition import PartitionLayout, get_layer_size
 
 
@@ -51,11 +51,28 @@ def check_model(args):
     --use-pp (the precompute is GraphSAGE's neighbour mean) or with a hidden width that does not split into --n-heads
     heads, and --aggregator pool with an attention model (an attention layer has no aggregator) or with --use-pp (a
     neighbour mean).  --model graphconv refuses --aggregator pool (it has no aggregator) and --sampling-rate < 1 (the
-    symmetric norm of a sampled graph needs every source's sampled out-degree, which depends on every peer's sample)."""
+    symmetric norm of a sampled graph needs every source's sampled out-degree, which depends on every peer's sample).
+    --model gcnii refuses the same two, --n-linear 0 (its last convolution is square: the logits come from a linear)
+    and --use-pp (graph layer 0 begins with fc_in, so a precomputed neighbour aggregate of x has no place)."""
     attention = args.model in ('gat', 'gatv2')
     aggregator = getattr(args, 'aggregator', 'mean')
     if aggregator not in ('mean', 'pool'):
         raise ValueError(f"--aggregator {aggregator}: expected mean or pool")
+    if args.model == 'gcnii':
+        if args.n_linear < 1:
+            raise ValueError("--model gcnii needs --n-linear >= 1: its last convolution is square, so the logits "
+                             "come from a linear")
+        if args.n_layers - args.n_linear < 1:
+            raise ValueError("--model gcnii needs --n-layers > --n-linear (at least one convolution)")
+        if args.use_pp:
+            raise NotImplementedError("--model gcnii with --use-pp: graph layer 0 begins with fc_in, so a precomputed "
+                                      "neighbour aggregate of the features has no place")
+        if aggregator == 'pool':
+            raise ValueError("--aggregator pool is a GraphSAGE aggregator; --model gcnii has none")
+        if getattr(args, 'sampling_rate', 1.0) < 1.0:
+            raise NotImplementedError("--model gcnii with --sampling-rate < 1: the symmetric norm of the sampled "
+                                      "graph needs every source's sampled out-degree")
+        return
     if args.model == 'graphconv':
         if aggregator == 'pool':
             raise ValueError("--aggregator pool is a GraphSAGE aggregator; --model graphconv has none")
@@ -88,6 +105,10 @@ def create_model(layer_size, args, buffer=None, dtype=torch.float32):
     if args.model == 'graphconv':
         return GraphConv(layer_size, F.relu, args.use_pp, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
                          train_size=args.n_train, buffer=buffer, dtype=dtype)
+    if args.model == 'gcnii':
+        return GCNII(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
+                     train_size=args.n_train, buffer=buffer, dtype=dtype, alpha=getattr(args, 'gcnii_alpha', 0.1),
+                     lam=getattr(args, 'gcnii_lambda', 0.5))
     if args.model in ('gat', 'gatv2'):
         cls = GAT if args.model == 'gat' else GATv2
         return cls(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
@@ -207,12 +228,14 @@ class RankEngine:
         return getattr(self.world, 'is_local', False) and self.world.size > 1
 
     def _setup_steps(self, layout):
-        """Collective set-up (generator): --model graphconv first exchanges the halo rows' degrees; then the --use-pp
+        """Collective set-up (generator): --model graphconv and gcnii first exchange the halo rows' degrees; then the --use-pp
         precompute (train.py:169-189), cat(feat, neighbour mean) over the raw features' halo rows, or else the
         one-shot exchange of the static layer-0 halo rows (SURVEY.md §8f-2)."""
-        sym = self.args.model == 'graphconv'
+        sym = self.args.model in ('graphconv', 'gcnii')
         if sym:
             yield from _sym_norm_steps(self.world, layout, self.graph, 'pipegcn.buffer.norm', self.buffer.timeout_ms)
+            if self.args.model == 'gcnii':
+                self.graph.gcnii_norm(getattr(self.args, 'gcnii_alpha', 0.1))
         if self.args.use_pp:
             self.feat = yield from _raw_halo_steps(self.world, layout, self.feat, self.args.n_feat, 'pipegcn.buffer.pp',
                                                    self.buffer.timeout_ms,
@@ -383,7 +406,7 @@ class RankEngine:
             # one key per evaluation layout (every rank opens them in the same order): several may be alive at once
             self._n_eval_layouts = getattr(self, '_n_eval_layouts', 0) + 1
             key = 'pipegcn.eval.layout%d' % self._n_eval_layouts
-        sym = args.model == 'graphconv'
+        sym = args.model in ('graphconv', 'gcnii')
         st.xch = EvalExchange(self.world, lay.num_in, lay.num_all, lay.boundary, lay.recv_shape, widths, n_graph,
                               self.dtype, key=key, timeout_ms=self.buffer.timeout_ms)
         self.last_eval_exchange = st.xch
@@ -403,6 +426,8 @@ class RankEngine:
 
         if sym:         # the degrees of this layout's own graph, next to its layer-0 feature exchange
             yield from _sym_norm_steps(self.world, lay, st.graph, key + '.norm', self.buffer.timeout_ms)
+            if args.model == 'gcnii':
+                st.graph.gcnii_norm(getattr(args, 'gcnii_alpha', 0.1))
 
         def use(rows):
             if args.use_pp:
