@@ -476,6 +476,40 @@ int pg_gatv2_bwd_src(const pg_csr* gt, const void* zs, int64_t ldzs, const void*
                      void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Graph transformer (PyG TransformerConv with concat=True, beta=False, root_weight=True, no edge features, no
+ * attention dropout) over the `_U` rows [inner | halo] of one partition.  q and skip [N_in, H * D], k and v
+ * [num_all, H * D] (fp32 or bf16, `dtype`, each with its own row stride) are the four projections; for the in-edges
+ * u -> v of the forward CSR, per head h:
+ *   e_uv = scale <q[v, h], k[u, h]>  (scale = 1/sqrt(D), passed in fp32),  a_uv = softmax over u of e_uv,
+ *   out[v, h] = sum_u a_uv v[u, h] + skip[v, h]    (attention part 0 for a row without a kept in-edge)
+ * `keep` and the chunk-table plan as for pg_gat_*; fp32 accumulation, no atomics, no per-edge storage, D <= 512; the
+ * results are the same bits from run to run, and both backward passes recompute a_uv with the forward's bits.
+ * Scratch (fp32, may be NULL when n_seg == 0): n_seg * H * (D + 2) floats for the aggregate, n_seg * H * (2 D + 1) for
+ * the destination pass, n_seg * H * 2 D for the source pass.
+ * ---------------------------------------------------------------------------------------- */
+int pg_tconv_preload(void);
+/* out (activation dtype; skip added in fp32 before the one rounding) and the softmax statistics m (maximum), s (sum
+ * of exp(e - m)), fp32 [N_in, H] */
+int pg_tconv_aggregate(const pg_csr* g, const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                       int64_t ldv, const void* skip, int64_t ldskip, int32_t H, int32_t D, int dtype, float scale,
+                       const uint8_t* keep, int32_t num_in, void* out, int64_t ldo, float* m, float* s,
+                       float* scratch, void* stream);
+/* backward over the forward CSR, grad = dL/d out, gd_uv = <grad[v, h], v[u, h]>:
+ *   delta[v, h] = sum_u a_uv gd_uv   (fp32 [N_in, H])
+ *   dq[v, h] = scale sum_u a_uv (gd_uv - delta_v) k[u, h],  gcopy[v, h] = grad[v, h]   (activation dtype) */
+int pg_tconv_bwd_dst(const pg_csr* g, const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                     int64_t ldv, const void* grad, int64_t ldg, int32_t H, int32_t D, int dtype, float scale,
+                     const float* m, const float* s, const uint8_t* keep, int32_t num_in, void* dq, int64_t lddq,
+                     void* gcopy, int64_t ldgc, float* delta, float* scratch, void* stream);
+/* backward over the CSC gt (rows = all `_U` rows u, columns = destinations v):
+ *   dv[u, h] = sum_v a_uv grad[v, h],  dk[u, h] = scale sum_v a_uv (gd_uv - delta_v) q[v, h]
+ *   (activation dtype; unkept halo rows: 0) */
+int pg_tconv_bwd_src(const pg_csr* gt, const void* q, int64_t ldq, const void* k, int64_t ldk, const void* v,
+                     int64_t ldv, const void* grad, int64_t ldg, int32_t H, int32_t D, int dtype, float scale,
+                     const float* m, const float* s, const float* delta, const uint8_t* keep, int32_t num_in,
+                     void* dk, int64_t lddk, void* dv, int64_t lddv, float* scratch, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Max-pool GraphSAGE (DGL SAGEConv(aggregator_type='pool')) over the `_U` rows [inner | halo] of one partition.
  * Q [num_all, d] (fp32 or bf16, `dtype`) is the pooled transform h Wp^T + bp.  For the in-edges u -> v of the forward
  * CSR g (each edge once):

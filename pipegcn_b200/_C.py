@@ -129,6 +129,13 @@ def _load():
                                        i32, vp, i64, vp, vp, i64, vp, vp]),
         "pg_gatv2_bwd_src": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, vp, i64, i32, i32, C.c_int, vp, vp, vp, vp,
                                        vp, i32, vp, i64, vp, vp]),
+        "pg_tconv_preload": (C.c_int, []),
+        "pg_tconv_aggregate": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, vp, i64, vp, i64, i32, i32, C.c_int, f32,
+                                         vp, i32, vp, i64, vp, vp, vp, vp]),
+        "pg_tconv_bwd_dst": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, vp, i64, vp, i64, i32, i32, C.c_int, f32,
+                                       vp, vp, vp, i32, vp, i64, vp, i64, vp, vp, vp]),
+        "pg_tconv_bwd_src": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, vp, i64, vp, i64, i32, i32, C.c_int, f32,
+                                       vp, vp, vp, vp, i32, vp, i64, vp, i64, vp, vp]),
         "pg_pool_preload": (C.c_int, []),
         "pg_max_aggregate": (C.c_int, [C.POINTER(pg_csr), vp, i64, i32, C.c_int, vp, i64, vp, i64, vp, i64, vp]),
         "pg_max_aggregate_bwd": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, vp, i64, i32, C.c_int, vp, i64, vp,

@@ -199,19 +199,16 @@ __global__ void __launch_bounds__(kGatWarps * 32) gat_fwd_kernel(FwdArgs a) {
   walk_chunk(a.w, c, [&](int v, int e0, int n, int slot) { fwd_row<T, NJ>(a, a.w, v, e0, n, slot, k, lane); });
 }
 
-// merge the (m, s, acc) partials of every long row in segment order
-template <typename T, int NJ>
-__global__ void __launch_bounds__(kGatWarps * 32) gat_fwd_fixup_kernel(FwdArgs a) {
-  const int lane = threadIdx.x & 31;
-  const int li = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
-  const int k = blockIdx.y;
-  if (li >= a.w.n_long) return;
-  const int H = a.H, D = a.D;
-  float m = -INFINITY, s = 0.f, acc[NJ];
+// merge the (m, s, acc) partials ([n_seg][H][D + 2]) of long row li, head k, in segment order
+template <int NJ>
+__device__ __forceinline__ void fwd_merge(const Walk& w, const float* scratch, int li, int k, int H, int D, int lane,
+                                          float& m, float& s, float (&acc)[NJ]) {
+  m = -INFINITY;
+  s = 0.f;
 #pragma unroll
   for (int j = 0; j < NJ; ++j) acc[j] = 0.f;
-  for (int sg = a.w.long_seg_ptr[li]; sg < a.w.long_seg_ptr[li + 1]; ++sg) {
-    const float* p = a.scratch + (static_cast<int64_t>(sg) * H + k) * (D + 2);
+  for (int sg = w.long_seg_ptr[li]; sg < w.long_seg_ptr[li + 1]; ++sg) {
+    const float* p = scratch + (static_cast<int64_t>(sg) * H + k) * (D + 2);
     const float mi = p[0];
     if (mi == -INFINITY) continue;
     const float mn = fmaxf(m, mi);
@@ -224,6 +221,16 @@ __global__ void __launch_bounds__(kGatWarps * 32) gat_fwd_fixup_kernel(FwdArgs a
     }
     m = mn;
   }
+}
+
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32) gat_fwd_fixup_kernel(FwdArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int li = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (li >= a.w.n_long) return;
+  float m, s, acc[NJ];
+  fwd_merge<NJ>(a.w, a.scratch, li, k, a.H, a.D, lane, m, s, acc);
   fwd_store<T, NJ>(a, a.w.long_row[li], k, lane, m, s, acc);
 }
 
@@ -884,6 +891,364 @@ __global__ void __launch_bounds__(kGatWarps * 32) gatv2_bwd_src_fixup_kernel(V2A
   v2_src_store<T, NJ>(a, a.w.long_row[li], k, lane, acc);
 }
 
+// ---------------------------------------------------------------------------------------------------- transformer
+// Graph transformer (PyG TransformerConv, concat=True, beta=False, root_weight=True): per head k,
+//   e_uv = scale <q[v, k], k[u, k]>,  a_uv = softmax over u of e_uv,  out[v, k] = sum_u a_uv v[u, k] + skip[v, k].
+// The warp layout and the E-edges-at-a-time batches are GATv2's.  Every score is dot_part(q_v, k_u) summed over
+// warp_sum's tree (through warp_sum_n) and then multiplied by scale with __fmul_rn, so no pass can contract it into a
+// later subtraction: e_uv has the same bits in all three passes and the backward recomputes a_uv exactly from (m, s).
+// edges in flight per warp: the most that every pass compiles with at NJ columns per lane without local-memory spills
+template <int NJ> __host__ __device__ constexpr int tc_edges() { return NJ <= 4 ? 4 : 2; }
+
+struct TcArgs {
+  Walk w;
+  const void* q; int64_t ldq;             // [N_in, H * D]
+  const void* k; int64_t ldk;             // [num_all, H * D]
+  const void* v; int64_t ldv;             // [num_all, H * D]
+  const void* skip; int64_t ldskip;       // forward: [N_in, H * D]
+  const void* g; int64_t ldg;             // backward: dL/d out [N_in, H * D]
+  const float* m; const float* s;         // backward: softmax statistics [N_in, H]
+  const float* delta;                     // source pass: delta_v [N_in, H]
+  const uint8_t* keep; int32_t num_in;
+  void* out; int64_t ldo;                 // forward: out; destination pass: dq; source pass: dk
+  void* out2; int64_t ldo2;               // destination pass: the copy of g; source pass: dv
+  float* m_out; float* s_out;             // forward
+  float* delta_out;                       // destination pass
+  float* scratch;
+  float scale;
+  int32_t H, D;
+};
+
+template <typename T>
+__device__ __forceinline__ const T* head_row(const void* base, int64_t ld, int r, int k, int D) {
+  return static_cast<const T*>(base) + static_cast<int64_t>(r) * ld + static_cast<int64_t>(k) * D;
+}
+template <typename T>
+__device__ __forceinline__ T* head_row_out(void* base, int64_t ld, int r, int k, int D) {
+  return static_cast<T*>(base) + static_cast<int64_t>(r) * ld + static_cast<int64_t>(k) * D;
+}
+
+// the batch of E in-edges of row v from entry e0 + b: kept sources in u (else -1), their k rows in x and v rows in y
+template <typename T, int NJ, int E>
+__device__ __forceinline__ void tc_gather(const TcArgs& a, int e0, int b, int n, int kh, int lane, int (&u)[E],
+                                          float (&x)[E][NJ], float (&y)[E][NJ]) {
+#pragma unroll
+  for (int t = 0; t < E; ++t) {
+    u[t] = -1;
+    if (b + t < n) {
+      const int ut = a.w.pidx[e0 + b + t] & kColMask;
+      if (is_kept(a.keep, a.num_in, ut)) u[t] = ut;
+    }
+  }
+#pragma unroll
+  for (int t = 0; t < E; ++t) {
+    if (u[t] >= 0) {
+      load_head<T, NJ>(head_row<T>(a.k, a.ldk, u[t], kh, a.D), a.D, lane, x[t]);
+      load_head<T, NJ>(head_row<T>(a.v, a.ldv, u[t], kh, a.D), a.D, lane, y[t]);
+    } else {
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) { x[t][j] = 0.f; y[t][j] = 0.f; }
+    }
+  }
+}
+
+template <typename T, int NJ>
+__device__ __forceinline__ void tc_fwd_store(const TcArgs& a, int v, int kh, int lane, float m, float s,
+                                             const float (&acc)[NJ]) {
+  const T* sk = head_row<T>(a.skip, a.ldskip, v, kh, a.D);
+  T* o = head_row_out<T>(a.out, a.ldo, v, kh, a.D);
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int col = lane + 32 * j;
+    if (col < a.D) o[col] = from_f<T>((s > 0.f ? __fdiv_rn(acc[j], s) : 0.f) + ldf(sk + col));
+  }
+  if (lane == 0) {
+    a.m_out[static_cast<int64_t>(v) * a.H + kh] = m;
+    a.s_out[static_cast<int64_t>(v) * a.H + kh] = s;
+  }
+}
+
+// online softmax of one row (or segment) for head kh, E in-edges at a time; a segment writes GAT's (m, s, acc) partial
+template <typename T, int NJ>
+__device__ __forceinline__ void tc_fwd_row(const TcArgs& a, int v, int e0, int n, int slot, int kh, int lane) {
+  constexpr int E = tc_edges<NJ>();
+  const int D = a.D;
+  float qv[NJ], acc[NJ];
+  load_head<T, NJ>(head_row<T>(a.q, a.ldq, v, kh, D), D, lane, qv);
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) acc[j] = 0.f;
+  float m = -INFINITY, s = 0.f;
+  for (int b = 0; b < n; b += E) {
+    int u[E];
+    float x[E][NJ], y[E][NJ], p[E];
+    tc_gather<T, NJ, E>(a, e0, b, n, kh, lane, u, x, y);
+#pragma unroll
+    for (int t = 0; t < E; ++t) p[t] = dot_part<NJ>(qv, x[t]);
+    warp_sum_n<E>(p, lane);
+    float bm = -INFINITY;
+#pragma unroll
+    for (int t = 0; t < E; ++t) {
+      p[t] = __fmul_rn(p[t], a.scale);
+      if (u[t] >= 0) bm = fmaxf(bm, p[t]);
+    }
+    if (bm == -INFINITY) continue;            // warp-uniform: no kept source in this batch
+    const float mn = fmaxf(m, bm);
+    const float sc = expf(m - mn);
+    s *= sc;
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) acc[j] *= sc;
+#pragma unroll
+    for (int t = 0; t < E; ++t) {
+      if (u[t] < 0) continue;
+      const float pt = expf(p[t] - mn);
+      s += pt;
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) acc[j] = fmaf(pt, y[t][j], acc[j]);
+    }
+    m = mn;
+  }
+  if (slot < 0) {
+    tc_fwd_store<T, NJ>(a, v, kh, lane, m, s, acc);
+  } else {
+    float* p = a.scratch + (static_cast<int64_t>(slot) * a.H + kh) * (D + 2);
+    if (lane == 0) { p[0] = m; p[1] = s; }
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int col = lane + 32 * j;
+      if (col < D) p[2 + col] = acc[j];
+    }
+  }
+}
+
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32) tconv_fwd_kernel(TcArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int c = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (c >= a.w.n_chunks) return;
+  walk_chunk(a.w, c, [&](int v, int e0, int n, int slot) { tc_fwd_row<T, NJ>(a, v, e0, n, slot, k, lane); });
+}
+
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32) tconv_fwd_fixup_kernel(TcArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int li = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (li >= a.w.n_long) return;
+  float m, s, acc[NJ];
+  fwd_merge<NJ>(a.w, a.scratch, li, k, a.H, a.D, lane, m, s, acc);
+  tc_fwd_store<T, NJ>(a, a.w.long_row[li], k, lane, m, s, acc);
+}
+
+// destination pass of row v, head kh, from the sums over its in-edges (w = a_uv, gd = <g_v, v_u>, ad = w gd):
+//   delta = sum ad,  A = sum ad k_u,  B = sum w k_u  (per column),  dq = scale (A - delta B),
+// since dq_v = scale sum_u a_uv (gd_uv - delta_v) k_u.  The copy of g_v goes next to dq (the input-gradient GEMM reads
+// [dq | g] as one operand).
+template <typename T, int NJ>
+__device__ __forceinline__ void tc_dst_store(const TcArgs& a, int v, int kh, int lane, float sd, const float (&A)[NJ],
+                                             const float (&B)[NJ], const float (&gv)[NJ]) {
+  T* dq = head_row_out<T>(a.out, a.ldo, v, kh, a.D);
+  T* gc = head_row_out<T>(a.out2, a.ldo2, v, kh, a.D);
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int col = lane + 32 * j;
+    if (col < a.D) {
+      dq[col] = from_f<T>(a.scale * fmaf(-sd, B[j], A[j]));
+      gc[col] = from_f<T>(gv[j]);
+    }
+  }
+  if (lane == 0) a.delta_out[static_cast<int64_t>(v) * a.H + kh] = sd;
+}
+
+// scratch of a long-row segment: [H][2 D + 1] = (delta, A[D], B[D])
+template <typename T, int NJ>
+__device__ __forceinline__ void tc_dst_row(const TcArgs& a, int v, int e0, int n, int slot, int kh, int lane) {
+  constexpr int E = tc_edges<NJ>();
+  const int D = a.D;
+  float qv[NJ], gv[NJ], A[NJ], B[NJ];
+  load_head<T, NJ>(head_row<T>(a.q, a.ldq, v, kh, D), D, lane, qv);
+  load_head<T, NJ>(head_row<T>(a.g, a.ldg, v, kh, D), D, lane, gv);
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) { A[j] = 0.f; B[j] = 0.f; }
+  float sd = 0.f;
+  const int64_t vk = static_cast<int64_t>(v) * a.H + kh;
+  const float mv = a.m[vk], sv = a.s[vk];
+  for (int b = 0; sv > 0.f && b < n; b += E) {
+    int u[E];
+    float x[E][NJ], y[E][NJ], p[2 * E];
+    tc_gather<T, NJ, E>(a, e0, b, n, kh, lane, u, x, y);
+#pragma unroll
+    for (int t = 0; t < E; ++t) {
+      p[t] = dot_part<NJ>(qv, x[t]);
+      p[E + t] = dot_part<NJ>(gv, y[t]);
+    }
+    warp_sum_n<2 * E>(p, lane);
+#pragma unroll
+    for (int t = 0; t < E; ++t) {
+      if (u[t] < 0) continue;
+      const float w = __fdiv_rn(expf(__fmul_rn(p[t], a.scale) - mv), sv);
+      const float ad = w * p[E + t];
+      sd += ad;
+#pragma unroll
+      for (int j = 0; j < NJ; ++j) {
+        A[j] = fmaf(ad, x[t][j], A[j]);
+        B[j] = fmaf(w, x[t][j], B[j]);
+      }
+    }
+  }
+  if (slot < 0) {
+    tc_dst_store<T, NJ>(a, v, kh, lane, sd, A, B, gv);
+  } else {
+    float* p = a.scratch + (static_cast<int64_t>(slot) * a.H + kh) * (2 * D + 1);
+    if (lane == 0) p[0] = sd;
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int col = lane + 32 * j;
+      if (col < D) { p[1 + col] = A[j]; p[1 + D + col] = B[j]; }
+    }
+  }
+}
+
+template <typename T, int NJ>
+// no __launch_bounds__: with it ptxas spills the NJ = 2 instances (launched with kGatWarps * 32 threads as well)
+__global__ void tconv_bwd_dst_kernel(TcArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int c = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (c >= a.w.n_chunks) return;
+  walk_chunk(a.w, c, [&](int v, int e0, int n, int slot) { tc_dst_row<T, NJ>(a, v, e0, n, slot, k, lane); });
+}
+
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32) tconv_bwd_dst_fixup_kernel(TcArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int li = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (li >= a.w.n_long) return;
+  const int D = a.D, v = a.w.long_row[li];
+  float sd = 0.f, A[NJ], B[NJ], gv[NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) { A[j] = 0.f; B[j] = 0.f; }
+  for (int sg = a.w.long_seg_ptr[li]; sg < a.w.long_seg_ptr[li + 1]; ++sg) {
+    const float* p = a.scratch + (static_cast<int64_t>(sg) * a.H + k) * (2 * D + 1);
+    sd += p[0];
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int col = lane + 32 * j;
+      if (col < D) { A[j] += p[1 + col]; B[j] += p[1 + D + col]; }
+    }
+  }
+  load_head<T, NJ>(head_row<T>(a.g, a.ldg, v, k, D), D, lane, gv);
+  tc_dst_store<T, NJ>(a, v, k, lane, sd, A, B, gv);
+}
+
+template <typename T, int NJ>
+__device__ __forceinline__ void tc_src_store(const TcArgs& a, int u, int kh, int lane, const float (&dk)[NJ],
+                                             const float (&dv)[NJ]) {
+  T* ok = head_row_out<T>(a.out, a.ldo, u, kh, a.D);
+  T* ov = head_row_out<T>(a.out2, a.ldo2, u, kh, a.D);
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int col = lane + 32 * j;
+    if (col < a.D) {
+      ok[col] = from_f<T>(a.scale * dk[j]);
+      ov[col] = from_f<T>(dv[j]);
+    }
+  }
+}
+
+// over the CSC row u (the destinations v of source u), with c_uv = a_uv (<g_v, v_u> - delta_v):
+//   dv_u = sum_v a_uv g_v,  dk_u = scale sum_v c_uv q_v;  an unkept source gets 0.  Scratch of a segment: [H][2 D].
+template <typename T, int NJ>
+__device__ __forceinline__ void tc_src_row(const TcArgs& a, int u, int e0, int n, int slot, int kh, int lane) {
+  constexpr int E = tc_edges<NJ>();
+  const int D = a.D;
+  float dk[NJ], dv[NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) { dk[j] = 0.f; dv[j] = 0.f; }
+  if (is_kept(a.keep, a.num_in, u)) {
+    float ku[NJ], vu[NJ];
+    load_head<T, NJ>(head_row<T>(a.k, a.ldk, u, kh, D), D, lane, ku);
+    load_head<T, NJ>(head_row<T>(a.v, a.ldv, u, kh, D), D, lane, vu);
+    for (int b = 0; b < n; b += E) {
+      int v[E];
+      float x[E][NJ], y[E][NJ], p[2 * E], mv[E], sv[E], dl[E];
+#pragma unroll
+      for (int t = 0; t < E; ++t) v[t] = b + t < n ? a.w.pidx[e0 + b + t] & kColMask : -1;
+#pragma unroll
+      for (int t = 0; t < E; ++t) {
+        if (v[t] >= 0) {
+          load_head<T, NJ>(head_row<T>(a.q, a.ldq, v[t], kh, D), D, lane, x[t]);
+          load_head<T, NJ>(head_row<T>(a.g, a.ldg, v[t], kh, D), D, lane, y[t]);
+          const int64_t vk = static_cast<int64_t>(v[t]) * a.H + kh;
+          mv[t] = a.m[vk]; sv[t] = a.s[vk]; dl[t] = a.delta[vk];
+        } else {
+#pragma unroll
+          for (int j = 0; j < NJ; ++j) { x[t][j] = 0.f; y[t][j] = 0.f; }
+          mv[t] = 0.f; sv[t] = 0.f; dl[t] = 0.f;
+        }
+      }
+#pragma unroll
+      for (int t = 0; t < E; ++t) {
+        p[t] = dot_part<NJ>(x[t], ku);        // the forward's <q_v, k_u>, column for column
+        p[E + t] = dot_part<NJ>(y[t], vu);    // the destination pass's <g_v, v_u>
+      }
+      warp_sum_n<2 * E>(p, lane);
+#pragma unroll
+      for (int t = 0; t < E; ++t) {
+        if (!(sv[t] > 0.f)) continue;         // also the slots past the row's end
+        const float w = __fdiv_rn(expf(__fmul_rn(p[t], a.scale) - mv[t]), sv[t]);
+        const float c = w * (p[E + t] - dl[t]);
+#pragma unroll
+        for (int j = 0; j < NJ; ++j) {
+          dv[j] = fmaf(w, y[t][j], dv[j]);
+          dk[j] = fmaf(c, x[t][j], dk[j]);
+        }
+      }
+    }
+  }
+  if (slot < 0) {
+    tc_src_store<T, NJ>(a, u, kh, lane, dk, dv);
+  } else {
+    float* p = a.scratch + (static_cast<int64_t>(slot) * a.H + kh) * (2 * D);
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int col = lane + 32 * j;
+      if (col < D) { p[col] = dk[j]; p[D + col] = dv[j]; }
+    }
+  }
+}
+
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32) tconv_bwd_src_kernel(TcArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int c = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (c >= a.w.n_chunks) return;
+  walk_chunk(a.w, c, [&](int u, int e0, int n, int slot) { tc_src_row<T, NJ>(a, u, e0, n, slot, k, lane); });
+}
+
+template <typename T, int NJ>
+__global__ void __launch_bounds__(kGatWarps * 32) tconv_bwd_src_fixup_kernel(TcArgs a) {
+  const int lane = threadIdx.x & 31;
+  const int li = blockIdx.x * kGatWarps + (threadIdx.x >> 5);
+  const int k = blockIdx.y;
+  if (li >= a.w.n_long) return;
+  const int D = a.D;
+  float dk[NJ], dv[NJ];
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) { dk[j] = 0.f; dv[j] = 0.f; }
+  for (int sg = a.w.long_seg_ptr[li]; sg < a.w.long_seg_ptr[li + 1]; ++sg) {
+    const float* p = a.scratch + (static_cast<int64_t>(sg) * a.H + k) * (2 * D);
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int col = lane + 32 * j;
+      if (col < D) { dk[j] += p[col]; dv[j] += p[D + col]; }
+    }
+  }
+  tc_src_store<T, NJ>(a, a.w.long_row[li], k, lane, dk, dv);
+}
+
 // ---------------------------------------------------------------------------------------------------- dispatch
 int nj_of(int32_t D) { return D <= 32 ? 1 : D <= 64 ? 2 : D <= 128 ? 4 : D <= 256 ? 8 : D <= 512 ? 16 : 0; }
 
@@ -922,6 +1287,22 @@ void preload_v2_all() {
   cudaFuncAttributes a;
   cudaFuncGetAttributes(&a, gat_colsum_kernel<T>);
 }
+template <typename T, int NJ>
+void preload_tc_t() {
+  cudaFuncAttributes a;
+  cudaFuncGetAttributes(&a, tconv_fwd_kernel<T, NJ>);
+  cudaFuncGetAttributes(&a, tconv_fwd_fixup_kernel<T, NJ>);
+  cudaFuncGetAttributes(&a, tconv_bwd_dst_kernel<T, NJ>);
+  cudaFuncGetAttributes(&a, tconv_bwd_dst_fixup_kernel<T, NJ>);
+  cudaFuncGetAttributes(&a, tconv_bwd_src_kernel<T, NJ>);
+  cudaFuncGetAttributes(&a, tconv_bwd_src_fixup_kernel<T, NJ>);
+}
+template <typename T>
+void preload_tc_all() {
+  preload_tc_t<T, 1>(); preload_tc_t<T, 2>(); preload_tc_t<T, 4>(); preload_tc_t<T, 8>(); preload_tc_t<T, 16>();
+  cudaFuncAttributes a;
+  cudaFuncGetAttributes(&a, gat_colsum_kernel<T>);
+}
 template <typename T>
 void preload_all() {
   preload_t<T, 1>(); preload_t<T, 2>(); preload_t<T, 4>(); preload_t<T, 8>(); preload_t<T, 16>();
@@ -957,6 +1338,17 @@ static void gatv2_preload() {
   std::call_once(once, [] {
     preload_v2_all<float>();
     preload_v2_all<__nv_bfloat16>();
+    cudaFuncAttributes a;
+    cudaFuncGetAttributes(&a, gat_colsum_final_kernel);
+    cudaGetLastError();
+  });
+}
+
+static void tconv_preload() {
+  static std::once_flag once;
+  std::call_once(once, [] {
+    preload_tc_all<float>();
+    preload_tc_all<__nv_bfloat16>();
     cudaFuncAttributes a;
     cudaFuncGetAttributes(&a, gat_colsum_final_kernel);
     cudaGetLastError();
@@ -1209,6 +1601,106 @@ extern "C" int pg_gatv2_bwd_src(const pg_csr* gt, const void* zs, int64_t ldzs, 
     if (gt->n_long) PG_GAT_NJ(__nv_bfloat16, pg::gatv2_bwd_src_fixup_kernel, grid_fix, st, a);
   } else {
     pg::set_error("pg_gatv2_bwd_src: unknown dtype %d", dtype);
+    return PG_ERR_INVALID;
+  }
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+extern "C" int pg_tconv_preload(void) {
+  pg::tconv_preload();
+  return PG_OK;
+}
+
+extern "C" int pg_tconv_aggregate(const pg_csr* g, const void* q, int64_t ldq, const void* k, int64_t ldk,
+                                  const void* v, int64_t ldv, const void* skip, int64_t ldskip, int32_t H, int32_t D,
+                                  int dtype, float scale, const uint8_t* keep, int32_t num_in, void* out, int64_t ldo,
+                                  float* m, float* s, float* scratch, void* stream) {
+  pg::tconv_preload();
+  if (int rc = pg::check_plan(g, "pg_tconv_aggregate")) return rc;
+  const int nj = pg::nj_of(D);
+  const int64_t hd = static_cast<int64_t>(H) * D;
+  PG_REQUIRE(H > 0 && D > 0 && nj > 0 && ldq >= hd && ldk >= hd && ldv >= hd && ldskip >= hd && ldo >= hd,
+             "pg_tconv_aggregate: bad sizes (H %d, D %d; D must be in 1..512)", H, D);
+  if (g->n_rows == 0) return PG_OK;
+  PG_REQUIRE(q && k && v && skip && out && m && s && (g->n_seg == 0 || scratch), "pg_tconv_aggregate: null argument");
+  pg::TcArgs a{pg::make_walk(g), q, ldq, k, ldk, v, ldv, skip, ldskip, nullptr, 0, nullptr, nullptr, nullptr, keep,
+               num_in, out, ldo, nullptr, 0, m, s, nullptr, scratch, scale, H, D};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const dim3 grid((g->n_chunks + kGatWarps - 1) / kGatWarps, H), grid_fix((g->n_long + kGatWarps - 1) / kGatWarps, H);
+  if (dtype == PG_F32) {
+    if (g->n_chunks) PG_GAT_NJ(float, pg::tconv_fwd_kernel, grid, st, a);
+    if (g->n_long) PG_GAT_NJ(float, pg::tconv_fwd_fixup_kernel, grid_fix, st, a);
+  } else if (dtype == PG_BF16) {
+    if (g->n_chunks) PG_GAT_NJ(__nv_bfloat16, pg::tconv_fwd_kernel, grid, st, a);
+    if (g->n_long) PG_GAT_NJ(__nv_bfloat16, pg::tconv_fwd_fixup_kernel, grid_fix, st, a);
+  } else {
+    pg::set_error("pg_tconv_aggregate: unknown dtype %d", dtype);
+    return PG_ERR_INVALID;
+  }
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+extern "C" int pg_tconv_bwd_dst(const pg_csr* g, const void* q, int64_t ldq, const void* k, int64_t ldk,
+                                const void* v, int64_t ldv, const void* grad, int64_t ldg, int32_t H, int32_t D,
+                                int dtype, float scale, const float* m, const float* s, const uint8_t* keep,
+                                int32_t num_in, void* dq, int64_t lddq, void* gcopy, int64_t ldgc, float* delta,
+                                float* scratch, void* stream) {
+  pg::tconv_preload();
+  if (int rc = pg::check_plan(g, "pg_tconv_bwd_dst")) return rc;
+  const int nj = pg::nj_of(D);
+  const int64_t hd = static_cast<int64_t>(H) * D;
+  PG_REQUIRE(H > 0 && D > 0 && nj > 0 && ldq >= hd && ldk >= hd && ldv >= hd && ldg >= hd && lddq >= hd && ldgc >= hd,
+             "pg_tconv_bwd_dst: bad sizes (H %d, D %d; D must be in 1..512)", H, D);
+  if (g->n_rows == 0) return PG_OK;
+  PG_REQUIRE(q && k && v && grad && m && s && dq && gcopy && delta && (g->n_seg == 0 || scratch),
+             "pg_tconv_bwd_dst: null argument");
+  pg::TcArgs a{pg::make_walk(g), q, ldq, k, ldk, v, ldv, nullptr, 0, grad, ldg, m, s, nullptr, keep,
+               num_in, dq, lddq, gcopy, ldgc, nullptr, nullptr, delta, scratch, scale, H, D};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const dim3 grid((g->n_chunks + kGatWarps - 1) / kGatWarps, H), grid_fix((g->n_long + kGatWarps - 1) / kGatWarps, H);
+  if (dtype == PG_F32) {
+    if (g->n_chunks) PG_GAT_NJ(float, pg::tconv_bwd_dst_kernel, grid, st, a);
+    if (g->n_long) PG_GAT_NJ(float, pg::tconv_bwd_dst_fixup_kernel, grid_fix, st, a);
+  } else if (dtype == PG_BF16) {
+    if (g->n_chunks) PG_GAT_NJ(__nv_bfloat16, pg::tconv_bwd_dst_kernel, grid, st, a);
+    if (g->n_long) PG_GAT_NJ(__nv_bfloat16, pg::tconv_bwd_dst_fixup_kernel, grid_fix, st, a);
+  } else {
+    pg::set_error("pg_tconv_bwd_dst: unknown dtype %d", dtype);
+    return PG_ERR_INVALID;
+  }
+  PG_LAUNCH_CHECK();
+  return PG_OK;
+}
+
+extern "C" int pg_tconv_bwd_src(const pg_csr* gt, const void* q, int64_t ldq, const void* k, int64_t ldk,
+                                const void* v, int64_t ldv, const void* grad, int64_t ldg, int32_t H, int32_t D,
+                                int dtype, float scale, const float* m, const float* s, const float* delta,
+                                const uint8_t* keep, int32_t num_in, void* dk, int64_t lddk, void* dv, int64_t lddv,
+                                float* scratch, void* stream) {
+  pg::tconv_preload();
+  if (int rc = pg::check_plan(gt, "pg_tconv_bwd_src")) return rc;
+  const int nj = pg::nj_of(D);
+  const int64_t hd = static_cast<int64_t>(H) * D;
+  PG_REQUIRE(H > 0 && D > 0 && nj > 0 && ldq >= hd && ldk >= hd && ldv >= hd && ldg >= hd && lddk >= hd &&
+                 lddv >= hd && num_in >= 0,
+             "pg_tconv_bwd_src: bad sizes (H %d, D %d; D must be in 1..512)", H, D);
+  if (gt->n_rows == 0) return PG_OK;
+  PG_REQUIRE(k && v && (num_in == 0 || (q && grad && m && s && delta)) && dk && dv && (gt->n_seg == 0 || scratch),
+             "pg_tconv_bwd_src: null argument");
+  pg::TcArgs a{pg::make_walk(gt), q, ldq, k, ldk, v, ldv, nullptr, 0, grad, ldg, m, s, delta, keep,
+               num_in, dk, lddk, dv, lddv, nullptr, nullptr, nullptr, scratch, scale, H, D};
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const dim3 grid((gt->n_chunks + kGatWarps - 1) / kGatWarps, H), grid_fix((gt->n_long + kGatWarps - 1) / kGatWarps, H);
+  if (dtype == PG_F32) {
+    if (gt->n_chunks) PG_GAT_NJ(float, pg::tconv_bwd_src_kernel, grid, st, a);
+    if (gt->n_long) PG_GAT_NJ(float, pg::tconv_bwd_src_fixup_kernel, grid_fix, st, a);
+  } else if (dtype == PG_BF16) {
+    if (gt->n_chunks) PG_GAT_NJ(__nv_bfloat16, pg::tconv_bwd_src_kernel, grid, st, a);
+    if (gt->n_long) PG_GAT_NJ(__nv_bfloat16, pg::tconv_bwd_src_fixup_kernel, grid_fix, st, a);
+  } else {
+    pg::set_error("pg_tconv_bwd_src: unknown dtype %d", dtype);
     return PG_ERR_INVALID;
   }
   PG_LAUNCH_CHECK();

@@ -17,9 +17,10 @@ training: every epoch each partition keeps a random fraction p of its halo nodes
 that epoch, so the halo exchange moves p times the bytes.  Evaluation always uses the full graph.  Like
 `--eval-partitioned` it has a suppressed default: read it with getattr(args, 'sampling_rate', 1.0).
 
-`--model gat` trains graph attention (DGL's GATConv) instead of GraphSAGE, and `--model gatv2` dynamic graph attention
-(DGL's GATv2Conv); `--n-heads k` (not in the reference, default 4, suppressed like `--sampling-rate`: read it with
-getattr(args, 'n_heads', 4)) sets the heads per hidden layer of either.
+`--model gat` trains graph attention (DGL's GATConv) instead of GraphSAGE, `--model gatv2` dynamic graph attention
+(DGL's GATv2Conv) and `--model transformer` the graph transformer (PyG's TransformerConv: dot-product attention over
+the in-edges with a skip connection); `--n-heads k` (not in the reference, default 4, suppressed like
+`--sampling-rate`: read it with getattr(args, 'n_heads', 4)) sets the heads per hidden layer of each of them.
 
 `--model graphconv` (not in the reference) trains Kipf & Welling's graph convolution (DGL's GraphConv, norm='both'):
 every layer aggregates c_v sum_u c_u h_u with c = deg^-1/2, the halo rows' degrees supplied by their owners.  `--model
@@ -33,7 +34,8 @@ read it with getattr(args, 'halo_bits', None).
 
 `--aggregator {mean,pool}` (not in the reference) selects the neighbour reduction of the GraphSAGE layers: `mean` (the
 reference's) or `pool`, Hamilton et al.'s max-pool aggregator (DGL `SAGEConv(aggregator_type='pool')`): every layer
-takes the element-wise neighbour maximum of ReLU(h Wp^T + bp).  It cannot be combined with --model gat, --model gatv2 or --use-pp.
+takes the element-wise neighbour maximum of ReLU(h Wp^T + bp).  It cannot be combined with --model gat, gatv2 or
+transformer, or with --use-pp.
 Suppressed like `--sampling-rate`: read it with getattr(args, 'aggregator', 'mean').
 
 `--model gcnii` (not in the reference) trains GCNII (Chen et al., ICML 2020; DGL's GCN2Conv): graph layer 0 is a linear
@@ -50,8 +52,8 @@ import argparse
 _FLAGS = [
     ("dataset", dict(type=str, default='reddit', help="the input dataset (or synthetic:<shape>)")),
     ("graph-name", dict(type=str, default='')),
-    ("model", dict(type=str, default='graphsage', help="model for training (graphsage | gcn | gat | gatv2 | graphconv | "
-                                                              "gcnii; gcn is GraphSAGE)")),
+    ("model", dict(type=str, default='graphsage', help="model for training (graphsage | gcn | gat | gatv2 | transformer | "
+                                                              "graphconv | gcnii; gcn is GraphSAGE)")),
     ("dropout", dict(type=float, default=0.5, help="dropout probability")),
     ("lr", dict(type=float, default=1e-2, help="learning rate")),
     ("n-epochs", dict(type=int, default=200, help="the number of training epochs")),
@@ -145,7 +147,8 @@ def build_parser():
                         help="boundary-node sampling: the fraction of halo nodes every partition keeps per epoch "
                              "(synchronous training; default 1 = all)")
     parser.add_argument('--n-heads', '--n_heads', type=_n_heads, default=argparse.SUPPRESS,
-                        help="--model gat / gatv2: attention heads of every hidden layer (default 4)")
+                        help="--model gat / gatv2 / transformer: attention heads of every hidden layer "
+                             "(default 4)")
     parser.add_argument('--halo-bits', '--halo_bits', type=int, choices=[8, 4], default=argparse.SUPPRESS,
                         help="send the halo messages of graph layers >= 1 as stochastically rounded 8- or 4-bit codes "
                              "(default: exact)")

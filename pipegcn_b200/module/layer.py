@@ -36,6 +36,19 @@ State-dict keys are GATv2Conv's: `fc_src.weight` / `fc_dst.weight` [H*D, d_in], 
 gain = calculate_gain('relu'): xavier_normal_(fc_src.weight), fc_src.bias = 0, xavier_normal_(fc_dst.weight),
 fc_dst.bias = 0, xavier_normal_(attn).
 
+`TransformerLayer` (not in the reference): PyG's `TransformerConv` with concat=True, beta=False, dropout=0,
+edge_dim=None, bias=True, root_weight=True (Shi et al., "Masked Label Prediction: Unified Message Passing Model for
+Semi-Supervised Classification", IJCAI 2021), over the same rows, per head k:
+
+    q = h[:N_in] @ W_q^T + b_q,  k = h @ W_k^T + b_k,  v = h @ W_v^T + b_v,  skip = h[:N_in] @ W_s^T + b_s,
+    e_uv = <q[v, k], k[u, k]> / sqrt(D),
+    out[v, k] = sum_u softmax_u(e_uv) v[u, k] + skip[v, k]       (attention part 0 for a row without in-edges)
+
+State-dict keys are TransformerConv's: `lin_query.*`, `lin_key.*`, `lin_value.*`, `lin_skip.*`, weights [H*D, d_in]
+and biases [H*D].  Initialisation is TransformerConv.reset_parameters, in this draw order, each PyG `Linear` drawing
+as `nn.Linear` does (weight kaiming_uniform_(a=sqrt(5)), then bias U(-1/sqrt(d_in), 1/sqrt(d_in))): lin_key,
+lin_query, lin_value, lin_skip.
+
 `GraphConvLayer` (not in the reference): DGL's `GraphConv(in, out, norm='both', weight=True, bias=True)` (Kipf & Welling,
 "Semi-Supervised Classification with Graph Convolutional Networks", ICLR 2017), no activation inside, over the same
 rows, with c = clamp(deg, min=1)^(-1/2) of every [inner | halo] row (deg: in-degree with the self loop in the whole
@@ -237,3 +250,26 @@ class GATv2Layer(nn.Module):
         """As GATLayer.forward."""
         return ops.gatv2_layer(feat, graph, keep, self.num_heads, self.fc_src.weight, self.fc_src.bias,
                                self.fc_dst.weight, self.fc_dst.bias, self.attn, drop_bwd)
+
+
+class TransformerLayer(nn.Module):
+
+    def __init__(self, in_feats, out_feats, num_heads):
+        super().__init__()
+        self.in_feats, self.out_feats, self.num_heads = in_feats, out_feats, num_heads
+        self.lin_key = nn.Linear(in_feats, out_feats * num_heads)
+        self.lin_query = nn.Linear(in_feats, out_feats * num_heads)
+        self.lin_value = nn.Linear(in_feats, out_feats * num_heads)
+        self.lin_skip = nn.Linear(in_feats, out_feats * num_heads)
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        """TransformerConv.reset_parameters (beta=False, root_weight=True)."""
+        for lin in (self.lin_key, self.lin_query, self.lin_value, self.lin_skip):
+            lin.reset_parameters()
+
+    def forward(self, graph, feat, keep=None, drop_bwd=None):
+        """As GATLayer.forward."""
+        return ops.transformer_layer(feat, graph, keep, self.num_heads, self.lin_query.weight, self.lin_query.bias,
+                                     self.lin_key.weight, self.lin_key.bias, self.lin_value.weight,
+                                     self.lin_value.bias, self.lin_skip.weight, self.lin_skip.bias, drop_bwd)

@@ -23,6 +23,9 @@ and unkept rows are absent from every softmax.
 `GATv2(GAT)` (not in the reference) is `GAT` with `GATv2Layer`s (DGL's GATv2Conv): the same heads, keep mask and
 partitioned evaluation; only the graph layers and the kernels they load differ.
 
+`GraphTransformer(GAT)` (not in the reference) is `GAT` with `TransformerLayer`s (PyG's TransformerConv): the same
+heads, keep mask and partitioned evaluation; only the graph layers and the kernels they load differ.
+
 `GraphConv(GraphSAGE)` (not in the reference) is the same layer loop with `GraphConvLayer`s (DGL's GraphConv,
 norm='both'): the layers read the symmetric norm from the graph (`PartGraph.sym_norm`) instead of the in-degrees.
 `GCN` stays the reference's name for GraphSAGE.
@@ -38,7 +41,7 @@ from torch import nn
 import torch.nn.functional as F
 
 from ..helper import context as ctx
-from .layer import GATLayer, GATv2Layer, GCNIILayer, GraphConvLayer, GraphSAGELayer
+from .layer import GATLayer, GATv2Layer, GCNIILayer, GraphConvLayer, GraphSAGELayer, TransformerLayer
 
 
 class GNNBase(nn.Module):
@@ -330,3 +333,15 @@ class GATv2(GAT):
     def _preload(self):
         from .. import ops
         ops.gatv2_preload()
+
+
+class GraphTransformer(GAT):
+
+    def _graph_layer(self, i, d_in, d_out):
+        if i < self.n_layers - 1:
+            return TransformerLayer(d_in, d_out // self.n_heads, self.n_heads)
+        return TransformerLayer(d_in, d_out, 1)          # the logits: one head of n_class, and so does the skip
+
+    def _preload(self):
+        from .. import ops
+        ops.transformer_preload()

@@ -7,6 +7,7 @@ the aggregate / exchange path.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 
 import torch
@@ -1353,6 +1354,184 @@ class GatV2LayerFn(torch.autograd.Function):
 
 def gatv2_layer(feat, graph, keep, heads, w_s, b_s, w_d, b_d, attn, drop_bwd=None) -> torch.Tensor:
     return GatV2LayerFn.apply(feat, graph, keep, int(heads), w_s, b_s, w_d, b_d, attn, drop_bwd)
+
+
+# ---- graph transformer, TransformerConv (csrc/attention.cu) -------------------------------------------------
+def transformer_preload():
+    """Load every graph-transformer kernel now (see gat_preload)."""
+    _C.check(_C.lib.pg_tconv_preload(), "pg_tconv_preload")
+
+
+def transformer_width(hd: int, dtype) -> int:
+    """Columns of each half of the paired [k | v] and [q | skip] operands: H*D, rounded up to a multiple of 8 when
+    H*D elements are not a multiple of 16 bytes, so that the second half starts 16-byte aligned like every GEMM
+    operand (a misaligned view would be copied by _tma_ready)."""
+    es = torch.empty((), dtype=dtype).element_size()
+    return hd if (hd * es) % 16 == 0 else (hd + 7) // 8 * 8
+
+
+def _tconv_scale(d: int) -> float:
+    return 1.0 / math.sqrt(d)
+
+
+def transformer_aggregate(graph: PartGraph, q, k, v, skip, heads: int, keep=None):
+    """out [N_in, H*D] = per-head edge softmax of <q[v], k[u]> / sqrt(D) over the forward CSR applied to v, + skip;
+    with the softmax statistics m, s [N_in, H] fp32."""
+    plan = graph.fwd
+    n, hd = plan.n_rows, q.shape[1]
+    d = hd // heads
+    out = alloc_rows(n, hd, q.dtype, q.device)
+    m = torch.empty(n, heads, dtype=torch.float32, device=q.device)
+    s = torch.empty(n, heads, dtype=torch.float32, device=q.device)
+    scratch = plan.scratch(heads * (d + 2))
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_tconv_aggregate(C.byref(plan.c), q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0),
+                                       v.data_ptr(), v.stride(0), skip.data_ptr(), skip.stride(0), heads, d,
+                                       _C.dtype_code(q.dtype), _tconv_scale(d), _ptr(keep), graph.num_in,
+                                       out.data_ptr(), out.stride(0), m.data_ptr(), s.data_ptr(), _ptr(scratch),
+                                       _C.stream_ptr()), "pg_tconv_aggregate")
+    return out, m, s
+
+
+def transformer_bwd_dst(graph: PartGraph, q, k, v, g, m, s, heads: int, keep=None, dq=None, gc=None):
+    """(dq [N_in, H*D], gc = a copy of g, both in q's dtype, delta [N_in, H] fp32) over the forward CSR, with
+    delta_v = sum_u a_uv <g_v, v_u>.  `dq` / `gc`: the views to write (allocated when None)."""
+    plan = graph.fwd
+    n, hd = plan.n_rows, q.shape[1]
+    d = hd // heads
+    dq = alloc_rows(n, hd, q.dtype, q.device) if dq is None else dq
+    gc = alloc_rows(n, hd, q.dtype, q.device) if gc is None else gc
+    delta = torch.empty(n, heads, dtype=torch.float32, device=q.device)
+    scratch = plan.scratch(heads * (2 * d + 1))
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_tconv_bwd_dst(C.byref(plan.c), q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0),
+                                     v.data_ptr(), v.stride(0), g.data_ptr(), g.stride(0), heads, d,
+                                     _C.dtype_code(q.dtype), _tconv_scale(d), m.data_ptr(), s.data_ptr(), _ptr(keep),
+                                     graph.num_in, dq.data_ptr(), dq.stride(0), gc.data_ptr(), gc.stride(0),
+                                     delta.data_ptr(), _ptr(scratch), _C.stream_ptr()), "pg_tconv_bwd_dst")
+    return dq, gc, delta
+
+
+def transformer_bwd_src(graph: PartGraph, q, k, v, g, m, s, delta, heads: int, keep=None, dk=None, dv=None):
+    """(dk, dv) [num_all, H*D] in k's dtype over the CSC of the graph (0 on unkept halo rows).  `dk` / `dv`: the
+    views to write (allocated when None)."""
+    plan = graph.bwd
+    n, hd = plan.n_rows, k.shape[1]
+    d = hd // heads
+    dk = alloc_rows(n, hd, k.dtype, k.device) if dk is None else dk
+    dv = alloc_rows(n, hd, k.dtype, k.device) if dv is None else dv
+    scratch = plan.scratch(heads * 2 * d)
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_tconv_bwd_src(C.byref(plan.c), q.data_ptr(), q.stride(0), k.data_ptr(), k.stride(0),
+                                     v.data_ptr(), v.stride(0), g.data_ptr(), g.stride(0), heads, d,
+                                     _C.dtype_code(k.dtype), _tconv_scale(d), m.data_ptr(), s.data_ptr(),
+                                     delta.data_ptr(), _ptr(keep), graph.num_in, dk.data_ptr(), dk.stride(0),
+                                     dv.data_ptr(), dv.stride(0), _ptr(scratch), _C.stream_ptr()), "pg_tconv_bwd_src")
+    return dk, dv
+
+
+def _pair_weight(wa, wb, width: int, dtype, transpose: bool = False) -> torch.Tensor:
+    """[2 width, d_in] in the activation dtype with wa in rows [0, H*D) and wb in rows [width, width + H*D), zero
+    rows between (transpose: its [d_in, 2 width] transpose), built from the fp32 masters."""
+    hd, d_in = wa.shape
+    pad = width != hd
+    if transpose:
+        out = alloc_rows(d_in, 2 * width, dtype, wa.device, zero=pad)
+        out[:, :hd].copy_(wa.detach().t())
+        out[:, width:width + hd].copy_(wb.detach().t())
+    else:
+        out = alloc_rows(2 * width, d_in, dtype, wa.device, zero=pad)
+        out[:hd].copy_(wa.detach())
+        out[width:width + hd].copy_(wb.detach())
+    return out
+
+
+def _pair_bias(ba, bb, hd: int, width: int) -> torch.Tensor:
+    out = torch.zeros(2 * width, dtype=torch.float32, device=ba.device)
+    out[:hd].copy_(ba.detach())
+    out[width:width + hd].copy_(bb.detach())
+    return out
+
+
+class TransformerLayerFn(torch.autograd.Function):
+    """One graph-transformer layer (PyG TransformerConv, concat=True, beta=False, root_weight=True, no edge features,
+    no attention dropout) over the [inner | halo] rows `feat` of a partition, returning the inner rows.  With W the
+    half width of transformer_width:
+
+        [k | v]    = feat @ [W_k; W_v]^T + [b_k; b_v]          [num_all, 2W]   one pg_linear over all rows
+        [q | skip] = feat[:N_in] @ [W_q; W_s]^T + [b_q; b_s]   [N_in, 2W]      one pg_linear over the inner rows
+        out = softmax-aggregate(v) + skip                      [N_in, H*D]     pg_tconv_aggregate (+ statistics m, s)
+
+    Backward: dq next to a copy of g (pg_tconv_bwd_dst over the CSR, which also writes delta_v), [dk | dv]
+    (pg_tconv_bwd_src over the CSC), the bias gradients as fixed-order column sums (b_s from the column sum the
+    LayerNorm backward stashed, when there is one; b_k's is exactly 0, the softmax being shift-invariant), the weight gradients as one pg_wgrad per row set, and
+    g_feat = [dk | dv] @ [W_k; W_v] (+ [dq | g] @ [W_q; W_s] on the inner rows, one two-source pg_linear), with the
+    dropout backward of `drop_bwd` in its epilogue.  `keep`: the boundary-node sample of the halo rows (uint8), or
+    None."""
+
+    @staticmethod
+    def forward(ctx, feat, graph, keep, heads, w_q, b_q, w_k, b_k, w_v, b_v, w_s, b_s, drop_bwd=None):
+        ctx.drop_bwd = drop_bwd
+        if feat.stride(1) != 1:
+            feat = feat.contiguous()
+        n_in, hd = graph.num_in, w_q.shape[0]
+        w = transformer_width(hd, feat.dtype)
+        fsp = presplit(feat)                   # fp32: one split of feat for both products
+        kv = gemm_nt(fsp, _pair_weight(w_k, w_v, w, feat.dtype), bias=_pair_bias(b_k, b_v, hd, w))
+        qs = gemm_nt(fsp.rows(0, n_in) if isinstance(fsp, Split) else feat[:n_in],
+                     _pair_weight(w_q, w_s, w, feat.dtype), bias=_pair_bias(b_q, b_s, hd, w))
+        out, m, s = transformer_aggregate(graph, qs[:, :hd], kv[:, :hd], kv[:, w:w + hd], qs[:, w:w + hd], heads,
+                                          keep)
+        ctx.save_for_backward(feat, kv, qs, m, s, w_q, w_k, w_v, w_s)
+        ctx.graph, ctx.keep, ctx.heads, ctx.width = graph, keep, heads, w
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        feat, kv, qs, m, s, w_q, w_k, w_v, w_s = ctx.saved_tensors
+        graph, heads, keep, w = ctx.graph, ctx.heads, ctx.keep, ctx.width
+        n_in, n_all, hd = graph.num_in, feat.shape[0], w_q.shape[0]
+        colsum = _take_colsum(g)
+        g = _tma_ready(g if g.dtype == feat.dtype else g.to(feat.dtype))
+        q, k, v = qs[:, :hd], kv[:, :hd], kv[:, w:w + hd]
+        dqg = alloc_rows(n_in, 2 * w, feat.dtype, feat.device, zero=w != hd)
+        dkv = alloc_rows(n_all, 2 * w, feat.dtype, feat.device, zero=w != hd)
+        _, _, delta = transformer_bwd_dst(graph, q, k, v, g, m, s, heads, keep, dq=dqg[:, :hd], gc=dqg[:, w:w + hd])
+        transformer_bwd_src(graph, q, k, v, g, m, s, delta, heads, keep, dk=dkv[:, :hd], dv=dkv[:, w:w + hd])
+        # b_k shifts every score of a destination row by the same <q_v, b_k>, which the softmax cancels: its gradient
+        # sum_u dk_u = scale sum_v q_v sum_u a_uv (gd_uv - delta_v) is exactly 0, so it is not summed from rounded dk
+        gbk = torch.zeros(hd, dtype=torch.float32, device=feat.device)
+        gbv = gat_colsum(dkv[:, w:w + hd])
+        if colsum is not None:
+            gbq, gbs = gat_colsum(dqg[:, :hd]), colsum
+        else:
+            gb_qs = gat_colsum(dqg)
+            gbq, gbs = gb_qs[:hd], gb_qs[w:w + hd]
+        dkvp, dqgp = presplit(dkv), presplit(dqg)
+        is_split = isinstance(dkvp, Split)
+        g_feat = None
+        if ctx.needs_input_grad[0]:
+            g_feat = alloc_rows(n_all, feat.shape[1], feat.dtype, feat.device)
+            wkv = _pair_weight(w_k, w_v, w, feat.dtype, transpose=True)
+            drop = ctx.drop_bwd if ctx.drop_bwd is not None and ctx.drop_bwd.p > 0 else None
+            db = drop if drop is not None and feat.shape[1] <= 256 and _drop_ok(g_feat) else None
+            gemm_nt(dkvp.rows(0, n_in) if is_split else dkv[:n_in], wkv, dqgp,
+                    _pair_weight(w_q, w_s, w, feat.dtype, transpose=True), out=g_feat[:n_in], drop=db)
+            if n_all > n_in:
+                gemm_nt(dkvp.rows(n_in) if is_split else dkv[n_in:], wkv, out=g_feat[n_in:], drop=db, drop_row0=n_in)
+            if drop is not None and db is None:
+                dropout_rows(g_feat, drop, out=g_feat)
+        fsp = presplit(feat)
+        gw_kv = wgrad(dkvp, fsp)
+        gw_qs = wgrad(dqgp, fsp.rows(0, n_in) if isinstance(fsp, Split) else feat[:n_in])
+        gwq, gwk, gwv, gws = [t.contiguous() for t in (gw_qs[:hd], gw_kv[:hd], gw_kv[w:w + hd], gw_qs[w:w + hd])]
+        return (g_feat, None, None, None, gwq.to(w_q.dtype), gbq.contiguous(), gwk.to(w_k.dtype), gbk,
+                gwv.to(w_v.dtype), gbv, gws.to(w_s.dtype), gbs.contiguous(), None)
+
+
+def transformer_layer(feat, graph, keep, heads, w_q, b_q, w_k, b_k, w_v, b_v, w_s, b_s,
+                      drop_bwd=None) -> torch.Tensor:
+    return TransformerLayerFn.apply(feat, graph, keep, int(heads), w_q, b_q, w_k, b_k, w_v, b_v, w_s, b_s, drop_bwd)
 
 
 # ---- max-pool GraphSAGE (csrc/pool.cu) ---------------------------------------------------------------------

@@ -32,7 +32,7 @@ from .helper import context as ctx
 from .helper.feature_buffer import Buffer, EvalExchange, OneShotExchange, check_halo_bits, check_sampling
 from .helper.reducer import Reducer
 from .helper.timer.comm_timer import CommTimer
-from .module.model import GAT, GATv2, GCNII, GraphConv, GraphSAGE
+from .module.model import GAT, GATv2, GCNII, GraphConv, GraphSAGE, GraphTransformer
 from .partition import PartitionLayout, get_layer_size
 
 
@@ -47,14 +47,15 @@ def _quant_seed(args):
 
 
 def check_model(args):
-    """Refuses, before anything is allocated, a configuration that is not implemented: --model gat or gatv2 with
-    --use-pp (the precompute is GraphSAGE's neighbour mean) or with a hidden width that does not split into --n-heads
-    heads, and --aggregator pool with an attention model (an attention layer has no aggregator) or with --use-pp (a
-    neighbour mean).  --model graphconv refuses --aggregator pool (it has no aggregator) and --sampling-rate < 1 (the
-    symmetric norm of a sampled graph needs every source's sampled out-degree, which depends on every peer's sample).
-    --model gcnii refuses the same two, --n-linear 0 (its last convolution is square: the logits come from a linear)
-    and --use-pp (graph layer 0 begins with fc_in, so a precomputed neighbour aggregate of x has no place)."""
-    attention = args.model in ('gat', 'gatv2')
+    """Refuses, before anything is allocated, a configuration that is not implemented: --model gat, gatv2 or
+    transformer with --use-pp (the precompute is GraphSAGE's neighbour mean) or with a hidden width that does not
+    split into --n-heads heads, and --aggregator pool with an attention model (an attention layer has no aggregator)
+    or with --use-pp (a neighbour mean).  --model graphconv refuses --aggregator pool (it has no aggregator) and
+    --sampling-rate < 1 (the symmetric norm of a sampled graph needs every source's sampled out-degree, which
+    depends on every peer's sample).  --model gcnii refuses the same two, --n-linear 0 (its last convolution is
+    square: the logits come from a linear) and --use-pp (graph layer 0 begins with fc_in, so a precomputed neighbour
+    aggregate of x has no place)."""
+    attention = args.model in ('gat', 'gatv2', 'transformer')
     aggregator = getattr(args, 'aggregator', 'mean')
     if aggregator not in ('mean', 'pool'):
         raise ValueError(f"--aggregator {aggregator}: expected mean or pool")
@@ -109,8 +110,8 @@ def create_model(layer_size, args, buffer=None, dtype=torch.float32):
         return GCNII(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
                      train_size=args.n_train, buffer=buffer, dtype=dtype, alpha=getattr(args, 'gcnii_alpha', 0.1),
                      lam=getattr(args, 'gcnii_lambda', 0.5))
-    if args.model in ('gat', 'gatv2'):
-        cls = GAT if args.model == 'gat' else GATv2
+    if args.model in ('gat', 'gatv2', 'transformer'):
+        cls = {'gat': GAT, 'gatv2': GATv2, 'transformer': GraphTransformer}[args.model]
         return cls(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
                    train_size=args.n_train, buffer=buffer, dtype=dtype, n_heads=getattr(args, 'n_heads', 4))
     raise NotImplementedError(args.model)
