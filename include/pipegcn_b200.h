@@ -412,6 +412,13 @@ int pg_boundary_add_q(void* grad, int64_t ld_grad, int32_t d, int dtype, const u
  * with keep[u - num_in] == 0 is absent from every softmax and gets no gradient.  The plan must carry the chunk table
  * (pg_csr::chunks); `scratch` is fp32 of n_seg * H * (D + 2) floats (may be NULL when n_seg == 0).  fp32 accumulation,
  * no atomics, no per-edge storage, D <= 512; the results are the same bits from run to run.
+ * For this section, GATv2's and the graph transformer's:
+ * - A destination row without a kept source (no in-edge, or every source unkept) gets m = -inf, s = 0 and the
+ *   output bias (GAT), 0 (GATv2) or skip (transformer) rounded once to the dtype; its gradient terms are exactly 0,
+ *   and so are the source-pass outputs of an unkept halo row and of a row that is nobody's source (except GAT's
+ *   der (x) attn_r of an inner row).
+ * - Every pass writes columns [0, H * D) of each row of its wide outputs, [0, H) of each row of the per-head ones,
+ *   and nothing else: no pad columns, no other rows.
  * ---------------------------------------------------------------------------------------- */
 /* loads every attention kernel (call it before any halo wait can spin: a first launch may wait for the device) */
 int pg_gat_preload(void);
