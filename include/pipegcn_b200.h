@@ -290,10 +290,16 @@ int pg_push_rows_per_cta(void);
  * scalars of `t *= m; t += (1 - m) * recv` (feature_buffer.py:190-191) */
 /* the flag value published is `value` (+ *value_dev when value_dev != NULL: an epoch counter that lives on the
  * device, so that a captured CUDA graph of an epoch can be replayed) */
+/* Vectors: the widest of 16, 8, 4 and (bf16) 2 bytes that src's base address and row stride allow, V elements each
+ * (V = 1 for a bf16 source of odd stride, such as a contiguous [N, d] tensor with odd d).  Row r of message m is
+ * written as columns [0, round_up(d, V)) of dst + r * ld_dst -- the tail of the last vector receives src's own pad
+ * columns (with `ema`, the mirror's columns [0, round_up(d, V)) are updated too) -- so ld_dst and ld_ema must be
+ * >= round_up(d, V), and dst must be aligned to the vector.  Rows >= n_rows are not touched. */
 int pg_halo_push(const pg_msg* msgs, int32_t n_msgs, int32_t n_ctas, const void* src, int64_t ld_src, int32_t d,
                  int dtype, float momentum, float one_minus, uint32_t value, const uint32_t* value_dev, void* stream);
 /* the same with the RECEIVER's dropout applied to every row as it is stored into peer memory (after the EMA, whose
- * mirror stays clean): the halo rows arrive as the rows of dropout(cat(feat, halo)) the receiver will consume */
+ * mirror stays clean): the halo rows arrive as the rows of dropout(cat(feat, halo)) the receiver will consume.  The
+ * mask is defined on 16-byte vectors: a source that allows narrower ones is refused (PG_ERR_INVALID). */
 int pg_halo_push_drop(const pg_msg* msgs, int32_t n_msgs, int32_t n_ctas, const void* src, int64_t ld_src, int32_t d,
                       int dtype, float momentum, float one_minus, uint32_t value, const uint32_t* value_dev,
                       const pg_drop* drop, void* stream);
@@ -319,7 +325,9 @@ int pg_scale_rows(const void* src, int64_t ld_src, void* dst, int64_t ld_dst, in
 
 /*
  * grad[urow[i], 0:d] += sum_k recv[usrc[k], 0:d]  for k in [uptr[i], uptr[i+1]), in that order
- * (peers ascending), replacing the per-peer loop at feature_buffer.py:208-217.
+ * (peers ascending), replacing the per-peer loop at feature_buffer.py:208-217.  bf16 sums are rounded to bf16
+ * after every add.  Like the push, rows are moved in the widest vectors both operands allow (bf16: at least 4
+ * bytes, else PG_ERR_INVALID), and columns [0, round_up(d, V)) of the urow rows are written.
  */
 int pg_boundary_add(void* grad, int64_t ld_grad, const void* recv, int64_t ld_recv, int32_t d, int dtype,
                     const int32_t* urow, const int32_t* uptr, const int32_t* usrc, int32_t n_urow, void* stream);

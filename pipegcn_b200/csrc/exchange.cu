@@ -365,6 +365,12 @@ static int halo_push_t(const pg_msg* msgs, int n_msgs, int n_ctas, const void* s
       case 16: halo_push_kernel<T, 16><<<n_ctas, kPushThreads, 0, st>>>(msgs, n_msgs, sp, ld_src, nvec, momentum, one_minus, value, value_dev, da); break;
       case 8: halo_push_kernel<T, 8><<<n_ctas, kPushThreads, 0, st>>>(msgs, n_msgs, sp, ld_src, nvec, momentum, one_minus, value, value_dev, da); break;
       case 4: halo_push_kernel<T, 4><<<n_ctas, kPushThreads, 0, st>>>(msgs, n_msgs, sp, ld_src, nvec, momentum, one_minus, value, value_dev, da); break;
+      case 2:      // bf16 rows of odd stride or base, e.g. a contiguous [N, d] tensor with odd d
+        if constexpr (sizeof(T) == 2) {
+          halo_push_kernel<T, 2><<<n_ctas, kPushThreads, 0, st>>>(msgs, n_msgs, sp, ld_src, nvec, momentum, one_minus, value, value_dev, da);
+          break;
+        }
+        [[fallthrough]];
       default: set_error("pg_halo_push: unsupported vector width %d", vb); return PG_ERR_INVALID;
     }
     PG_LAUNCH_CHECK();
@@ -378,7 +384,8 @@ extern "C" int pg_push_rows_per_cta(void) { return pg::kPushRows; }
 
 // `vec_hint` is folded into ld_src's alignment: all message buffers are allocated by
 // Buffer.init_buffer with the same padded stride, the host passes d and strides, and the
-// widest vector legal for src is used; destinations must be at least as aligned.
+// widest vector legal for src is used (16, 8, 4 or, for bf16, 2 bytes); destinations must be
+// at least as aligned, and their stride at least round_up(d, vector) (the header's write region).
 extern "C" int pg_halo_push(const pg_msg* msgs, int32_t n_msgs, int32_t n_ctas, const void* src, int64_t ld_src,
                             int32_t d, int dtype, float momentum, float one_minus, uint32_t value, const uint32_t* value_dev,
                             void* stream) {

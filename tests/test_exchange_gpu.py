@@ -16,8 +16,11 @@ MODES = {
 
 
 @pytest.mark.parametrize("mode", list(MODES))
-@pytest.mark.parametrize("n_parts", [2, 3])
-def test_buffer_replay_bit_exact(n_parts, mode):
+@pytest.mark.parametrize("n_parts,n_hidden", [(2, 16), (3, 16), (4, 16), (8, 16), (4, 37), (8, 37)],
+                         ids=["2", "3", "4", "8", "4-h37", "8-h37"])
+def test_buffer_replay_bit_exact(n_parts, n_hidden, mode):
+    """P = 8 is the partition count the project is measured at (seven peers per push); a hidden width of 37 leaves
+    a ragged last 16-byte vector in every row of the hidden layers."""
     from oracle.train import run_world
     from pipegcn_b200.helper.feature_buffer import Buffer
     from pipegcn_b200.helper.timer.comm_timer import CommTimer
@@ -27,7 +30,7 @@ def test_buffer_replay_bit_exact(n_parts, mode):
 
     g, _, layouts, setups = small_world("tiny", n_parts)
     n_epochs, n_layers = 4, 3
-    oargs, _ = make_args(g, 5, n_epochs=n_epochs, n_layers=n_layers, **MODES[mode])
+    oargs, _ = make_args(g, 5, n_epochs=n_epochs, n_layers=n_layers, n_hidden=n_hidden, **MODES[mode])
     traces = run_world(setups, oargs)
     layer_size = get_layer_size(g.n_feat, oargs.n_hidden, 5, n_layers)[:n_layers]
 
