@@ -549,6 +549,54 @@ int pg_max_aggregate_bwd(const pg_csr* gt, const void* q, int64_t ldq, const int
                          int64_t ld_scratch, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Principal neighbourhood aggregation (DGL PNAConvTower, aggregators mean/max/min/std) over the `_U` rows
+ * [inner | halo] of one partition.  zs [num_all, d] (fp32 or bf16, `dtype`) is the source half h W_s^T of the message
+ * linear, zd [N_in, d] fp32 its destination half h W_d^T + b.  For the in-edges u -> v of the forward CSR g (each edge
+ * once, D_v of them), per column:
+ *   mu = mean_u zs[u],  var = mean_u (zs[u] - mu)^2,  mx / mn = max_u / min_u zs[u] with sources A+ / A-
+ *   agg[v] = [mu + zd | mx + zd | mn + zd | sqrt(max(var, 0) + 1e-30)]   (zd added in fp32, one rounding to dtype)
+ * The four parts start `seg` elements apart (seg >= d, a multiple of the 16-byte vector); columns [d, seg) of each part
+ * are not written.  The moments use Welford's update per edge and Chan's merge across long-row segments, so a row whose
+ * sources are all equal gets var = 0 exactly.  A tie of an extreme goes to the first source in CSR order; the first NaN
+ * source becomes the value and the source.  A row without in-edges gets agg = 0, mu = var = 0 and A+- = -1.  A+- hold
+ * int32 `_U` row ids.  mu / var (fp32) and A+ / A- may be NULL (pairwise): they are then not written.  Rows start on
+ * 16-byte boundaries with strides that are multiples of 16 bytes, covering the last 16-byte vector of a row.  The plans
+ * must carry the chunk table; scratch is fp32 [n_seg][ld_scratch] (may be NULL when n_seg == 0).  No atomics: the
+ * results are the same bits from run to run.
+ * ---------------------------------------------------------------------------------------- */
+/* loads every PNA kernel (call it before any halo wait can spin: a first launch may wait for the device) */
+int pg_pna_preload(void);
+/* agg [N_in, 4 seg] (dtype), mu / var [N_in, d] fp32, A+ / A- [N_in, d] int32 over the forward CSR g;
+ * ld_scratch >= 6 d */
+int pg_pna_aggregate(const pg_csr* g, const void* zs, int64_t ldz, const float* zd, int64_t ldzd, int32_t d, int dtype,
+                     void* agg, int64_t ldagg, int64_t seg, float* mu, float* var, int64_t ldst, int32_t* amax,
+                     int32_t* amin, int64_t lda, float* scratch, int64_t ld_scratch, void* stream);
+/* out[v, o] = fl(fl(y[v, o] + fl(a[v] z[v, o])) + fl(t[v] z[v, d_out + o])) in fp32, rounded once to dtype: the
+ * degree scalers a (amplification) and t (attenuation) applied to the GEMM outputs y = [h | agg] [W_x; W_1]^T + b and
+ * z = agg [W_2; W_3]^T, fp32 [n_rows, d_out] and [n_rows, 2 d_out] */
+int pg_pna_combine(const float* y, int64_t ldy, const float* z, int64_t ldz, const float* a, const float* t,
+                   int32_t n_rows, int32_t d_out, int dtype, void* out, int64_t ldo, void* stream);
+/* out = [g | a g | t g] (dtype, each product rounded once), the three parts `seg` elements apart; columns
+ * [d_out, seg) of each part are not written */
+int pg_pna_grad_scale(const void* g, int64_t ldg, const float* a, const float* t, int32_t n_rows, int32_t d_out,
+                      int dtype, void* out, int64_t ldo, int64_t seg, void* stream);
+/* per destination element, from g_agg = [g_mu | g_mx | g_mn | g_sigma] (fp32, parts `seg` apart), mu, var and
+ * D_v = indptr[v + 1] - indptr[v]:
+ *   g_zd = g_mu + g_mx + g_mn,  beta = [var > 0] g_sigma / (D sigma),  alpha = g_mu / D - beta mu  (fp32)
+ * g_zd, g_mx and g_mn in dtype, alpha and beta fp32; every output 0 on a row without in-edges */
+int pg_pna_bwd_dst(const int32_t* indptr, const float* gagg, int64_t ldga, int64_t seg, const float* mu,
+                   const float* var, int64_t ldst, int32_t n_rows, int32_t d, int dtype, void* gzd, int64_t ldgzd,
+                   float* alpha, float* beta, int64_t ldab, void* gmx, void* gmn, int64_t ldgm, void* stream);
+/* g_zs[u] = S1 + zs[u] S2 over the CSC row u of gt (rows = all num_all `_U` rows), with S1 = sum alpha_v + the g_mx_v
+ * of the destinations whose A+ is u + the g_mn_v of those whose A- is u, and S2 = sum beta_v, each accumulated in
+ * fp32 in CSC order (edge by edge: alpha, then g_mx, then g_mn); the product is applied once at the end.  A row
+ * without out-edges gets exactly 0.  ld_scratch >= 2 d */
+int pg_pna_bwd_src(const pg_csr* gt, const void* zs, int64_t ldz, const float* alpha, const float* beta, int64_t ldab,
+                   const int32_t* amax, const int32_t* amin, int64_t lda, const void* gmx, const void* gmn,
+                   int64_t ldgm, int32_t d, int dtype, void* gzs, int64_t ldgzs, float* scratch, int64_t ld_scratch,
+                   void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Symmetric heap: device memory that peers map through CUDA IPC (host pointers out).
  * ---------------------------------------------------------------------------------------- */
 #define PG_IPC_HANDLE_BYTES 64

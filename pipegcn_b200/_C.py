@@ -140,6 +140,15 @@ def _load():
         "pg_max_aggregate": (C.c_int, [C.POINTER(pg_csr), vp, i64, i32, C.c_int, vp, i64, vp, i64, vp, i64, vp]),
         "pg_max_aggregate_bwd": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, vp, i64, i32, C.c_int, vp, i64, vp,
                                            i64, vp]),
+        "pg_pna_preload": (C.c_int, []),
+        "pg_pna_aggregate": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, i32, C.c_int, vp, i64, i64, vp, vp, i64,
+                                       vp, vp, i64, vp, i64, vp]),
+        "pg_pna_combine": (C.c_int, [vp, i64, vp, i64, vp, vp, i32, i32, C.c_int, vp, i64, vp]),
+        "pg_pna_grad_scale": (C.c_int, [vp, i64, vp, vp, i32, i32, C.c_int, vp, i64, i64, vp]),
+        "pg_pna_bwd_dst": (C.c_int, [vp, vp, i64, i64, vp, vp, i64, i32, i32, C.c_int, vp, i64, vp, vp, i64, vp, vp,
+                                     i64, vp]),
+        "pg_pna_bwd_src": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, vp, i64, vp, vp, i64, vp, vp, i64, i32, C.c_int,
+                                     vp, i64, vp, i64, vp]),
         "pg_heap_alloc": (C.c_int, [C.c_size_t, C.POINTER(vp)]),
         "pg_heap_free": (C.c_int, [vp]),
         "pg_ipc_export": (C.c_int, [vp, C.c_char_p]),

@@ -202,6 +202,17 @@ class PartGraph:
                                                                                device=c.device)).contiguous())
         return cached[1]
 
+    def pna_scalers(self, delta: float):
+        """PNA's per-row scalers (a, t) = (log(D + 1) / delta, delta / log(D + 1)), fp32 [num_in] each, from the CSR row
+        lengths D (ops.pna_scalers_host).  Computed once per delta, on the host from the integer degrees, and kept at
+        this address: captured CUDA graphs read them."""
+        cached = getattr(self, "_pna_at", None)
+        if cached is None or cached[0] != float(delta):
+            from .ops import pna_scalers_host
+            a, t = pna_scalers_host((self.fwd.indptr[1:] - self.fwd.indptr[:-1]).cpu(), delta)
+            cached = self._pna_at = (float(delta), a.to(self.device), t.to(self.device))
+        return cached[1], cached[2]
+
     def num_nodes(self, ntype: str = "_U") -> int:
         if ntype == "_U":
             return self.num_all

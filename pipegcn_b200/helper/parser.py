@@ -45,6 +45,12 @@ layer, the convolutions and the `--n-linear` (>= 1) trailing linears.  `--gcnii-
 and `--gcnii-lambda l` (l > 0, finite, default 0.5) set alpha and lambda; suppressed like `--sampling-rate`: read them
 with getattr(args, 'gcnii_alpha', 0.1) and getattr(args, 'gcnii_lambda', 0.5).  It cannot be combined with --use-pp,
 --aggregator pool or --sampling-rate < 1.
+
+`--model pna` (not in the reference) trains principal neighbourhood aggregation (Corso et al., NeurIPS 2020; DGL's
+PNAConvTower): every layer reduces the messages M(cat(h_u, h_v)) with mean, max, min and std, scales the result by
+the identity, log(D + 1) / delta and delta / log(D + 1) (D the in-degree, delta the mean of log(D + 1) over the
+training graph, derived at set-up), and maps cat(h_v, the 12 scaled aggregates) through a linear U.  It has no flags
+of its own.  It cannot be combined with --aggregator pool, --use-pp or --sampling-rate < 1.
 """
 import argparse
 
@@ -53,7 +59,7 @@ _FLAGS = [
     ("dataset", dict(type=str, default='reddit', help="the input dataset (or synthetic:<shape>)")),
     ("graph-name", dict(type=str, default='')),
     ("model", dict(type=str, default='graphsage', help="model for training (graphsage | gcn | gat | gatv2 | transformer | "
-                                                              "graphconv | gcnii; gcn is GraphSAGE)")),
+                                                              "graphconv | gcnii | pna; gcn is GraphSAGE)")),
     ("dropout", dict(type=float, default=0.5, help="dropout probability")),
     ("lr", dict(type=float, default=1e-2, help="learning rate")),
     ("n-epochs", dict(type=int, default=200, help="the number of training epochs")),

@@ -72,6 +72,23 @@ h0 = ReLU(fc_in(dropout(x))) is the model's initial representation; graph layer 
 [d, n_feat], default initialisation, drawn first) in front of its convolution and computes it over every [inner | halo]
 row of x.  State-dict keys: `fc_in.weight` / `fc_in.bias` (layer 0 only), `weight1` [d, d] (in x out, DGL's layout),
 `bias` [d].  Initialisation is the GCNII authors': weight1 ~ U(-1/sqrt(d), 1/sqrt(d)), then bias = 0.
+
+`PNALayer` (not in the reference): principal neighbourhood aggregation (Corso et al., "Principal Neighbourhood
+Aggregation for Graph Nets", NeurIPS 2020), DGL's `PNAConvTower` with aggregators mean, max, min, std, scalers
+identity, amplification, attenuation, one tower and no edge features, over the same rows.  With D_v the in-degree of v
+(its CSR row length, self loop included) and delta the mean of log(D + 1) over the training graph:
+
+    m_uv    = M(cat(h[u], h[v])) = zs[u] + zd[v],   zs = h @ W_s^T,  zd = h[:N_in] @ W_d^T + b_M   (M.weight = [W_s | W_d])
+    agg_v   = [mean_u m_uv | max_u m_uv | min_u m_uv | std_u m_uv]                                 (4 d_in)
+    h_neigh = [agg_v | a_v agg_v | t_v agg_v],   a_v = log(D_v + 1) / delta,  t_v = delta / log(D_v + 1)
+    out[v]  = U(cat(h[v], h_neigh))                                                                   (13 d_in -> d_out)
+
+The std is sqrt(max(var, 0) + 1e-30) of the messages; it equals that of zs (the shift zd[v] cancels), so it is computed
+over zs alone (DGL takes relu(E[m^2] - E[m]^2) over the messages).  A row without in-edges gets h_neigh = 0, as DGL does
+not reduce a node without messages.  Left out of DGL's tower: the graph-size norm, the tower's batch norm and dropout
+(the model's loop supplies LayerNorm, ReLU and dropout between layers); there is no mixing layer and no residual.
+State-dict keys: `M.weight` [d_in, 2 d_in], `M.bias`, `U.weight` [d_out, 13 d_in], `U.bias`, both `nn.Linear` with
+the default initialisation, M drawn before U.  delta is not a layer parameter: the model sets it (`PNA.set_delta`).
 """
 import math
 
@@ -273,3 +290,19 @@ class TransformerLayer(nn.Module):
         return ops.transformer_layer(feat, graph, keep, self.num_heads, self.lin_query.weight, self.lin_query.bias,
                                      self.lin_key.weight, self.lin_key.bias, self.lin_value.weight,
                                      self.lin_value.bias, self.lin_skip.weight, self.lin_skip.bias, drop_bwd)
+
+
+class PNALayer(nn.Module):
+
+    def __init__(self, in_feats, out_feats):
+        super().__init__()
+        self.in_feats, self.out_feats = in_feats, out_feats
+        self.M = nn.Linear(2 * in_feats, in_feats)
+        self.U = nn.Linear(13 * in_feats, out_feats)
+        self.delta = None
+
+    def forward(self, graph, feat, arg=None, drop_bwd=None):
+        """As GraphSAGELayer.forward; `arg` is unused (the scalers live on the graph, `PartGraph.pna_scalers`)."""
+        if self.delta is None:
+            raise RuntimeError("PNALayer: delta is not set (PNA.set_delta, set by the trainer or a loaded checkpoint)")
+        return ops.pna_layer(feat, graph, self.delta, self.M.weight, self.M.bias, self.U.weight, self.U.bias, drop_bwd)

@@ -35,13 +35,20 @@ fc_in + ReLU + convolution 1 over the exchanged input features, every later grap
 the trailing `n_linear` (>= 1) linears produce the logits.  Every layer reads h0 = ReLU(fc_in(dropout(x))) through
 the `ops.GCNIIState` of the forward; h0 enters convolution 1 through its own keyed dropout and the residuals clean.
 Between the graph layers the loop applies norm, ReLU and dropout as for every other model; the paper has ReLU only.
+
+`PNA(GraphSAGE)` (not in the reference) is the same layer loop with `PNALayer`s (DGL's PNAConvTower, module/layer.py).
+Its degree scalers need delta, the mean of log(D + 1) over the training graph's nodes: the trainer computes it from the
+merged integer degree histograms of all partitions (`train.RankEngine`) and sets it with `set_delta`.  delta is model
+state: the state dict carries it as the fp64 scalar `pna_delta`, so a loaded checkpoint evaluates with the delta it
+was trained with.  Every graph (partition, whole graph, evaluation layout) computes its own rows' scalers from its row
+degrees and this delta (`PartGraph.pna_scalers`).
 """
 import torch
 from torch import nn
 import torch.nn.functional as F
 
 from ..helper import context as ctx
-from .layer import GATLayer, GATv2Layer, GCNIILayer, GraphConvLayer, GraphSAGELayer, TransformerLayer
+from .layer import GATLayer, GATv2Layer, GCNIILayer, GraphConvLayer, GraphSAGELayer, PNALayer, TransformerLayer
 
 
 class GNNBase(nn.Module):
@@ -345,3 +352,49 @@ class GraphTransformer(GAT):
     def _preload(self):
         from .. import ops
         ops.transformer_preload()
+
+
+class PNA(GraphSAGE):
+
+    def __init__(self, layer_size, activation, dropout=0.5, norm='layer', train_size=None, n_linear=0, buffer=None,
+                 dtype=torch.float32):
+        super().__init__(layer_size, activation, False, dropout=dropout, norm=norm, train_size=train_size,
+                         n_linear=n_linear, buffer=buffer, dtype=dtype)
+        self.register_buffer('pna_delta', torch.tensor(float('nan'), dtype=torch.float64))
+        self.delta = None
+
+    def _graph_layer(self, i, d_in, d_out):
+        return PNALayer(d_in, d_out)
+
+    def _layer_arg(self, in_deg):
+        """PNA layers take no degrees: the scalers live on the graph."""
+        return None
+
+    def set_delta(self, delta: float):
+        """delta of the degree scalers (the mean of log(D + 1) over the training graph), for every graph layer."""
+        self.delta = float(delta)
+        self.pna_delta.fill_(self.delta)
+        for i in range(self.n_graph_layers):
+            self.layers[i].delta = self.delta
+
+    def _load_from_state_dict(self, state_dict, prefix, *args, **kwargs):
+        super()._load_from_state_dict(state_dict, prefix, *args, **kwargs)
+        d = state_dict.get(prefix + 'pna_delta')
+        if d is not None and bool(torch.isfinite(d)):
+            self.set_delta(float(d))
+
+    def _prepare(self, g):
+        """Loads the kernels and the graph's scalers before any halo wait can spin (both may wait for the device)."""
+        from .. import ops
+        ops.pna_preload()
+        if self.delta is None:
+            raise RuntimeError("PNA: delta is not set (train through RankEngine, or load a checkpoint)")
+        g.pna_scalers(self.delta)
+
+    def forward(self, g, feat, in_deg=None):
+        self._prepare(g)
+        return super().forward(g, feat, in_deg)
+
+    def forward_partitioned(self, g, xch, pp_feat=None, push0=False):
+        self._prepare(g)
+        return (yield from super().forward_partitioned(g, xch, pp_feat, push0))

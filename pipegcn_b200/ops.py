@@ -1649,6 +1649,258 @@ def sage_pool_layer(feat, graph, keep, w1, b1, w2, b2, wp, bp, drop_bwd=None) ->
     return SagePoolLayerFn.apply(feat, graph, keep, w1, b1, w2, b2, wp, bp, drop_bwd)
 
 
+# ---- principal neighbourhood aggregation, PNAConv (csrc/pna.cu) --------------------------------------------
+def pna_preload():
+    """Load every PNA kernel now (see gat_preload)."""
+    _C.check(_C.lib.pg_pna_preload(), "pg_pna_preload")
+
+
+def pna_width(d: int) -> int:
+    """Stride of the parts of the concatenated PNA operands ([mu | max | min | std], [g | a g | t g], [g_zs | g_zd]):
+    d rounded up to a multiple of 8, so that every part starts on a 16-byte boundary.  The columns between the parts
+    are zero."""
+    return (int(d) + 7) // 8 * 8
+
+
+def pna_degree_histogram(indptr: torch.Tensor) -> list:
+    """Counts of the row lengths 0, 1, ... of a CSR (a partition's inner rows): the integer input of pna_delta."""
+    deg = (indptr[1:] - indptr[:-1]).to(device="cpu", dtype=torch.int64)
+    return torch.bincount(deg).tolist() if deg.numel() else []
+
+
+def pna_delta(histograms) -> float:
+    """PNA's delta, the mean of log(D + 1) over the nodes, from the degree histograms of all partitions: merged as
+    integers, then sum_k count_k log1p(k) / N in fp64 in ascending k -- the same bits on every rank, for any
+    partitioning of the same graph."""
+    merged = [0] * max((len(h) for h in histograms), default=0)
+    for h in histograms:
+        for k, c in enumerate(h):
+            merged[k] += int(c)
+    n = sum(merged)
+    if n == 0:
+        raise ValueError("PNA: delta of an empty graph")
+    s = 0.0
+    for k, c in enumerate(merged):
+        if c:
+            s += c * math.log1p(k)
+    delta = s / n
+    if not delta > 0:
+        raise ValueError(f"PNA: delta {delta} (every node without in-edges)")
+    return delta
+
+
+def pna_scalers_host(deg: torch.Tensor, delta: float):
+    """(a, t) fp32: the amplification log(D + 1) / delta and attenuation delta / log(D + 1) of rows with D in-edges,
+    computed in fp64 and rounded once (t = 0 for D = 0: such a row aggregates to 0)."""
+    lg = torch.log1p(deg.to(torch.float64))
+    a = lg / float(delta)
+    t = torch.where(deg > 0, float(delta) / torch.where(deg > 0, lg, torch.ones_like(lg)), torch.zeros_like(lg))
+    return a.to(torch.float32), t.to(torch.float32)
+
+
+def pna_aggregate(plan: CsrPlan, zs: torch.Tensor, zd: torch.Tensor, stats: bool = True):
+    """(agg, mu, var, amax, amin) over the forward CSR `plan` (pg_pna_aggregate): agg [n_rows, 4 W] in zs's dtype
+    ([mu + zd | max + zd | min + zd | std], parts W = pna_width(d) apart, zero between), mu / var [n_rows, d] fp32 and
+    the sources of the extremes amax / amin [n_rows, d] int32.  `stats` False: only agg (the others are None)."""
+    _rows(zs), _rows(zd)
+    n, d = plan.n_rows, zs.shape[1]
+    w = pna_width(d)
+    assert zd.dtype == torch.float32 and zd.shape == (n, d)
+    dev = zs.device
+    agg = alloc_rows(n, 4 * w, zs.dtype, dev, zero=w != d)
+    mu = var = amax = amin = None
+    if stats:
+        mv = alloc_rows(n, 2 * w, torch.float32, dev)
+        ar = alloc_rows(n, 2 * w, torch.int32, dev)
+        mu, var, amax, amin = mv[:, :d], mv[:, w:w + d], ar[:, :d], ar[:, w:w + d]
+    scratch = plan.scratch(6 * d)
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_pna_aggregate(C.byref(plan.c), zs.data_ptr(), zs.stride(0), zd.data_ptr(), zd.stride(0), d,
+                                     _C.dtype_code(zs.dtype), agg.data_ptr(), agg.stride(0), w, _ptr(mu), _ptr(var),
+                                     mu.stride(0) if stats else 0, _ptr(amax), _ptr(amin),
+                                     amax.stride(0) if stats else 0, _ptr(scratch), _scratch_ld(6 * d),
+                                     _C.stream_ptr()), "pg_pna_aggregate")
+    return agg, mu, var, amax, amin
+
+
+def pna_combine(y: torch.Tensor, z: torch.Tensor, a: torch.Tensor, t: torch.Tensor, dtype) -> torch.Tensor:
+    """out [n, d_out] = y + a * z[:, :d_out] + t * z[:, d_out:] in fp32, rounded once to `dtype` (pg_pna_combine)."""
+    n, d_out = y.shape
+    out = alloc_rows(n, d_out, dtype, y.device)
+    _C.count()
+    _C.check(_C.lib.pg_pna_combine(y.data_ptr(), y.stride(0), z.data_ptr(), z.stride(0), a.data_ptr(), t.data_ptr(),
+                                   n, d_out, _C.dtype_code(dtype), out.data_ptr(), out.stride(0), _C.stream_ptr()),
+             "pg_pna_combine")
+    return out
+
+
+def pna_grad_scale(g: torch.Tensor, a: torch.Tensor, t: torch.Tensor) -> torch.Tensor:
+    """G3 = [g | a g | t g] in g's dtype, parts pna_width(d_out) apart, zero between (pg_pna_grad_scale)."""
+    _rows(g)
+    n, d_out = g.shape
+    wo = pna_width(d_out)
+    out = alloc_rows(n, 3 * wo, g.dtype, g.device, zero=wo != d_out)
+    _C.count()
+    _C.check(_C.lib.pg_pna_grad_scale(g.data_ptr(), g.stride(0), a.data_ptr(), t.data_ptr(), n, d_out,
+                                      _C.dtype_code(g.dtype), out.data_ptr(), out.stride(0), wo, _C.stream_ptr()),
+             "pg_pna_grad_scale")
+    return out
+
+
+def pna_bwd_dst(indptr: torch.Tensor, gagg: torch.Tensor, mu: torch.Tensor, var: torch.Tensor, gzd: torch.Tensor):
+    """(alpha, beta [n, d] fp32, g_mx, g_mn [n, d] in gzd's dtype) from g_agg [n, 4 W] fp32 (pg_pna_bwd_dst); writes
+    g_zd into `gzd`."""
+    n, d = mu.shape
+    w = pna_width(d)
+    dev = mu.device
+    ab = alloc_rows(n, 2 * w, torch.float32, dev)
+    gm = alloc_rows(n, 2 * w, gzd.dtype, dev)
+    alpha, beta, gmx, gmn = ab[:, :d], ab[:, w:w + d], gm[:, :d], gm[:, w:w + d]
+    _C.count()
+    _C.check(_C.lib.pg_pna_bwd_dst(indptr.data_ptr(), gagg.data_ptr(), gagg.stride(0), w, mu.data_ptr(),
+                                   var.data_ptr(), mu.stride(0), n, d, _C.dtype_code(gzd.dtype), gzd.data_ptr(),
+                                   gzd.stride(0), alpha.data_ptr(), beta.data_ptr(), alpha.stride(0), gmx.data_ptr(),
+                                   gmn.data_ptr(), gmx.stride(0), _C.stream_ptr()), "pg_pna_bwd_dst")
+    return alpha, beta, gmx, gmn
+
+
+def pna_bwd_src(plan_t: CsrPlan, zs, alpha, beta, amax, amin, gmx, gmn, gzs: torch.Tensor) -> torch.Tensor:
+    """g_zs over the CSC `plan_t` into `gzs` [plan_t.n_rows, d] (pg_pna_bwd_src)."""
+    d = zs.shape[1]
+    scratch = plan_t.scratch(2 * d)
+    _C.count(2 if plan_t.n_long else 1)
+    _C.check(_C.lib.pg_pna_bwd_src(C.byref(plan_t.c), zs.data_ptr(), zs.stride(0), alpha.data_ptr(), beta.data_ptr(),
+                                   alpha.stride(0), amax.data_ptr(), amin.data_ptr(), amax.stride(0), gmx.data_ptr(),
+                                   gmn.data_ptr(), gmx.stride(0), d, _C.dtype_code(zs.dtype), gzs.data_ptr(),
+                                   gzs.stride(0), _ptr(scratch), _scratch_ld(2 * d), _C.stream_ptr()),
+             "pg_pna_bwd_src")
+    return gzs
+
+
+def pna_u_operands(w_u: torch.Tensor, d: int, dtype, transposed: bool = False):
+    """U's scaled-aggregate columns [W_1 | W_2 | W_3] ([d_out, 12 d]) as the padded GEMM operands of a PNA layer, each
+    written once from the master weights in the activation dtype, zero in the columns between the parts (pna_width):
+    W_1 [d_out, 4 W] and [W_2; W_3] [2 d_out, 4 W] for the forward, and with `transposed` also the backward's
+    [W_1; W_2; W_3]^T [4 W, 3 Wo] (element (k W + c, s Wo + o) = W_{s+1}[o, k d + c]).  None in place of the last one
+    otherwise."""
+    d_out = w_u.shape[0]
+    w, wo = pna_width(d), pna_width(d_out)
+    pad = w != d
+    src = w_u.detach()[:, d:].view(d_out, 3, 4, d)
+    w1 = alloc_rows(d_out, 4 * w, dtype, w_u.device, zero=pad)
+    w1.view(d_out, 4, w)[:, :, :d].copy_(src[:, 0])
+    w23 = alloc_rows(2 * d_out, 4 * w, dtype, w_u.device, zero=pad)
+    w23.view(2, d_out, 4, w)[:, :, :, :d].copy_(src[:, 1:].permute(1, 0, 2, 3))
+    w123t = None
+    if transposed:
+        w123t = alloc_rows(4 * w, 3 * wo, dtype, w_u.device, zero=pad or wo != d_out)
+        w123t.view(4, w, 3, wo)[:, :d, :, :d_out].copy_(src.permute(2, 3, 1, 0))
+    return w1, w23, w123t
+
+
+def _col_split(sp, lo: int, hi: int):
+    """Columns [lo, hi) of an fp32 `Split` (or of a plain tensor)."""
+    if not isinstance(sp, Split):
+        return sp[:, lo:hi]
+    out = Split.__new__(Split)
+    out.x, out.hi, out.lo = sp.x[:, lo:hi], sp.hi[:, lo:hi], sp.lo[:, lo:hi]
+    return out
+
+
+class PnaLayerFn(torch.autograd.Function):
+    """One PNA layer (DGL PNAConvTower: aggregators mean, max, min, std; scalers identity, amplification,
+    attenuation; one tower, no edge features) over the [inner | halo] rows `feat` of a partition, returning the inner
+    rows.  With M.weight = [W_s | W_d], U.weight = [W_x | W_1 | W_2 | W_3], W = pna_width(d):
+
+        zs  = feat @ W_s^T                                  [num_all, d]    pg_linear over all rows
+        zd  = feat[:N_in] @ W_d^T + b_M                     [N_in, d] fp32  pg_linear over the inner rows
+        agg = [mu + zd | max + zd | min + zd | std]         [N_in, 4W]      pg_pna_aggregate (+ mu, var, A+, A-)
+        y   = feat[:N_in] @ W_x^T + agg @ W_1^T + b_U       [N_in, d_out]   fp32, one two-source pg_linear
+        z   = agg @ [W_2; W_3]^T                            [N_in, 2 d_out] fp32, pg_linear
+        out = y + a * z[:, :d_out] + t * z[:, d_out:]                       pg_pna_combine
+
+    The per-row scalers a, t are applied to d_out-wide outputs, so the 12d-wide scaled aggregate is never formed.
+    Backward: G3 = [g | a g | t g] (pg_pna_grad_scale), g_agg = G3 @ [W_1; W_2; W_3] (fp32, pg_linear), g_zd, alpha,
+    beta, g_mx, g_mn (pg_pna_bwd_dst), g_zs (pg_pna_bwd_src over the CSC), written side by side as [g_zs | g_zd];
+    g_feat = g @ W_x + [g_zs | g_zd] @ [W_s; W_d] on the inner rows and g_zs @ W_s on the halo rows with the dropout
+    backward of `drop_bwd` in their epilogues; dW_x = g^T feat[:N_in], [dW_1; dW_2; dW_3] = G3^T agg,
+    dW_s = g_zs^T feat, dW_d = g_zd^T feat[:N_in] (pg_wgrad), db_U = colsum(g), db_M = colsum(g_zd)."""
+
+    @staticmethod
+    def forward(ctx, feat, graph, delta, w_m, b_m, w_u, b_u, drop_bwd=None):
+        ctx.drop_bwd = drop_bwd
+        if feat.stride(1) != 1:
+            feat = feat.contiguous()
+        n_in, d = graph.num_in, feat.shape[1]
+        sa, st = graph.pna_scalers(delta)
+        fsp = presplit(feat)                   # fp32: one split of feat for every product
+        finner = fsp.rows(0, n_in) if isinstance(fsp, Split) else feat[:n_in]
+        zs = gemm_nt(fsp, padded_weight(w_m[:, :d], feat.dtype))
+        zd = gemm_nt(finner, padded_weight(w_m[:, d:], feat.dtype), bias=b_m, out_dtype=torch.float32)
+        keep = any(ctx.needs_input_grad)
+        agg, mu, var, amax, amin = pna_aggregate(graph.fwd, zs, zd, stats=keep)
+        del zd
+        w1, w23, w123t = pna_u_operands(w_u, d, feat.dtype, transposed=keep)
+        aggsp = presplit(agg)
+        y = gemm_nt(finner, padded_weight(w_u[:, :d], feat.dtype), aggsp, w1, bias=b_u, out_dtype=torch.float32)
+        z = gemm_nt(aggsp, w23, out_dtype=torch.float32)
+        out = pna_combine(y, z, sa, st, feat.dtype)
+        if keep:
+            ctx.save_for_backward(feat, zs, agg, mu, var, amax, amin, w_m, w_u)
+            ctx.graph, ctx.sa, ctx.st, ctx.has_bias = graph, sa, st, (b_m is not None, b_u is not None)
+            ctx.w123t = w123t                  # the step's weights: the backward uses the forward's operand
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        feat, zs, agg, mu, var, amax, amin, w_m, w_u = ctx.saved_tensors
+        graph = ctx.graph
+        n_in, n_all, d, d_out = graph.num_in, feat.shape[0], feat.shape[1], w_u.shape[0]
+        w, wo = pna_width(d), pna_width(d_out)
+        dt = feat.dtype
+        colsum = _take_colsum(g)
+        g = _tma_ready(g if g.dtype == dt else g.to(dt))
+        g3 = pna_grad_scale(g, ctx.sa, ctx.st)
+        g3sp = presplit(g3)
+        gagg = gemm_nt(g3sp, ctx.w123t, out_dtype=torch.float32)
+        ctx.w123t = None
+        pz = alloc_rows(n_all, 2 * w, dt, feat.device, zero=w != d)      # [g_zs | g_zd]
+        gzd = pz[:n_in, w:w + d]
+        alpha, beta, gmx, gmn = pna_bwd_dst(graph.fwd.indptr, gagg, mu, var, gzd)
+        del gagg
+        pna_bwd_src(graph.bwd, zs, alpha, beta, amax, amin, gmx, gmn, pz[:, :d])
+        del alpha, beta, gmx, gmn
+        gsp, pzsp = presplit(g), presplit(pz)
+        is_split = isinstance(pzsp, Split)
+        g_feat = None
+        if ctx.needs_input_grad[0]:
+            g_feat = alloc_rows(n_all, d, dt, feat.device)
+            drop = ctx.drop_bwd if ctx.drop_bwd is not None and ctx.drop_bwd.p > 0 else None
+            db = drop if drop is not None and d <= 256 and _drop_ok(g_feat) else None
+            gemm_nt(gsp, padded_weight(w_u[:, :d], dt, transpose=True), pzsp.rows(0, n_in) if is_split else pz[:n_in],
+                    _pair_weight(w_m[:, :d], w_m[:, d:], w, dt, transpose=True), out=g_feat[:n_in], drop=db)
+            if n_all > n_in:
+                gemm_nt(_col_split(pzsp.rows(n_in) if is_split else pz[n_in:], 0, d),
+                        padded_weight(w_m[:, :d], dt, transpose=True), out=g_feat[n_in:], drop=db, drop_row0=n_in)
+            if drop is not None and db is None:
+                dropout_rows(g_feat, drop, out=g_feat)
+        fsp = presplit(feat)
+        finner = fsp.rows(0, n_in) if isinstance(fsp, Split) else feat[:n_in]
+        gws = wgrad(_col_split(pzsp, 0, d), fsp)
+        gwd = wgrad(_col_split(pzsp.rows(0, n_in) if is_split else pz[:n_in], w, w + d), finner)
+        gwx = wgrad(gsp, finner)
+        gr = wgrad(g3sp, presplit(agg)).view(3, wo, 4, w)[:, :d_out, :, :d]
+        gw_u = torch.cat([gwx, gr.permute(1, 0, 2, 3).reshape(d_out, 12 * d)], 1)
+        gw_m = torch.cat([gws, gwd], 1)
+        gbm = gat_colsum(gzd) if ctx.has_bias[0] else None
+        gbu = (colsum if colsum is not None else g.float().sum(0)) if ctx.has_bias[1] else None
+        return g_feat, None, None, gw_m.to(w_m.dtype), gbm, gw_u.to(w_u.dtype), gbu, None
+
+
+def pna_layer(feat, graph, delta, w_m, b_m, w_u, b_u, drop_bwd=None) -> torch.Tensor:
+    return PnaLayerFn.apply(feat, graph, float(delta), w_m, b_m, w_u, b_u, drop_bwd)
+
+
 # ---- row-wise epilogues (csrc/rowops.cu) -------------------------------------------------------------------
 # column sums of a gradient tensor computed as a by-product by the kernel that produced it, keyed by the
 # tensor's address: the bias gradient of the linear upstream (saves a full pass over [N, d])

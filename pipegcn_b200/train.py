@@ -32,7 +32,7 @@ from .helper import context as ctx
 from .helper.feature_buffer import Buffer, EvalExchange, OneShotExchange, check_halo_bits, check_sampling
 from .helper.reducer import Reducer
 from .helper.timer.comm_timer import CommTimer
-from .module.model import GAT, GATv2, GCNII, GraphConv, GraphSAGE, GraphTransformer
+from .module.model import GAT, GATv2, GCNII, PNA, GraphConv, GraphSAGE, GraphTransformer
 from .partition import PartitionLayout, get_layer_size
 
 
@@ -54,7 +54,9 @@ def check_model(args):
     --sampling-rate < 1 (the symmetric norm of a sampled graph needs every source's sampled out-degree, which
     depends on every peer's sample).  --model gcnii refuses the same two, --n-linear 0 (its last convolution is
     square: the logits come from a linear) and --use-pp (graph layer 0 begins with fc_in, so a precomputed neighbour
-    aggregate of x has no place)."""
+    aggregate of x has no place).  --model pna refuses --aggregator pool (it has its own aggregators), --use-pp (the
+    precompute is a neighbour mean) and --sampling-rate < 1 (sampling changes the degrees, the scalers and the sources
+    the extremes range over)."""
     attention = args.model in ('gat', 'gatv2', 'transformer')
     aggregator = getattr(args, 'aggregator', 'mean')
     if aggregator not in ('mean', 'pool'):
@@ -73,6 +75,15 @@ def check_model(args):
         if getattr(args, 'sampling_rate', 1.0) < 1.0:
             raise NotImplementedError("--model gcnii with --sampling-rate < 1: the symmetric norm of the sampled "
                                       "graph needs every source's sampled out-degree")
+        return
+    if args.model == 'pna':
+        if aggregator == 'pool':
+            raise ValueError("--aggregator pool is a GraphSAGE aggregator; --model pna has its own")
+        if args.use_pp:
+            raise NotImplementedError("--model pna with --use-pp: the precompute is a neighbour mean")
+        if getattr(args, 'sampling_rate', 1.0) < 1.0:
+            raise NotImplementedError("--model pna with --sampling-rate < 1: sampling changes the degrees, the scalers "
+                                      "and the sources the extremes range over")
         return
     if args.model == 'graphconv':
         if aggregator == 'pool':
@@ -110,6 +121,9 @@ def create_model(layer_size, args, buffer=None, dtype=torch.float32):
         return GCNII(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
                      train_size=args.n_train, buffer=buffer, dtype=dtype, alpha=getattr(args, 'gcnii_alpha', 0.1),
                      lam=getattr(args, 'gcnii_lambda', 0.5))
+    if args.model == 'pna':
+        return PNA(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
+                   train_size=args.n_train, buffer=buffer, dtype=dtype)
     if args.model in ('gat', 'gatv2', 'transformer'):
         cls = {'gat': GAT, 'gatv2': GATv2, 'transformer': GraphTransformer}[args.model]
         return cls(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
@@ -203,6 +217,8 @@ class RankEngine:
         if init_state is not None:
             self.model.load_state_dict(init_state)
         self.model.to(dev)
+        if getattr(self, 'pna_delta', None) is not None:           # the set-up has already derived it
+            self.model.set_delta(self.pna_delta)
         self.reducer = reducer if reducer is not None else Reducer(world)
         self.reducer.init(self.model, world)
         for name, p in self.model.named_parameters():
@@ -229,9 +245,12 @@ class RankEngine:
         return getattr(self.world, 'is_local', False) and self.world.size > 1
 
     def _setup_steps(self, layout):
-        """Collective set-up (generator): --model graphconv and gcnii first exchange the halo rows' degrees; then the --use-pp
+        """Collective set-up (generator): --model pna first derives delta from every rank's degree histogram,
+        --model graphconv and gcnii first exchange the halo rows' degrees; then the --use-pp
         precompute (train.py:169-189), cat(feat, neighbour mean) over the raw features' halo rows, or else the
         one-shot exchange of the static layer-0 halo rows (SURVEY.md §8f-2)."""
+        if self.args.model == 'pna':
+            yield from self._pna_delta_steps(layout)
         sym = self.args.model in ('graphconv', 'gcnii')
         if sym:
             yield from _sym_norm_steps(self.world, layout, self.graph, 'pipegcn.buffer.norm', self.buffer.timeout_ms)
@@ -246,6 +265,18 @@ class RankEngine:
         self.buffer.load_inner(0, self.feat)
         yield 'publish'
         yield from self._static0_steps()
+
+    def _pna_delta_steps(self, layout):
+        """--model pna (generator): delta, the mean of log(D + 1) over the training graph's nodes, from the integer
+        histograms of every rank's inner-row degrees (`ops.pna_delta`): the same bits on every rank and for every
+        partitioning.  Sets it on the model (once that exists) and computes this partition's scalers."""
+        from . import ops
+        self.world.publish('pipegcn.pna.degrees', ops.pna_degree_histogram(layout.indptr))
+        yield 'publish'
+        self.pna_delta = ops.pna_delta(self.world.collect('pipegcn.pna.degrees'))
+        self.graph.pna_scalers(self.pna_delta)
+        if getattr(self, 'model', None) is not None:
+            self.model.set_delta(self.pna_delta)
 
     def _static0_steps(self):
         self.buffer.static0_begin(self.buffer.input_rows())
