@@ -597,6 +597,55 @@ int pg_pna_bwd_src(const pg_csr* gt, const void* zs, int64_t ldz, const float* a
                    void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Softmax-aggregation graph convolution (DeeperGCN; PyG GENConv, aggr='softmax', one scalar temperature t) over the
+ * `_U` rows [inner | halo] of one partition.  xs [num_all, d] (fp32 or bf16, `dtype`) is x_src = h W_src^T (or h),
+ * xd [N_in, d] (dtype) x_dst.  For the in-edges u -> v of the forward CSR g whose source is kept, per column c:
+ *   m_u = ReLU(xs[u]) + 1e-7,  s_u = t m_u   (fp32, one rounding each; a NaN x stays NaN)
+ *   M = max_u s_u,  W = sum_u exp(s_u - M),  A = sum_u exp(s_u - M) m_u,  B = sum_u exp(s_u - M) m_u^2
+ *   agg = A / W,  L = M + log W,  var = max(B / W - agg^2, 0),  S = agg + xd   (S rounded once to dtype)
+ * The state is updated online, one expf per edge and element (exp(-|s - M|) weighs the new edge or rescales the old
+ * state), in CSR order; long rows come as segments whose states a fix-up merges in segment order.  No atomics: the
+ * results are the same bits from run to run.  A row without a kept in-edge gets agg = 0, L = -inf, var = 0 and S = xd;
+ * a NaN source makes its destinations' agg, L, var and S NaN.  t is read from device memory (a captured CUDA graph
+ * sees every update of it).  keep (uint8 [num_all - num_in], or NULL: every source kept) is the keep mask of the halo
+ * rows: a source u >= num_in with keep[u - num_in] == 0 is skipped.  Rows start on 16-byte boundaries with strides that
+ * are multiples of 16 bytes, covering the last 16-byte vector of a row; only columns [0, d) are written.  The plans
+ * must carry the chunk table; scratch is fp32 [n_seg][ld_scratch] (may be NULL when n_seg == 0).
+ * ---------------------------------------------------------------------------------------- */
+/* fp64 block partials of pg_genconv_bwd_dst's dt: the `partial` workspace holds this many doubles */
+#define PG_GENCONV_DT_PARTIALS 264
+/* loads every GENConv kernel (call it before any halo wait can spin: a first launch may wait for the device) */
+int pg_genconv_preload(void);
+/* S [N_in, d] (dtype) over the forward CSR g; with agg != NULL also agg and L (fp32 [N_in, d], the backward's
+ * operands), with var != NULL (needs agg) also var (fp32 [N_in, d], the temperature's gradient).  ld_scratch >= 3 d,
+ * or 4 d with var */
+int pg_genconv_aggregate(const pg_csr* g, const void* xs, int64_t ldxs, const void* xd, int64_t ldxd, int32_t d,
+                         int dtype, const float* t, const uint8_t* keep, int32_t num_in, void* s, int64_t lds,
+                         float* agg, int64_t ldagg, float* lse, int64_t ldlse, float* var, int64_t ldvar,
+                         float* scratch, int64_t ld_scratch, void* stream);
+/* per destination element, from g_S (fp32 [n_rows, d], the gradient of S) and agg:
+ *   Q = fl(t fl(g_S agg))  (fp32);  gst = g_S rounded to dtype (may be NULL: not written)
+ * and with var != NULL:  dt = sum_{v, c} g_S var  (fp64 products and sums: each of at most PG_GENCONV_DT_PARTIALS
+ * CTAs sums its elements in grid-stride order and a fixed tree, then one CTA sums the partials in a fixed order and
+ * rounds once to fp32 into the device scalar *dt).  The grid depends on n_rows * d only: the same bits from run to run.
+ * var and dt are NULL together */
+int pg_genconv_bwd_dst(const float* gs, int64_t ldg, const float* agg, int64_t ldagg, const float* var, int64_t ldvar,
+                       const float* t, int32_t n_rows, int32_t d, int dtype, float* q, int64_t ldq, void* gst,
+                       int64_t ldgst, double* partial, float* dt, void* stream);
+/* dx[u] over the CSC row u of gt (rows = all num_all `_U` rows), per column:
+ *   acc = sum_v exp(fl(t m_u) - L_v) (G_v (1 + t m_u) - Q_v)   (G = g_S; fp32, one multiply-add per term, CSC order;
+ *                                                              long rows: segment sums added in segment order)
+ *   dx  = dropout([xs[u] > 0] ? acc : 0  (+ add[u] for u < n_add))   rounded once to dtype
+ * with m_u recomputed from xs.  A row without out-edges, and an unkept halo row, get acc = 0 (so 0, or add[u]).
+ * add (fp32 [n_add, d], may be NULL when n_add == 0) lets the inner rows take g_S when x_src is h itself; drop (may be
+ * NULL) is the dropout key of the layer input, applied as pg_dropout_rows does (row u, 16-byte vectors).
+ * ld_scratch >= d */
+int pg_genconv_bwd_src(const pg_csr* gt, const void* xs, int64_t ldxs, const float* t, const uint8_t* keep,
+                       int32_t num_in, const float* lse, int64_t ldlse, const float* gs, int64_t ldg, const float* q,
+                       int64_t ldq, const float* add, int64_t ldadd, int32_t n_add, const pg_drop* drop, int32_t d,
+                       int dtype, void* dx, int64_t lddx, float* scratch, int64_t ld_scratch, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Symmetric heap: device memory that peers map through CUDA IPC (host pointers out).
  * ---------------------------------------------------------------------------------------- */
 #define PG_IPC_HANDLE_BYTES 64

@@ -1,5 +1,6 @@
-// The chunk walk shared by the neighbour-extreme kernels (pool.cu, pna.cu): one warp owns one chunk of a pg_csr plan
-// (include/pipegcn_b200.h: pg_csr::chunks) and visits its rows, or its one long-row segment, through walk_chunk.
+// The chunk walk shared by the plan-walking kernels (pool.cu, pna.cu, genconv.cu): one warp owns one chunk of a
+// pg_csr plan (include/pipegcn_b200.h: pg_csr::chunks) and visits its rows, or its one long-row segment, through
+// walk_chunk.
 #pragma once
 #include "common.cuh"
 
@@ -54,6 +55,42 @@ template <typename T> struct Vec {
 template <typename T> __device__ __forceinline__ T to_t(float x);
 template <> __device__ __forceinline__ float to_t<float>(float x) { return x; }
 template <> __device__ __forceinline__ __nv_bfloat16 to_t<__nv_bfloat16>(float x) { return __float2bfloat16_rn(x); }
+
+// V consecutive fp32 values at p (16-byte aligned when all V are valid and V is a multiple of 4): the side outputs and
+// operands of pna.cu and genconv.cu
+template <int V>
+__device__ __forceinline__ void st_f32(float* p, const float (&f)[V], int valid) {
+  if (valid >= V && V % 4 == 0) {
+#pragma unroll
+    for (int k = 0; k < V; k += 4) *reinterpret_cast<float4*>(p + k) = make_float4(f[k], f[k + 1], f[k + 2], f[k + 3]);
+  } else {
+#pragma unroll
+    for (int k = 0; k < V; ++k) if (k < valid) p[k] = f[k];
+  }
+}
+template <int V>
+__device__ __forceinline__ void ld_f32(const float* p, float (&f)[V], int valid) {
+  if (valid >= V && V % 4 == 0) {
+#pragma unroll
+    for (int k = 0; k < V; k += 4) {
+      const float4 x = __ldg(reinterpret_cast<const float4*>(p + k));
+      f[k] = x.x; f[k + 1] = x.y; f[k + 2] = x.z; f[k + 3] = x.w;
+    }
+  } else {
+#pragma unroll
+    for (int k = 0; k < V; ++k) f[k] = k < valid ? __ldg(p + k) : 0.f;
+  }
+}
+// one 16-byte vector of T from V floats (one rounding each), or its first `valid` elements
+template <typename T, int V>
+__device__ __forceinline__ void st_t(T* p, const float (&f)[V], int valid) {
+  if (valid >= V) {
+    st_vec<16>(p, Pack<T, 16>::pack(f));
+  } else {
+#pragma unroll
+    for (int k = 0; k < V; ++k) if (k < valid) p[k] = to_t<T>(f[k]);
+  }
+}
 
 int check_plan(const pg_csr* g, const char* who) {
   PG_REQUIRE(g != nullptr, "%s: null plan", who);

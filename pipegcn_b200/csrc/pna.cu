@@ -25,17 +25,7 @@ __device__ __forceinline__ void take_min(float& m, int32_t& a, float x, int32_t 
   if (a < 0 || x < m || (x != x && m == m)) { m = x; a = u; }
 }
 
-// V consecutive fp32 / int32 values at p (16-byte aligned when all V are valid and V is a multiple of 4)
-template <int V>
-__device__ __forceinline__ void st_f32(float* p, const float (&f)[V], int valid) {
-  if (valid >= V && V % 4 == 0) {
-#pragma unroll
-    for (int k = 0; k < V; k += 4) *reinterpret_cast<float4*>(p + k) = make_float4(f[k], f[k + 1], f[k + 2], f[k + 3]);
-  } else {
-#pragma unroll
-    for (int k = 0; k < V; ++k) if (k < valid) p[k] = f[k];
-  }
-}
+// V consecutive int32 values at p (16-byte aligned when all V are valid and V is a multiple of 4)
 template <int V>
 __device__ __forceinline__ void st_i32(int32_t* p, const int32_t (&f)[V], int valid) {
   if (valid >= V && V % 4 == 0) {
@@ -46,29 +36,6 @@ __device__ __forceinline__ void st_i32(int32_t* p, const int32_t (&f)[V], int va
     for (int k = 0; k < V; ++k) if (k < valid) p[k] = f[k];
   }
 }
-template <int V>
-__device__ __forceinline__ void ld_f32(const float* p, float (&f)[V], int valid) {
-  if (valid >= V && V % 4 == 0) {
-#pragma unroll
-    for (int k = 0; k < V; k += 4) {
-      const float4 x = __ldg(reinterpret_cast<const float4*>(p + k));
-      f[k] = x.x; f[k + 1] = x.y; f[k + 2] = x.z; f[k + 3] = x.w;
-    }
-  } else {
-#pragma unroll
-    for (int k = 0; k < V; ++k) f[k] = k < valid ? __ldg(p + k) : 0.f;
-  }
-}
-template <typename T, int V>
-__device__ __forceinline__ void st_t(T* p, const float (&f)[V], int valid) {
-  if (valid >= V) {
-    st_vec<16>(p, Pack<T, 16>::pack(f));
-  } else {
-#pragma unroll
-    for (int k = 0; k < V; ++k) if (k < valid) p[k] = to_t<T>(f[k]);
-  }
-}
-
 // std of a row from its variance: sqrt(max(var, 0) + 1e-30), a NaN variance kept
 __device__ __forceinline__ float pna_sigma(float var) { return sqrtf(__fadd_rn(var < 0.f ? 0.f : var, 1e-30f)); }
 

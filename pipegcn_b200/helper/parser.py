@@ -51,6 +51,14 @@ PNAConvTower): every layer reduces the messages M(cat(h_u, h_v)) with mean, max,
 the identity, log(D + 1) / delta and delta / log(D + 1) (D the in-degree, delta the mean of log(D + 1) over the
 training graph, derived at set-up), and maps cat(h_v, the 12 scaled aggregates) through a linear U.  It has no flags
 of its own.  It cannot be combined with --aggregator pool, --use-pp or --sampling-rate < 1.
+
+`--model genconv` (not in the reference) trains the softmax-aggregation graph convolution of DeeperGCN (Li et al., 2020;
+PyG's GENConv with aggr='softmax'): every layer aggregates m_u = ReLU(x_src[u]) + 1e-7 with a per-channel softmax of
+t m_u over the in-edges, adds x_dst and maps the sum through a two-layer MLP [d, 2d, d].  `--genconv-t T` (a finite
+float, default 1.0; 0 and negative values are allowed) sets the temperature, and `--genconv-learn-t` makes it a learnt
+parameter (`aggr_module.t` of every graph layer).  Both are suppressed like `--sampling-rate`: read them with
+getattr(args, 'genconv_t', 1.0) and getattr(args, 'genconv_learn_t', False).  It works with boundary-node sampling
+and cannot be combined with --use-pp or --aggregator pool.
 """
 import argparse
 
@@ -59,7 +67,7 @@ _FLAGS = [
     ("dataset", dict(type=str, default='reddit', help="the input dataset (or synthetic:<shape>)")),
     ("graph-name", dict(type=str, default='')),
     ("model", dict(type=str, default='graphsage', help="model for training (graphsage | gcn | gat | gatv2 | transformer | "
-                                                              "graphconv | gcnii | pna; gcn is GraphSAGE)")),
+                                                              "graphconv | gcnii | pna | genconv; gcn is GraphSAGE)")),
     ("dropout", dict(type=float, default=0.5, help="dropout probability")),
     ("lr", dict(type=float, default=1e-2, help="learning rate")),
     ("n-epochs", dict(type=int, default=200, help="the number of training epochs")),
@@ -133,6 +141,16 @@ def _gcnii_lambda(text):
     return lam
 
 
+def _genconv_t(text):
+    try:
+        t = float(text)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"invalid GENConv temperature '{text}'")
+    if not abs(t) < float('inf'):     # also refuses nan
+        raise argparse.ArgumentTypeError(f"--genconv-t {text}: expected a finite temperature")
+    return t
+
+
 def build_parser():
     parser = argparse.ArgumentParser(description='PipeGCN on H100')
     for flag, kw in _FLAGS:
@@ -164,6 +182,10 @@ def build_parser():
                         help="--model gcnii: weight of the initial residual (0 <= alpha <= 1, default 0.1)")
     parser.add_argument('--gcnii-lambda', '--gcnii_lambda', type=_gcnii_lambda, default=argparse.SUPPRESS,
                         help="--model gcnii: beta_l = ln(lambda / l + 1) (lambda > 0, default 0.5)")
+    parser.add_argument('--genconv-t', '--genconv_t', type=_genconv_t, default=argparse.SUPPRESS,
+                        help="--model genconv: softmax temperature t (finite, default 1.0)")
+    parser.add_argument('--genconv-learn-t', '--genconv_learn_t', action='store_true', default=argparse.SUPPRESS,
+                        help="--model genconv: learn t (one scalar per graph layer, initialised to --genconv-t)")
     return parser
 
 

@@ -89,6 +89,22 @@ not reduce a node without messages.  Left out of DGL's tower: the graph-size nor
 (the model's loop supplies LayerNorm, ReLU and dropout between layers); there is no mixing layer and no residual.
 State-dict keys: `M.weight` [d_in, 2 d_in], `M.bias`, `U.weight` [d_out, 13 d_in], `U.bias`, both `nn.Linear` with
 the default initialisation, M drawn before U.  delta is not a layer parameter: the model sets it (`PNA.set_delta`).
+
+`GENConvLayer` (not in the reference): the softmax-aggregation graph convolution of DeeperGCN (Li et al., "DeeperGCN:
+All You Need to Train Deeper GCNs", 2020), PyG's `GENConv(d_in, d, aggr='softmax', t=T, learn_t=L, norm=None,
+num_layers=2, expansion=2, eps=1e-7, bias=False)` without edge features or message norm, over the same rows:
+
+    x_src = h @ W_src^T  (h itself when d_in == d),   x_dst = h[:N_in] @ W_dst^T  (h[:N_in] when d_in == d)
+    m_u   = ReLU(x_src[u]) + 1e-7
+    agg_v = sum_{u -> v} softmax_u(t m_u) * m_u       (per channel; 0 for a row without in-edges)
+    out   = ReLU((agg + x_dst) @ W1^T) @ W2^T         (W1 [2d, d], W2 [d, 2d]: PyG's MLP with norm=None)
+
+With boundary-node sampling the sums cover the inner and the kept halo sources only.  t is a scalar: with `learn_t`
+a `Parameter` of shape [1] initialised to T (key `aggr_module.t`), else a constant outside the state dict, as in PyG.
+State-dict keys: `lin_src.weight` and `lin_dst.weight` [d, d_in] (only when d_in != d), `mlp.lins.0.weight`
+[2d, d], `mlp.lins.1.weight` [d, 2d] and `aggr_module.t`.  Every weight is drawn as `nn.Linear` draws it
+(kaiming_uniform_(a=sqrt(5))), in the order lin_src, lin_dst, mlp.lins.0, mlp.lins.1.  PyG draws some of them twice
+(at construction and in reset_parameters), so equal seeds do not give PyG's initial weights.
 """
 import math
 
@@ -306,3 +322,50 @@ class PNALayer(nn.Module):
         if self.delta is None:
             raise RuntimeError("PNALayer: delta is not set (PNA.set_delta, set by the trainer or a loaded checkpoint)")
         return ops.pna_layer(feat, graph, self.delta, self.M.weight, self.M.bias, self.U.weight, self.U.bias, drop_bwd)
+
+
+class _GenConvMLP(nn.Module):
+    """PyG's MLP([d, 2d, d], norm=None, bias=False) as a container of its two linears (keys `lins.0`, `lins.1`)."""
+
+    def __init__(self, d):
+        super().__init__()
+        self.lins = nn.ModuleList([nn.Linear(d, 2 * d, bias=False), nn.Linear(2 * d, d, bias=False)])
+
+
+class _SoftmaxAggr(nn.Module):
+    """PyG's SoftmaxAggregation(learn=True, channels=1): the learnable temperature `t` [1]."""
+
+    def __init__(self, t):
+        super().__init__()
+        self.t = nn.Parameter(torch.tensor([float(t)], dtype=torch.float32))
+
+
+class GENConvLayer(nn.Module):
+
+    def __init__(self, in_feats, out_feats, t=1.0, learn_t=False):
+        super().__init__()
+        if not math.isfinite(float(t)):
+            raise ValueError(f"GENConv: temperature {t} is not finite")
+        self.in_feats, self.out_feats, self.learn_t = in_feats, out_feats, bool(learn_t)
+        if in_feats != out_feats:
+            self.lin_src = nn.Linear(in_feats, out_feats, bias=False)
+            self.lin_dst = nn.Linear(in_feats, out_feats, bias=False)
+        else:
+            self.lin_src = self.lin_dst = None
+        self.mlp = _GenConvMLP(out_feats)
+        if self.learn_t:
+            self.aggr_module = _SoftmaxAggr(t)
+        else:
+            # a constant the kernels read from device memory; not part of the state dict
+            self.register_buffer('t_const', torch.tensor([float(t)], dtype=torch.float32), persistent=False)
+
+    def temperature(self) -> torch.Tensor:
+        return self.aggr_module.t if self.learn_t else self.t_const
+
+    def forward(self, graph, feat, keep=None, drop_bwd=None):
+        """As GATLayer.forward: `feat` [num_all, d_in] rows of `graph`, `keep` the keep mask of the halo rows
+        (boundary-node sampling, uint8) or None; returns the [N_in, d] inner rows."""
+        return ops.genconv_layer(feat, graph, keep, self.temperature(),
+                                 self.lin_src.weight if self.lin_src is not None else None,
+                                 self.lin_dst.weight if self.lin_dst is not None else None,
+                                 self.mlp.lins[0].weight, self.mlp.lins[1].weight, drop_bwd)

@@ -42,13 +42,20 @@ merged integer degree histograms of all partitions (`train.RankEngine`) and sets
 state: the state dict carries it as the fp64 scalar `pna_delta`, so a loaded checkpoint evaluates with the delta it
 was trained with.  Every graph (partition, whole graph, evaluation layout) computes its own rows' scalers from its row
 degrees and this delta (`PartGraph.pna_scalers`).
+
+`GENConv(GraphSAGE)` (not in the reference) is the same layer loop with `GENConvLayer`s (PyG's GENConv with the softmax
+aggregator, module/layer.py); a last graph layer that produces the logits is a GENConvLayer(d_in, n_class).  Like
+`GAT`, with boundary-node sampling its layers take the buffer's keep mask of the halo rows, and unkept rows are absent
+from every softmax.  The temperature `t` (constant, or learnt with `learn_t`) is read by the kernels from device
+memory, so a captured CUDA graph sees the optimizer's updates of it.
 """
 import torch
 from torch import nn
 import torch.nn.functional as F
 
 from ..helper import context as ctx
-from .layer import GATLayer, GATv2Layer, GCNIILayer, GraphConvLayer, GraphSAGELayer, PNALayer, TransformerLayer
+from .layer import (GATLayer, GATv2Layer, GCNIILayer, GENConvLayer, GraphConvLayer, GraphSAGELayer, PNALayer,
+                    TransformerLayer)
 
 
 class GNNBase(nn.Module):
@@ -397,4 +404,33 @@ class PNA(GraphSAGE):
 
     def forward_partitioned(self, g, xch, pp_feat=None, push0=False):
         self._prepare(g)
+        return (yield from super().forward_partitioned(g, xch, pp_feat, push0))
+
+
+class GENConv(GraphSAGE):
+
+    def __init__(self, layer_size, activation, dropout=0.5, norm='layer', train_size=None, n_linear=0, buffer=None,
+                 dtype=torch.float32, t=1.0, learn_t=False):
+        self.t, self.learn_t = float(t), bool(learn_t)
+        super().__init__(layer_size, activation, False, dropout=dropout, norm=norm, train_size=train_size,
+                         n_linear=n_linear, buffer=buffer, dtype=dtype)
+
+    def _graph_layer(self, i, d_in, d_out):
+        return GENConvLayer(d_in, d_out, t=self.t, learn_t=self.learn_t)
+
+    def _layer_arg(self, in_deg):
+        """The keep mask of this epoch's boundary-node sample (training with sampling), else None."""
+        buf = self._buffer() if self.training else None
+        return getattr(buf, 'keep_mask', None) if buf is not None else None
+
+    def _preload(self):
+        from .. import ops
+        ops.genconv_preload()
+
+    def forward(self, g, feat, in_deg=None):
+        self._preload()
+        return super().forward(g, feat, in_deg)
+
+    def forward_partitioned(self, g, xch, pp_feat=None, push0=False):
+        self._preload()
         return (yield from super().forward_partitioned(g, xch, pp_feat, push0))

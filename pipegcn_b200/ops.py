@@ -1901,6 +1901,175 @@ def pna_layer(feat, graph, delta, w_m, b_m, w_u, b_u, drop_bwd=None) -> torch.Te
     return PnaLayerFn.apply(feat, graph, float(delta), w_m, b_m, w_u, b_u, drop_bwd)
 
 
+# ---- softmax-aggregation graph convolution, GENConv (csrc/genconv.cu) ---------------------------------------
+GENCONV_DT_PARTIALS = 264          # PG_GENCONV_DT_PARTIALS of include/pipegcn_b200.h
+
+
+def genconv_preload():
+    """Load every GENConv kernel now (see gat_preload)."""
+    _C.check(_C.lib.pg_genconv_preload(), "pg_genconv_preload")
+
+
+def genconv_aggregate(plan: CsrPlan, xs: torch.Tensor, xd: torch.Tensor, t: torch.Tensor, keep=None, num_in: int = 0,
+                      stats: bool = True, learn_t: bool = False):
+    """(S, agg, lse, var) over the forward CSR `plan` (pg_genconv_aggregate): S [n_rows, d] in xs's dtype = the
+    per-channel softmax aggregate of ReLU(xs) + 1e-7 with temperature t (fp32 [1] on the device) plus xd; agg and
+    lse = log sum exp(t m) [n_rows, d] fp32 when `stats`, var [n_rows, d] fp32 when `stats` and `learn_t` (None
+    otherwise).  `keep`: uint8 keep mask of the halo rows (rows >= num_in of xs), or None."""
+    _rows(xs), _rows(xd)
+    n, d = plan.n_rows, xs.shape[1]
+    assert xd.dtype == xs.dtype and xd.shape == (n, d) and t.dtype == torch.float32 and t.is_cuda
+    dev = xs.device
+    s = alloc_rows(n, d, xs.dtype, dev)
+    agg = lse = var = None
+    if stats:
+        agg, lse = alloc_rows(n, d, torch.float32, dev), alloc_rows(n, d, torch.float32, dev)
+        if learn_t:
+            var = alloc_rows(n, d, torch.float32, dev)
+    parts = 4 if var is not None else 3
+    scratch = plan.scratch(parts * d)
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_genconv_aggregate(C.byref(plan.c), xs.data_ptr(), xs.stride(0), xd.data_ptr(), xd.stride(0), d,
+                                         _C.dtype_code(xs.dtype), t.data_ptr(), _ptr(keep), int(num_in), s.data_ptr(),
+                                         s.stride(0), _ptr(agg), agg.stride(0) if stats else 0, _ptr(lse),
+                                         lse.stride(0) if stats else 0, _ptr(var),
+                                         var.stride(0) if var is not None else 0, _ptr(scratch),
+                                         _scratch_ld(parts * d), _C.stream_ptr()), "pg_genconv_aggregate")
+    return s, agg, lse, var
+
+
+def genconv_bwd_dst(gs: torch.Tensor, agg: torch.Tensor, t: torch.Tensor, var: torch.Tensor = None, dtype=None):
+    """(Q, gst, dt) from g_S [n, d] fp32 (pg_genconv_bwd_dst): Q = t g_S agg fp32; gst = g_S rounded to `dtype` (None
+    when dtype is None); dt = sum g_S var as an fp32 [1] device tensor when var is given, else None."""
+    n, d = gs.shape
+    dev = gs.device
+    q = alloc_rows(n, d, torch.float32, dev)
+    gst = alloc_rows(n, d, dtype, dev) if dtype is not None else None
+    dt = partial = None
+    if var is not None:
+        dt = torch.empty(1, dtype=torch.float32, device=dev)
+        partial = torch.empty(GENCONV_DT_PARTIALS, dtype=torch.float64, device=dev)
+    _C.count(2 if var is not None else 1)
+    _C.check(_C.lib.pg_genconv_bwd_dst(gs.data_ptr(), gs.stride(0), agg.data_ptr(), agg.stride(0), _ptr(var),
+                                       var.stride(0) if var is not None else 0, t.data_ptr(), n, d,
+                                       _C.dtype_code(dtype if dtype is not None else torch.float32), q.data_ptr(),
+                                       q.stride(0), _ptr(gst), gst.stride(0) if gst is not None else 0, _ptr(partial),
+                                       _ptr(dt), _C.stream_ptr()), "pg_genconv_bwd_dst")
+    return q, gst, dt
+
+
+def genconv_bwd_src(plan_t: CsrPlan, xs: torch.Tensor, t: torch.Tensor, lse, gs, q, keep=None, num_in: int = 0,
+                    add: torch.Tensor = None, drop: DropSpec = None) -> torch.Tensor:
+    """dx [plan_t.n_rows, d] in xs's dtype over the CSC `plan_t` (pg_genconv_bwd_src): the gradient of x_src, plus
+    `add` (fp32) on its first add.shape[0] rows, through the dropout backward of `drop` when given."""
+    _rows(xs)
+    d = xs.shape[1]
+    dx = alloc_rows(plan_t.n_rows, d, xs.dtype, xs.device)
+    scratch = plan_t.scratch(d)
+    drop = drop if drop is not None and drop.p > 0 else None
+    _C.count(2 if plan_t.n_long else 1)
+    _C.check(_C.lib.pg_genconv_bwd_src(C.byref(plan_t.c), xs.data_ptr(), xs.stride(0), t.data_ptr(), _ptr(keep),
+                                       int(num_in), lse.data_ptr(), lse.stride(0), gs.data_ptr(), gs.stride(0),
+                                       q.data_ptr(), q.stride(0), _ptr(add), add.stride(0) if add is not None else 0,
+                                       add.shape[0] if add is not None else 0,
+                                       C.byref(drop.c()) if drop is not None else None, d, _C.dtype_code(xs.dtype),
+                                       dx.data_ptr(), dx.stride(0), _ptr(scratch), _scratch_ld(d), _C.stream_ptr()),
+             "pg_genconv_bwd_src")
+    return dx
+
+
+class GenConvLayerFn(torch.autograd.Function):
+    """One GENConv layer (PyG GENConv, aggr='softmax', scalar temperature t, no edge features, no message norm, MLP
+    [d, 2d, d] without norm or bias) over the [inner | halo] rows `feat` of a partition, returning the inner rows:
+
+        x_src = feat @ W_src^T   (or feat when d_in == d)   [num_all, d]    pg_linear over all rows
+        x_dst = feat[:N_in] @ W_dst^T  (or feat[:N_in])     [N_in, d]       pg_linear over the inner rows
+        S = softmax_aggregate(ReLU(x_src) + 1e-7) + x_dst   [N_in, d]       pg_genconv_aggregate (+ agg, L, var)
+        R = ReLU(S @ W1^T)                                  [N_in, 2d]      pg_linear, pg_gcnii_relu_drop
+        out = R @ W2^T                                      [N_in, d]       pg_linear
+
+    Backward: g_R = g @ W2 (pg_linear), g_H = ReLU'(R) g_R (pg_gcnii_relu_bwd), g_S = g_H @ W1 (fp32, pg_linear);
+    Q, g_S in the activation dtype and dt (pg_genconv_bwd_dst); dx_src over the CSC (pg_genconv_bwd_src); then
+    g_feat = dx_src @ W_src (+ g_S @ W_dst on the inner rows) as one two-source pg_linear with the dropout backward of
+    `drop_bwd` in its epilogue, or, when d_in == d, dx_src + g_S on the inner rows written by the source pass itself,
+    dropout backward included; dW2 = g^T R, dW1 = g_H^T S, dW_src = dx_src^T feat, dW_dst = g_S^T feat[:N_in]
+    (pg_wgrad).  `t` is an fp32 [1] device tensor read by the kernels (a CUDA graph sees its updates); its gradient dt
+    is returned when it requires one.  `keep`: the boundary-node sample of the halo rows (uint8), or None."""
+
+    @staticmethod
+    def forward(ctx, feat, graph, keep, t, w_src, w_dst, w1, w2, drop_bwd=None, train=True):
+        ctx.drop_bwd = drop_bwd
+        proj = w_src is not None
+        if not proj:
+            # feat is x_src itself: the kernels read whole 16-byte vectors of 16-byte aligned rows (a contiguous [N, d]
+            # tensor of an unaligned width, as whole-graph evaluation passes between layers, is copied to padded rows)
+            feat = _tma_ready(feat)
+        elif feat.stride(1) != 1:
+            feat = feat.contiguous()
+        n_in, dt_ = graph.num_in, feat.dtype
+        fsp = presplit(feat) if proj else feat
+        finner = fsp.rows(0, n_in) if isinstance(fsp, Split) else feat[:n_in]
+        xs = gemm_nt(fsp, padded_weight(w_src, dt_)) if proj else feat
+        xd = gemm_nt(finner, padded_weight(w_dst, dt_)) if proj else feat[:n_in]
+        keep_stats = train and any(ctx.needs_input_grad)
+        learn_t = keep_stats and ctx.needs_input_grad[3]
+        s, agg, lse, var = genconv_aggregate(graph.fwd, xs, xd, t, keep, n_in, stats=keep_stats, learn_t=learn_t)
+        del xd
+        r, _ = gcnii_relu_drop(gemm_nt(s, padded_weight(w1, dt_)))
+        out = gemm_nt(r, padded_weight(w2, dt_))
+        if keep_stats:
+            ctx.save_for_backward(feat, xs, s, agg, lse, var, r, t, w_src, w_dst, w1, w2)
+            ctx.graph, ctx.keep, ctx.proj = graph, keep, proj
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        feat, xs, s, agg, lse, var, r, t, w_src, w_dst, w1, w2 = ctx.saved_tensors
+        graph, keep, proj = ctx.graph, ctx.keep, ctx.proj
+        n_in, n_all, d = graph.num_in, feat.shape[0], xs.shape[1]
+        dt_ = feat.dtype
+        g = _tma_ready(g if g.dtype == dt_ else g.to(dt_))
+        gsp = presplit(g)
+        gh = gcnii_relu_bwd(gemm_nt(gsp, padded_weight(w2, dt_, transpose=True)), r)
+        ghsp = presplit(gh)
+        gs = gemm_nt(ghsp, padded_weight(w1, dt_, transpose=True), out_dtype=torch.float32)
+        gw2 = wgrad(gsp, presplit(r)).to(w2.dtype)
+        gw1 = wgrad(ghsp, presplit(s)).to(w1.dtype)
+        del gh, ghsp
+        q, gst, d_t = genconv_bwd_dst(gs, agg, t, var if ctx.needs_input_grad[3] else None,
+                                      dtype=dt_ if proj and dt_ != torch.float32 else None)
+        need_feat = ctx.needs_input_grad[0]
+        drop = ctx.drop_bwd if ctx.drop_bwd is not None and ctx.drop_bwd.p > 0 else None
+        g_feat = gw_src = gw_dst = None
+        if not proj:
+            # x_src = feat: the source pass adds g_S on the inner rows and applies the dropout backward itself
+            g_feat = genconv_bwd_src(graph.bwd, xs, t, lse, gs, q, keep, n_in, add=gs, drop=drop) if need_feat else None
+        else:
+            dxs = genconv_bwd_src(graph.bwd, xs, t, lse, gs, q, keep, n_in)
+            gst = gst if gst is not None else gs
+            dxsp, gstsp = presplit(dxs), presplit(gst)
+            if need_feat:
+                g_feat = alloc_rows(n_all, feat.shape[1], dt_, feat.device)
+                db = drop if drop is not None and feat.shape[1] <= 256 and _drop_ok(g_feat) else None
+                gemm_nt(dxsp.rows(0, n_in) if isinstance(dxsp, Split) else dxs[:n_in],
+                        padded_weight(w_src, dt_, transpose=True), gstsp, padded_weight(w_dst, dt_, transpose=True),
+                        out=g_feat[:n_in], drop=db)
+                if n_all > n_in:
+                    gemm_nt(dxsp.rows(n_in) if isinstance(dxsp, Split) else dxs[n_in:],
+                            padded_weight(w_src, dt_, transpose=True), out=g_feat[n_in:], drop=db, drop_row0=n_in)
+                if drop is not None and db is None:
+                    dropout_rows(g_feat, drop, out=g_feat)
+            fsp = presplit(feat)
+            gw_src = wgrad(dxsp, fsp).to(w_src.dtype)
+            gw_dst = wgrad(gstsp, fsp.rows(0, n_in) if isinstance(fsp, Split) else feat[:n_in]).to(w_dst.dtype)
+        return g_feat, None, None, d_t, gw_src, gw_dst, gw1, gw2, None, None
+
+
+def genconv_layer(feat, graph, keep, t, w_src, w_dst, w1, w2, drop_bwd=None) -> torch.Tensor:
+    """GENConv layer (GenConvLayerFn); w_src and w_dst None when d_in == d.  `t`: fp32 [1] on the device."""
+    return GenConvLayerFn.apply(feat, graph, keep, t, w_src, w_dst, w1, w2, drop_bwd, torch.is_grad_enabled())
+
+
 # ---- row-wise epilogues (csrc/rowops.cu) -------------------------------------------------------------------
 # column sums of a gradient tensor computed as a by-product by the kernel that produced it, keyed by the
 # tensor's address: the bias gradient of the linear upstream (saves a full pass over [N, d])

@@ -18,6 +18,7 @@ With `--eval --eval-partitioned` evaluation is collective: every rank evaluates 
 from __future__ import annotations
 
 import contextlib
+import math
 import os
 import time
 from types import SimpleNamespace
@@ -32,7 +33,7 @@ from .helper import context as ctx
 from .helper.feature_buffer import Buffer, EvalExchange, OneShotExchange, check_halo_bits, check_sampling
 from .helper.reducer import Reducer
 from .helper.timer.comm_timer import CommTimer
-from .module.model import GAT, GATv2, GCNII, PNA, GraphConv, GraphSAGE, GraphTransformer
+from .module.model import GAT, GATv2, GCNII, GENConv, PNA, GraphConv, GraphSAGE, GraphTransformer
 from .partition import PartitionLayout, get_layer_size
 
 
@@ -56,7 +57,8 @@ def check_model(args):
     square: the logits come from a linear) and --use-pp (graph layer 0 begins with fc_in, so a precomputed neighbour
     aggregate of x has no place).  --model pna refuses --aggregator pool (it has its own aggregators), --use-pp (the
     precompute is a neighbour mean) and --sampling-rate < 1 (sampling changes the degrees, the scalers and the sources
-    the extremes range over)."""
+    the extremes range over).  --model genconv refuses --use-pp (the precompute is a neighbour mean) and --aggregator
+    pool (it has its own aggregator), and a temperature --genconv-t that is not finite."""
     attention = args.model in ('gat', 'gatv2', 'transformer')
     aggregator = getattr(args, 'aggregator', 'mean')
     if aggregator not in ('mean', 'pool'):
@@ -84,6 +86,15 @@ def check_model(args):
         if getattr(args, 'sampling_rate', 1.0) < 1.0:
             raise NotImplementedError("--model pna with --sampling-rate < 1: sampling changes the degrees, the scalers "
                                       "and the sources the extremes range over")
+        return
+    if args.model == 'genconv':
+        if args.use_pp:
+            raise NotImplementedError("--model genconv with --use-pp: the precompute is a neighbour mean")
+        if aggregator == 'pool':
+            raise ValueError("--aggregator pool is a GraphSAGE aggregator; --model genconv has its own")
+        t = getattr(args, 'genconv_t', 1.0)
+        if not math.isfinite(t):
+            raise ValueError(f"--genconv-t {t}: expected a finite temperature")
         return
     if args.model == 'graphconv':
         if aggregator == 'pool':
@@ -124,6 +135,10 @@ def create_model(layer_size, args, buffer=None, dtype=torch.float32):
     if args.model == 'pna':
         return PNA(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
                    train_size=args.n_train, buffer=buffer, dtype=dtype)
+    if args.model == 'genconv':
+        return GENConv(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
+                       train_size=args.n_train, buffer=buffer, dtype=dtype, t=getattr(args, 'genconv_t', 1.0),
+                       learn_t=getattr(args, 'genconv_learn_t', False))
     if args.model in ('gat', 'gatv2', 'transformer'):
         cls = {'gat': GAT, 'gatv2': GATv2, 'transformer': GraphTransformer}[args.model]
         return cls(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
