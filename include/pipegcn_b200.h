@@ -646,6 +646,43 @@ int pg_genconv_bwd_src(const pg_csr* gt, const void* xs, int64_t ldxs, const flo
                        int dtype, void* dx, int64_t lddx, float* scratch, int64_t ld_scratch, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Residual gated graph convolution (Bresson & Laurent, 2017; PyG ResGatedGraphConv, sigmoid gate, no edge features)
+ * over the `_U` rows [inner | halo] of one partition.  Every operand is fp32 or bf16 (`dtype`), and two of them are
+ * paired rows with halves `half` columns apart: qv [num_all rows] holds q at columns [0, d) and val at
+ * [half, half + d); ks [N_in rows] holds k at [0, d) and skip at [half, half + d) (skip carries the output bias).
+ * For the in-edges u -> v of the forward CSR g whose source is kept, per column c, with x = fl(k[v] + q[u]):
+ *   e = exp(-|x|),  r = 1 / (1 + e),  sigmoid(x) = x >= 0 ? r : e r,  sigmoid'(x) = e r r   (one expf per element)
+ *   out[v] = skip[v] + sum_u sigmoid(x) val[u]
+ * Sums are fp32 with one multiply-add per term, in CSR order (CSC order in the source pass); long rows come as
+ * segments whose partials a fix-up adds in segment order.  No atomics and no per-edge storage (both backward passes
+ * recompute the gate): the results are the same bits from run to run.  A row without a kept in-edge gets out = skip.
+ * keep (uint8 [num_all - num_in], or NULL: every source kept) is the keep mask of the halo rows: a source
+ * u >= num_in with keep[u - num_in] == 0 is skipped.  Every result is rounded once to dtype.  The kernels read and
+ * write whole vectors of VB bytes, VB the widest of 16, 8, 4 (and 2 for bf16) that every operand's base, second half
+ * and row stride allow; each row's last vector is written whole, the columns past d as 0, so `half` and every row
+ * stride must reach round_up(d, VB / element size) (past `half` too for a paired operand).  The plans must carry the
+ * chunk table; scratch is fp32 [n_seg][ld_scratch] (may be NULL when n_seg == 0).
+ * ---------------------------------------------------------------------------------------- */
+/* loads every ResGatedGCN kernel (call it before any halo wait can spin: a first launch may wait for the device) */
+int pg_resgated_preload(void);
+/* out [N_in, d] over the forward CSR g.  ld_scratch >= d */
+int pg_resgated_aggregate(const pg_csr* g, const void* qv, int64_t ldqv, const void* ks, int64_t ldks, int32_t half,
+                          int32_t d, int dtype, const uint8_t* keep, int32_t num_in, void* out, int64_t ldo,
+                          float* scratch, int64_t ld_scratch, void* stream);
+/* over the forward CSR g, with G = grad [N_in, d] the gradient of out: the paired rows dkg [N_in] get
+ *   dk[v] = G[v] sum_u sigmoid'(x) val[u]  at [0, d),   a copy of G[v]  at [half, half + d)
+ * (the [dk | G] operand of the input-gradient GEMM).  ld_scratch >= d */
+int pg_resgated_bwd_dst(const pg_csr* g, const void* qv, int64_t ldqv, const void* ks, int64_t ldks, int32_t half,
+                        const void* grad, int64_t ldg, int32_t d, int dtype, const uint8_t* keep, int32_t num_in,
+                        void* dkg, int64_t lddkg, float* scratch, int64_t ld_scratch, void* stream);
+/* over the CSC row u of gt (rows = all num_all `_U` rows, entries the destinations v of u): the paired rows dqv get
+ *   dq[u] = val[u] sum_v G[v] sigmoid'(x)  at [0, d),   dval[u] = sum_v G[v] sigmoid(x)  at [half, half + d)
+ * An unkept halo row, and a row without out-edges, get exact zeros (its val is not read).  ld_scratch >= 2 d */
+int pg_resgated_bwd_src(const pg_csr* gt, const void* qv, int64_t ldqv, const void* ks, int64_t ldks, int32_t half,
+                        const void* grad, int64_t ldg, int32_t d, int dtype, const uint8_t* keep, int32_t num_in,
+                        void* dqv, int64_t lddqv, float* scratch, int64_t ld_scratch, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Symmetric heap: device memory that peers map through CUDA IPC (host pointers out).
  * ---------------------------------------------------------------------------------------- */
 #define PG_IPC_HANDLE_BYTES 64

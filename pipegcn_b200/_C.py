@@ -156,6 +156,13 @@ def _load():
                                          vp]),
         "pg_genconv_bwd_src": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, vp, i32, vp, i64, vp, i64, vp, i64, vp, i64,
                                          i32, C.POINTER(pg_drop), i32, C.c_int, vp, i64, vp, i64, vp]),
+        "pg_resgated_preload": (C.c_int, []),
+        "pg_resgated_aggregate": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, i32, i32, C.c_int, vp, i32, vp, i64,
+                                            vp, i64, vp]),
+        "pg_resgated_bwd_dst": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, i32, vp, i64, i32, C.c_int, vp, i32,
+                                          vp, i64, vp, i64, vp]),
+        "pg_resgated_bwd_src": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, i32, vp, i64, i32, C.c_int, vp, i32,
+                                          vp, i64, vp, i64, vp]),
         "pg_heap_alloc": (C.c_int, [C.c_size_t, C.POINTER(vp)]),
         "pg_heap_free": (C.c_int, [vp]),
         "pg_ipc_export": (C.c_int, [vp, C.c_char_p]),

@@ -59,6 +59,11 @@ float, default 1.0; 0 and negative values are allowed) sets the temperature, and
 parameter (`aggr_module.t` of every graph layer).  Both are suppressed like `--sampling-rate`: read them with
 getattr(args, 'genconv_t', 1.0) and getattr(args, 'genconv_learn_t', False).  It works with boundary-node sampling
 and cannot be combined with --use-pp or --aggregator pool.
+
+`--model resgatedgcn` (not in the reference) trains the residual gated graph convolution of Bresson & Laurent (2017;
+PyG's ResGatedGraphConv): every layer sums the values val_u of its in-edges, each weighted by its own per-channel gate
+sigmoid(k_v + q_u), and adds a skip linear of h_v and a bias.  It has no flags of its own (--n-heads is ignored).  It
+works with boundary-node sampling and cannot be combined with --use-pp or --aggregator pool.
 """
 import argparse
 
@@ -67,7 +72,8 @@ _FLAGS = [
     ("dataset", dict(type=str, default='reddit', help="the input dataset (or synthetic:<shape>)")),
     ("graph-name", dict(type=str, default='')),
     ("model", dict(type=str, default='graphsage', help="model for training (graphsage | gcn | gat | gatv2 | transformer | "
-                                                              "graphconv | gcnii | pna | genconv; gcn is GraphSAGE)")),
+                                                              "graphconv | gcnii | pna | genconv | resgatedgcn; gcn is "
+                                                              "GraphSAGE)")),
     ("dropout", dict(type=float, default=0.5, help="dropout probability")),
     ("lr", dict(type=float, default=1e-2, help="learning rate")),
     ("n-epochs", dict(type=int, default=200, help="the number of training epochs")),

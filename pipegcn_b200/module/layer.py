@@ -105,6 +105,21 @@ State-dict keys: `lin_src.weight` and `lin_dst.weight` [d, d_in] (only when d_in
 [2d, d], `mlp.lins.1.weight` [d, 2d] and `aggr_module.t`.  Every weight is drawn as `nn.Linear` draws it
 (kaiming_uniform_(a=sqrt(5))), in the order lin_src, lin_dst, mlp.lins.0, mlp.lins.1.  PyG draws some of them twice
 (at construction and in reset_parameters), so equal seeds do not give PyG's initial weights.
+
+`ResGatedLayer` (not in the reference): the residual gated graph convolution of Bresson & Laurent ("Residual Gated
+Graph ConvNets", 2017), PyG's `ResGatedGraphConv(d_in, d_out, act=Sigmoid(), edge_dim=None, root_weight=True,
+bias=True)` with aggr='add', over the same rows, per channel:
+
+    k = h[:N_in] @ W_k^T + b_k,  q = h @ W_q^T + b_q,  val = h @ W_v^T + b_v,  skip = h[:N_in] @ W_s^T
+    out[v] = skip[v] + b + sum_{u -> v} sigmoid(k[v] + q[u]) * val[u]      (skip + b for a row without in-edges)
+
+Each edge has its own gate and nothing normalises the gates over the in-edges: with boundary-node sampling the unkept
+halo sources are absent from every sum, which is exactly the layer over the sampled graph (no rescaling).  State-dict
+keys are ResGatedGraphConv's: `lin_key.*`, `lin_query.*`, `lin_value.*` (weights [d_out, d_in] and biases [d_out]),
+`lin_skip.weight` [d_out, d_in] (no bias) and `bias` [d_out].  Each linear is drawn as `nn.Linear` draws it
+(kaiming_uniform_(a=sqrt(5)), then its bias U(-1/sqrt(d_in), 1/sqrt(d_in))), in the order lin_key, lin_query,
+lin_value, lin_skip, then bias = 0.  PyG draws the linears twice (at construction and in reset_parameters), so equal
+seeds do not give PyG's initial weights.
 """
 import math
 
@@ -369,3 +384,23 @@ class GENConvLayer(nn.Module):
                                  self.lin_src.weight if self.lin_src is not None else None,
                                  self.lin_dst.weight if self.lin_dst is not None else None,
                                  self.mlp.lins[0].weight, self.mlp.lins[1].weight, drop_bwd)
+
+
+class ResGatedLayer(nn.Module):
+    """ResGatedGraphConv(in_feats, out_feats), sigmoid gate, root weight and bias: module docstring."""
+
+    def __init__(self, in_feats, out_feats):
+        super().__init__()
+        self.in_feats, self.out_feats = in_feats, out_feats
+        self.lin_key = nn.Linear(in_feats, out_feats)
+        self.lin_query = nn.Linear(in_feats, out_feats)
+        self.lin_value = nn.Linear(in_feats, out_feats)
+        self.lin_skip = nn.Linear(in_feats, out_feats, bias=False)
+        self.bias = nn.Parameter(torch.zeros(out_feats))
+
+    def forward(self, graph, feat, keep=None, drop_bwd=None):
+        """As GATLayer.forward: `feat` [num_all, d_in] rows of `graph`, `keep` the keep mask of the halo rows
+        (boundary-node sampling, uint8) or None; returns the [N_in, d_out] inner rows."""
+        return ops.resgated_layer(feat, graph, keep, self.lin_key.weight, self.lin_key.bias, self.lin_query.weight,
+                                  self.lin_query.bias, self.lin_value.weight, self.lin_value.bias,
+                                  self.lin_skip.weight, self.bias, drop_bwd)

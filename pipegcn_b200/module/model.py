@@ -48,6 +48,11 @@ aggregator, module/layer.py); a last graph layer that produces the logits is a G
 `GAT`, with boundary-node sampling its layers take the buffer's keep mask of the halo rows, and unkept rows are absent
 from every softmax.  The temperature `t` (constant, or learnt with `learn_t`) is read by the kernels from device
 memory, so a captured CUDA graph sees the optimizer's updates of it.
+
+`ResGatedGCN(GraphSAGE)` (not in the reference) is the same layer loop with `ResGatedLayer`s (PyG's ResGatedGraphConv,
+module/layer.py); a last graph layer that produces the logits is a ResGatedLayer(d_in, n_class).  Like `GENConv`, with
+boundary-node sampling its layers take the buffer's keep mask of the halo rows, and unkept rows are absent from every
+sum.
 """
 import torch
 from torch import nn
@@ -55,7 +60,7 @@ import torch.nn.functional as F
 
 from ..helper import context as ctx
 from .layer import (GATLayer, GATv2Layer, GCNIILayer, GENConvLayer, GraphConvLayer, GraphSAGELayer, PNALayer,
-                    TransformerLayer)
+                    ResGatedLayer, TransformerLayer)
 
 
 class GNNBase(nn.Module):
@@ -407,7 +412,28 @@ class PNA(GraphSAGE):
         return (yield from super().forward_partitioned(g, xch, pp_feat, push0))
 
 
-class GENConv(GraphSAGE):
+class _KeepMaskLayers(GraphSAGE):
+    """The layer loop of a model whose graph layers take the keep mask of this epoch's boundary-node sample as their
+    third argument (`GENConv`, `ResGatedGCN`) and whose kernels `_preload` loads before any halo wait can spin."""
+
+    def _layer_arg(self, in_deg):
+        """The keep mask of this epoch's boundary-node sample (training with sampling), else None."""
+        buf = self._buffer() if self.training else None
+        return getattr(buf, 'keep_mask', None) if buf is not None else None
+
+    def _preload(self):
+        raise NotImplementedError
+
+    def forward(self, g, feat, in_deg=None):
+        self._preload()
+        return super().forward(g, feat, in_deg)
+
+    def forward_partitioned(self, g, xch, pp_feat=None, push0=False):
+        self._preload()
+        return (yield from super().forward_partitioned(g, xch, pp_feat, push0))
+
+
+class GENConv(_KeepMaskLayers):
 
     def __init__(self, layer_size, activation, dropout=0.5, norm='layer', train_size=None, n_linear=0, buffer=None,
                  dtype=torch.float32, t=1.0, learn_t=False):
@@ -418,19 +444,21 @@ class GENConv(GraphSAGE):
     def _graph_layer(self, i, d_in, d_out):
         return GENConvLayer(d_in, d_out, t=self.t, learn_t=self.learn_t)
 
-    def _layer_arg(self, in_deg):
-        """The keep mask of this epoch's boundary-node sample (training with sampling), else None."""
-        buf = self._buffer() if self.training else None
-        return getattr(buf, 'keep_mask', None) if buf is not None else None
-
     def _preload(self):
         from .. import ops
         ops.genconv_preload()
 
-    def forward(self, g, feat, in_deg=None):
-        self._preload()
-        return super().forward(g, feat, in_deg)
 
-    def forward_partitioned(self, g, xch, pp_feat=None, push0=False):
-        self._preload()
-        return (yield from super().forward_partitioned(g, xch, pp_feat, push0))
+class ResGatedGCN(_KeepMaskLayers):
+
+    def __init__(self, layer_size, activation, dropout=0.5, norm='layer', train_size=None, n_linear=0, buffer=None,
+                 dtype=torch.float32):
+        super().__init__(layer_size, activation, False, dropout=dropout, norm=norm, train_size=train_size,
+                         n_linear=n_linear, buffer=buffer, dtype=dtype)
+
+    def _graph_layer(self, i, d_in, d_out):
+        return ResGatedLayer(d_in, d_out)
+
+    def _preload(self):
+        from .. import ops
+        ops.resgated_preload()

@@ -2070,6 +2070,131 @@ def genconv_layer(feat, graph, keep, t, w_src, w_dst, w1, w2, drop_bwd=None) -> 
     return GenConvLayerFn.apply(feat, graph, keep, t, w_src, w_dst, w1, w2, drop_bwd, torch.is_grad_enabled())
 
 
+# ---- residual gated graph convolution, ResGatedGraphConv (csrc/resgated.cu) --------------------------------
+def resgated_preload():
+    """Load every ResGatedGCN kernel now (see gat_preload)."""
+    _C.check(_C.lib.pg_resgated_preload(), "pg_resgated_preload")
+
+
+def resgated_aggregate(graph: PartGraph, qv, ks, d: int, half: int, keep=None):
+    """out [N_in, d] in qv's dtype = skip[v] + sum_u sigmoid(k[v] + q[u]) val[u] over the forward CSR
+    (pg_resgated_aggregate); qv = [q | val] [num_all, >= half + d] and ks = [k | skip] [N_in, >= half + d] with the
+    second halves at column `half`."""
+    plan = graph.fwd
+    out = alloc_rows(plan.n_rows, d, qv.dtype, qv.device)
+    scratch = plan.scratch(d)
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_resgated_aggregate(C.byref(plan.c), qv.data_ptr(), qv.stride(0), ks.data_ptr(), ks.stride(0),
+                                          int(half), int(d), _C.dtype_code(qv.dtype), _ptr(keep), graph.num_in,
+                                          out.data_ptr(), out.stride(0), _ptr(scratch), _scratch_ld(d),
+                                          _C.stream_ptr()), "pg_resgated_aggregate")
+    return out
+
+
+def resgated_bwd_dst(graph: PartGraph, qv, ks, g, d: int, half: int, keep=None, dkg=None):
+    """[dk | g] [N_in, 2 half] in qv's dtype over the forward CSR (pg_resgated_bwd_dst): dk[v] = g[v] sum_u
+    sigmoid'(k[v] + q[u]) val[u] at [0, d), a copy of g at [half, half + d).  `dkg`: the tensor to write (allocated
+    when None, with zero pad columns)."""
+    plan = graph.fwd
+    if dkg is None:
+        dkg = alloc_rows(plan.n_rows, 2 * half, qv.dtype, qv.device, zero=half != d)
+    scratch = plan.scratch(d)
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_resgated_bwd_dst(C.byref(plan.c), qv.data_ptr(), qv.stride(0), ks.data_ptr(), ks.stride(0),
+                                        int(half), g.data_ptr(), g.stride(0), int(d), _C.dtype_code(qv.dtype),
+                                        _ptr(keep), graph.num_in, dkg.data_ptr(), dkg.stride(0), _ptr(scratch),
+                                        _scratch_ld(d), _C.stream_ptr()), "pg_resgated_bwd_dst")
+    return dkg
+
+
+def resgated_bwd_src(graph: PartGraph, qv, ks, g, d: int, half: int, keep=None, dqv=None):
+    """[dq | dval] [num_all, 2 half] in qv's dtype over the CSC of the graph (pg_resgated_bwd_src): dq[u] = val[u]
+    sum_v g[v] sigmoid'(k[v] + q[u]) at [0, d), dval[u] = sum_v g[v] sigmoid(k[v] + q[u]) at [half, half + d); 0 on
+    unkept halo rows.  `dqv`: the tensor to write (allocated when None, with zero pad columns)."""
+    plan = graph.bwd
+    if dqv is None:
+        dqv = alloc_rows(plan.n_rows, 2 * half, qv.dtype, qv.device, zero=half != d)
+    scratch = plan.scratch(2 * d)
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_resgated_bwd_src(C.byref(plan.c), qv.data_ptr(), qv.stride(0), ks.data_ptr(), ks.stride(0),
+                                        int(half), g.data_ptr(), g.stride(0), int(d), _C.dtype_code(qv.dtype),
+                                        _ptr(keep), graph.num_in, dqv.data_ptr(), dqv.stride(0), _ptr(scratch),
+                                        _scratch_ld(2 * d), _C.stream_ptr()), "pg_resgated_bwd_src")
+    return dqv
+
+
+class ResGatedLayerFn(torch.autograd.Function):
+    """One residual gated graph convolution (PyG ResGatedGraphConv, act=Sigmoid, root_weight=True, bias=True, no edge
+    features) over the [inner | halo] rows `feat` of a partition, returning the inner rows.  With W the half width of
+    transformer_width:
+
+        [q | val]  = feat @ [W_q; W_v]^T + [b_q; b_v]          [num_all, 2W]   one pg_linear over all rows
+        [k | skip] = feat[:N_in] @ [W_k; W_s]^T + [b_k; b]     [N_in, 2W]      one pg_linear over the inner rows
+        out[v] = skip[v] + sum_u sigmoid(k[v] + q[u]) val[u]   [N_in, d]       pg_resgated_aggregate
+
+    Backward: [dk | g] (pg_resgated_bwd_dst over the CSR), [dq | dval] (pg_resgated_bwd_src over the CSC), the bias
+    gradients as fixed-order column sums (b from the column sum the LayerNorm backward stashed, when there is one), the
+    weight gradients as one pg_wgrad per row set, and g_feat = [dq | dval] @ [W_q; W_v] (+ [dk | g] @ [W_k; W_s] on the
+    inner rows, one two-source pg_linear), with the dropout backward of `drop_bwd` in its epilogue.  `keep`: the
+    boundary-node sample of the halo rows (uint8), or None."""
+
+    @staticmethod
+    def forward(ctx, feat, graph, keep, w_k, b_k, w_q, b_q, w_v, b_v, w_s, bias, drop_bwd=None):
+        ctx.drop_bwd = drop_bwd
+        if feat.stride(1) != 1:
+            feat = feat.contiguous()
+        n_in, d = graph.num_in, w_q.shape[0]
+        w = transformer_width(d, feat.dtype)
+        fsp = presplit(feat)                   # fp32: one split of feat for both products
+        qv = gemm_nt(fsp, _pair_weight(w_q, w_v, w, feat.dtype), bias=_pair_bias(b_q, b_v, d, w))
+        ks = gemm_nt(fsp.rows(0, n_in) if isinstance(fsp, Split) else feat[:n_in],
+                     _pair_weight(w_k, w_s, w, feat.dtype), bias=_pair_bias(b_k, bias, d, w))
+        out = resgated_aggregate(graph, qv, ks, d, w, keep)
+        ctx.save_for_backward(feat, qv, ks, w_k, w_q, w_v, w_s)
+        ctx.graph, ctx.keep, ctx.width = graph, keep, w
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        feat, qv, ks, w_k, w_q, w_v, w_s = ctx.saved_tensors
+        graph, keep, w = ctx.graph, ctx.keep, ctx.width
+        n_in, n_all, d = graph.num_in, feat.shape[0], w_q.shape[0]
+        colsum = _take_colsum(g)
+        g = _tma_ready(g if g.dtype == feat.dtype else g.to(feat.dtype))
+        dkg = resgated_bwd_dst(graph, qv, ks, g, d, w, keep)
+        dqv = resgated_bwd_src(graph, qv, ks, g, d, w, keep)
+        gb_qv = gat_colsum(dqv)
+        if colsum is not None:
+            gbk, gb = gat_colsum(dkg[:, :d]), colsum
+        else:
+            gb_ks = gat_colsum(dkg)
+            gbk, gb = gb_ks[:d], gb_ks[w:w + d]
+        dqvp, dkgp = presplit(dqv), presplit(dkg)
+        is_split = isinstance(dqvp, Split)
+        g_feat = None
+        if ctx.needs_input_grad[0]:
+            g_feat = alloc_rows(n_all, feat.shape[1], feat.dtype, feat.device)
+            wqv = _pair_weight(w_q, w_v, w, feat.dtype, transpose=True)
+            drop = ctx.drop_bwd if ctx.drop_bwd is not None and ctx.drop_bwd.p > 0 else None
+            db = drop if drop is not None and feat.shape[1] <= 256 and _drop_ok(g_feat) else None
+            gemm_nt(dqvp.rows(0, n_in) if is_split else dqv[:n_in], wqv, dkgp,
+                    _pair_weight(w_k, w_s, w, feat.dtype, transpose=True), out=g_feat[:n_in], drop=db)
+            if n_all > n_in:
+                gemm_nt(dqvp.rows(n_in) if is_split else dqv[n_in:], wqv, out=g_feat[n_in:], drop=db, drop_row0=n_in)
+            if drop is not None and db is None:
+                dropout_rows(g_feat, drop, out=g_feat)
+        fsp = presplit(feat)
+        gw_qv = wgrad(dqvp, fsp)
+        gw_ks = wgrad(dkgp, fsp.rows(0, n_in) if isinstance(fsp, Split) else feat[:n_in])
+        gwk, gwq, gwv, gws = [t.contiguous() for t in (gw_ks[:d], gw_qv[:d], gw_qv[w:w + d], gw_ks[w:w + d])]
+        return (g_feat, None, None, gwk.to(w_k.dtype), gbk.contiguous(), gwq.to(w_q.dtype), gb_qv[:d].contiguous(),
+                gwv.to(w_v.dtype), gb_qv[w:w + d].contiguous(), gws.to(w_s.dtype), gb.contiguous(), None)
+
+
+def resgated_layer(feat, graph, keep, w_k, b_k, w_q, b_q, w_v, b_v, w_s, bias, drop_bwd=None) -> torch.Tensor:
+    return ResGatedLayerFn.apply(feat, graph, keep, w_k, b_k, w_q, b_q, w_v, b_v, w_s, bias, drop_bwd)
+
+
 # ---- row-wise epilogues (csrc/rowops.cu) -------------------------------------------------------------------
 # column sums of a gradient tensor computed as a by-product by the kernel that produced it, keyed by the
 # tensor's address: the bias gradient of the linear upstream (saves a full pass over [N, d])

@@ -33,7 +33,7 @@ from .helper import context as ctx
 from .helper.feature_buffer import Buffer, EvalExchange, OneShotExchange, check_halo_bits, check_sampling
 from .helper.reducer import Reducer
 from .helper.timer.comm_timer import CommTimer
-from .module.model import GAT, GATv2, GCNII, GENConv, PNA, GraphConv, GraphSAGE, GraphTransformer
+from .module.model import GAT, GATv2, GCNII, GENConv, PNA, GraphConv, GraphSAGE, GraphTransformer, ResGatedGCN
 from .partition import PartitionLayout, get_layer_size
 
 
@@ -58,7 +58,8 @@ def check_model(args):
     aggregate of x has no place).  --model pna refuses --aggregator pool (it has its own aggregators), --use-pp (the
     precompute is a neighbour mean) and --sampling-rate < 1 (sampling changes the degrees, the scalers and the sources
     the extremes range over).  --model genconv refuses --use-pp (the precompute is a neighbour mean) and --aggregator
-    pool (it has its own aggregator), and a temperature --genconv-t that is not finite."""
+    pool (it has its own aggregator), and a temperature --genconv-t that is not finite.  --model resgatedgcn refuses
+    --use-pp (the precompute is a neighbour mean) and --aggregator pool (it has its own aggregator)."""
     attention = args.model in ('gat', 'gatv2', 'transformer')
     aggregator = getattr(args, 'aggregator', 'mean')
     if aggregator not in ('mean', 'pool'):
@@ -95,6 +96,12 @@ def check_model(args):
         t = getattr(args, 'genconv_t', 1.0)
         if not math.isfinite(t):
             raise ValueError(f"--genconv-t {t}: expected a finite temperature")
+        return
+    if args.model == 'resgatedgcn':
+        if args.use_pp:
+            raise NotImplementedError("--model resgatedgcn with --use-pp: the precompute is a neighbour mean")
+        if aggregator == 'pool':
+            raise ValueError("--aggregator pool is a GraphSAGE aggregator; --model resgatedgcn has its own")
         return
     if args.model == 'graphconv':
         if aggregator == 'pool':
@@ -139,6 +146,9 @@ def create_model(layer_size, args, buffer=None, dtype=torch.float32):
         return GENConv(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
                        train_size=args.n_train, buffer=buffer, dtype=dtype, t=getattr(args, 'genconv_t', 1.0),
                        learn_t=getattr(args, 'genconv_learn_t', False))
+    if args.model == 'resgatedgcn':
+        return ResGatedGCN(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
+                           train_size=args.n_train, buffer=buffer, dtype=dtype)
     if args.model in ('gat', 'gatv2', 'transformer'):
         cls = {'gat': GAT, 'gatv2': GATv2, 'transformer': GraphTransformer}[args.model]
         return cls(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
