@@ -191,6 +191,21 @@ int pg_linear(int dtype_in, int dtype_out, const pg_gemm_src* srcs, int32_t n_sr
 int pg_linear_drop(int dtype_in, int dtype_out, const pg_gemm_src* srcs, int32_t n_src, const float* bias,
                    const float* row_div, void* c, int64_t ldc, int32_t m, int32_t n, const pg_drop* drop,
                    int64_t drop_row0, void* stream);
+/* Grouped form: n_prob (1..4) products that share their A operands, each with its own B operands and output, in one
+ * launch.  `srcs` holds n_prob x n_src pairs (problem-major, n_prob * n_src <= 12); pair s of every problem has the
+ * A operand (a, lda, k) of srcs[s].  Problem q writes outs[q] = sum_s A_s B_{q,s}^T (+ bias) (/ row_div), with the
+ * dropout of outs[q].drop, exactly as one pg_linear_drop call on its pairs would.  The CTAs working on the same rows
+ * of A run together, so A is read from HBM once for all problems (the rest from L2). */
+typedef struct pg_gemm_out {
+  const float* bias;     /* [n] or NULL */
+  const float* row_div;  /* [m] or NULL */
+  void* c;
+  int64_t ldc;
+  const pg_drop* drop;   /* NULL or p == 0: no dropout */
+  int64_t drop_row0;
+} pg_gemm_out;
+int pg_linear_group(int dtype_in, int dtype_out, const pg_gemm_src* srcs, int32_t n_src, int32_t n_prob,
+                    const pg_gemm_out* outs, int32_t m, int32_t n, void* stream);
 
 /*
  * Weight gradients on the Hopper tensor cores (MN-major bf16 operands, split-K over the rows, deterministic;
@@ -204,6 +219,20 @@ int pg_linear_drop(int dtype_in, int dtype_out, const pg_gemm_src* srcs, int32_t
 int64_t pg_wgrad_workspace(int32_t m, int32_t n, int32_t k, int dtype_in);
 int pg_wgrad(int dtype_in, const pg_gemm_src* srcs, int32_t n_src, float* out, int64_t ldo, int32_t m, int32_t n,
              int32_t k, float* workspace, int64_t workspace_floats, void* stream);
+/* Grouped form: n_prob (1..2) weight gradients of the same n x k shape in one launch (and one reduction launch).
+ * `srcs` holds n_prob x n_src pairs, problem-major.  Problem q has its own rows (outs[q].m), split-K partition and
+ * workspace (pg_wgrad_workspace(outs[q].m, n, k, dtype_in) floats) and gets the bits of a lone pg_wgrad call.  The CTAs
+ * of all problems over the same row slice run side by side, so an operand the problems share (g^T x and g^T ah) is
+ * read from HBM once. */
+typedef struct pg_wgrad_out {
+  float* out;
+  int64_t ldo;
+  int32_t m;
+  float* workspace;
+  int64_t workspace_floats;
+} pg_wgrad_out;
+int pg_wgrad_group(int dtype_in, const pg_gemm_src* srcs, int32_t n_src, int32_t n_prob, const pg_wgrad_out* outs,
+                   int32_t n, int32_t k, void* stream);
 
 /* hi = x with the 13 low mantissa bits cleared (a tf32 value), lo = x - hi (exact); [rows, d] fp32 */
 int pg_split_tf32(const float* x, int64_t ldx, float* hi, float* lo, int64_t ld, int32_t rows, int32_t d,

@@ -32,6 +32,16 @@ class pg_gemm_src(C.Structure):
     _fields_ = [("a", C.c_void_p), ("lda", C.c_int64), ("b", C.c_void_p), ("ldb", C.c_int64), ("k", C.c_int32)]
 
 
+class pg_gemm_out(C.Structure):
+    _fields_ = [("bias", C.c_void_p), ("row_div", C.c_void_p), ("c", C.c_void_p), ("ldc", C.c_int64),
+                ("drop", C.c_void_p), ("drop_row0", C.c_int64)]
+
+
+class pg_wgrad_out(C.Structure):
+    _fields_ = [("out", C.c_void_p), ("ldo", C.c_int64), ("m", C.c_int32), ("workspace", C.c_void_p),
+                ("workspace_floats", C.c_int64)]
+
+
 class pg_msg(C.Structure):
     _fields_ = [("idx", C.c_void_p), ("src_row0", C.c_int64), ("n_rows", C.c_int32), ("cta_begin", C.c_int32),
                 ("dst", C.c_void_p), ("ld_dst", C.c_int64), ("ema", C.c_void_p), ("ld_ema", C.c_int64),
@@ -81,8 +91,11 @@ def _load():
         "pg_linear": (C.c_int, [C.c_int, C.c_int, C.POINTER(pg_gemm_src), i32, vp, vp, vp, i64, i32, i32, vp]),
         "pg_linear_drop": (C.c_int, [C.c_int, C.c_int, C.POINTER(pg_gemm_src), i32, vp, vp, vp, i64, i32, i32,
                                      C.POINTER(pg_drop), i64, vp]),
+        "pg_linear_group": (C.c_int, [C.c_int, C.c_int, C.POINTER(pg_gemm_src), i32, i32, C.POINTER(pg_gemm_out), i32,
+                                      i32, vp]),
         "pg_wgrad_workspace": (i64, [i32, i32, i32, C.c_int]),
         "pg_wgrad": (C.c_int, [C.c_int, C.POINTER(pg_gemm_src), i32, vp, i64, i32, i32, i32, vp, i64, vp]),
+        "pg_wgrad_group": (C.c_int, [C.c_int, C.POINTER(pg_gemm_src), i32, i32, C.POINTER(pg_wgrad_out), i32, i32, vp]),
         "pg_split_tf32": (C.c_int, [vp, i64, vp, vp, i64, i32, i32, vp]),
         "pg_row_grid": (C.c_int, [i32]),
         "pg_dropout": (C.c_int, [vp, i64, vp, i64, i32, i32, C.c_int, f32, C.c_uint64, vp, vp]),

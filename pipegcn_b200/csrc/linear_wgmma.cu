@@ -7,6 +7,13 @@
 // GEMMs of its backward (row_div = in_deg fuses the `/ degs` gradient), and with three pairs per product
 // the split-fp32 "3xTF32" evaluation (hi*hi + hi*lo + lo*hi) used for fp32 activations.
 //
+// Grouped form: up to kMaxProb problems share the A operands (every source's A) and each has its own B operands, bias,
+// row scale, output and dropout -- the two dX products g W1 and (g W2) / deg of a layer backward.  The grid is a
+// multiple of the problem count and CTA b serves problem b % n_prob on M tiles b / n_prob, b / n_prob + gridDim /
+// n_prob, ...: the CTAs that multiply the same 128 rows of A are adjacent and run side by side, so every A tile after
+// the first comes from L2 and A is read from HBM once instead of once per problem.  A tile computes exactly what a
+// lone launch computes for it (same K order, same epilogue).
+//
 // Persistent, warp-specialised, sm_90a only, three warpgroups:
 //   warpgroup 0     one thread is the TMA producer: 128-byte-swizzled K-major tiles of A (128 rows) and B (NT rows)
 //                   into a 4-stage shared-memory ring, completion on mbarriers; its registers go to the consumers
@@ -30,45 +37,57 @@ constexpr int kGemmThreads = 384;       // producer warpgroup + 2 consumer warpg
 constexpr int kABytes = kBlockM * kRowBytes;   // 16 KB per stage
 
 constexpr int kMaxSrc = 6;              // 2 operands pairs x 3 passes of the split-fp32 (3xTF32) product
+constexpr int kMaxProb = 4;             // problems of one grouped launch
+constexpr int kMaxB = 12;               // B operands of one launch: problems x sources
 
 struct GemmMaps {
-  CUtensorMap a[kMaxSrc];
-  CUtensorMap b[kMaxSrc];
-  CUtensorMap c;             // output, box = [16 rows, 128 bytes], used by the TMA-store epilogue
+  CUtensorMap a[kMaxSrc];    // shared by every problem
+  CUtensorMap b[kMaxB];      // problem q, source s: b[q * n_src + s]
+  CUtensorMap c[kMaxProb];   // outputs, box = [16 rows, 128 bytes], used by the TMA-store epilogue
 };
 constexpr int kSlabRows = 16;                         // rows of the accumulator one warp holds
 constexpr int kSlabBytes = kSlabRows * kRowBytes;     // one staging slab: 16 rows x 128 B
 constexpr int kSlabsTotal = 8 /*consumer warps*/ * 2 * kSlabBytes;
 
-struct GemmArgs {
-  int m, n;
-  int n_src;
-  int kb_end[kMaxSrc];       // prefix sums of the k-blocks (of 128 bytes) of every source
-  int k_elems;               // elements per k-block
+struct GemmOut {
   const float* bias;         // [n] or null
   const float* row_div;      // [m] or null
   void* c;
   int64_t ldc;
-  int out_bf16;              // 1: bf16 output, 0: fp32 output
   int tma_store;             // 1: epilogue stages through shared memory and stores with TMA
-  int epi_slabs;             // 1 | 2 staging slabs per epilogue warp
   DropArg drop;              // dropout applied to the output as it is written (thresh16 == 0: none)
   int64_t drop_row0;         // row index of c's first row in the tensor the mask is defined on
-  int drop_nvec;             // 16-byte vectors per row of that tensor
+};
+
+struct GemmArgs {
+  int m, n;
+  int n_src;
+  int n_prob;
+  int kb_end[kMaxSrc];       // prefix sums of the k-blocks (of 128 bytes) of every source
+  int k_elems;               // elements per k-block
+  int out_bf16;              // 1: bf16 output, 0: fp32 output
+  int epi_slabs;             // 1 | 2 staging slabs per epilogue warp
+  int drop_nvec;             // 16-byte vectors per row of the tensor a dropout mask is defined on
+  GemmOut out[kMaxProb];
 };
 
 // Epilogue of one consumer warp: its 16 rows x NT columns of the accumulator.  This thread holds rows `row` and
 // `row + 8` (the layout in tc_common.cuh).  kOutBf16 ? bf16 : fp32 output.
 template <int NT, bool kOutBf16>
-__device__ __forceinline__ void epilogue_tma(const GemmMaps& maps, const GemmArgs& p, float (&acc)[NT / 2], const float* s_bias,
-                                             uint8_t* warp_slabs, uint32_t& ck, int row0, int lane, uint32_t drop_hi) {
+__device__ __forceinline__ void epilogue_tma(const CUtensorMap* map_c, const GemmArgs& p, const GemmOut& o,
+                                             float (&acc)[NT / 2], const float* s_bias, uint8_t* warp_slabs,
+                                             uint32_t& ck, int row0, int lane, uint32_t drop_hi) {
   constexpr int kCpc = kOutBf16 ? 64 : 32;                 // columns per 128-byte chunk
   const int q = lane & 3, rl = lane >> 2;                  // column pair and row inside the warp's 16 rows
+  // read once: `o` lives in parameter memory, which the compiler cannot tell apart from the slab stores below
+  const uint32_t thresh16 = o.drop.thresh16, seed_lo = o.drop.seed_lo;
+  const float drop_scale = o.drop.scale;
+  const int64_t drop_row0 = o.drop_row0;
   float scale[2];
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int row = row0 + rl + 8 * h;
-    scale[h] = (p.row_div != nullptr && row < p.m) ? 1.f / __ldg(p.row_div + row) : 1.f;
+    scale[h] = (o.row_div != nullptr && row < p.m) ? 1.f / __ldg(o.row_div + row) : 1.f;
   }
 #pragma unroll
   for (int ch = 0; ch < NT / kCpc; ++ch) {
@@ -93,15 +112,15 @@ __device__ __forceinline__ void epilogue_tma(const GemmMaps& maps, const GemmArg
         float v0 = (acc[4 * j + 2 * h] + b2.x) * scale[h];
         float v1 = (acc[4 * j + 2 * h + 1] + b2.y) * scale[h];
         const int r = rl + 8 * h;
-        if (p.drop.thresh16 != 0u) {
+        if (thresh16 != 0u) {
           // mask of the (rounded) output, per 16-byte vector: what pg_dropout_rows would make of c
-          const uint64_t ibase = static_cast<uint64_t>(p.drop_row0 + row0 + r) * p.drop_nvec;
+          const uint64_t ibase = static_cast<uint64_t>(drop_row0 + row0 + r) * p.drop_nvec;
           if (kOutBf16) {
             v0 = __bfloat162float(__float2bfloat16_rn(v0));
             v1 = __bfloat162float(__float2bfloat16_rn(v1));
-            drop_pair(v0, v1, ibase + (col >> 3), q, p.drop.thresh16, p.drop.scale, p.drop.seed_lo, drop_hi);
+            drop_pair(v0, v1, ibase + (col >> 3), q, thresh16, drop_scale, seed_lo, drop_hi);
           } else {
-            drop_pair(v0, v1, ibase + (col >> 2), q & 1, p.drop.thresh16, p.drop.scale, p.drop.seed_lo, drop_hi);
+            drop_pair(v0, v1, ibase + (col >> 2), q & 1, thresh16, drop_scale, seed_lo, drop_hi);
           }
         }
         // 128B swizzle of the slab: 16-byte chunk index XOR (row & 7)
@@ -116,7 +135,7 @@ __device__ __forceinline__ void epilogue_tma(const GemmMaps& maps, const GemmArg
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     __syncwarp();
     if (lane == 0) {
-      if (row0 < p.m) tma_store_2d(&maps.c, smem_u32(slab), c0, row0);
+      if (row0 < p.m) tma_store_2d(map_c, smem_u32(slab), c0, row0);
       // one group per chunk, empty or not: the slab parity (ck & 1) and the group count stay in step
       asm volatile("cp.async.bulk.commit_group;" ::: "memory");
     }
@@ -126,13 +145,14 @@ __device__ __forceinline__ void epilogue_tma(const GemmMaps& maps, const GemmArg
 
 // output rows that are not 16-byte aligned: plain stores from the accumulator registers
 template <int NT>
-__device__ __forceinline__ void epilogue_direct(const GemmArgs& p, float (&acc)[NT / 2], const float* s_bias, int row0, int lane) {
+__device__ __forceinline__ void epilogue_direct(const GemmArgs& p, const GemmOut& o, float (&acc)[NT / 2],
+                                                const float* s_bias, int row0, int lane) {
   const int q = lane & 3, rl = lane >> 2;
 #pragma unroll
   for (int h = 0; h < 2; ++h) {
     const int row = row0 + rl + 8 * h;
     if (row >= p.m) continue;
-    const float scale = p.row_div != nullptr ? 1.f / __ldg(p.row_div + row) : 1.f;
+    const float scale = o.row_div != nullptr ? 1.f / __ldg(o.row_div + row) : 1.f;
 #pragma unroll
     for (int j = 0; j < NT / 8; ++j) {
 #pragma unroll
@@ -140,8 +160,8 @@ __device__ __forceinline__ void epilogue_direct(const GemmArgs& p, float (&acc)[
         const int col = 8 * j + 2 * q + e;
         if (col >= p.n) continue;
         const float v = (acc[4 * j + 2 * h + e] + s_bias[col]) * scale;
-        if (p.out_bf16) static_cast<__nv_bfloat16*>(p.c)[static_cast<int64_t>(row) * p.ldc + col] = __float2bfloat16_rn(v);
-        else static_cast<float*>(p.c)[static_cast<int64_t>(row) * p.ldc + col] = v;
+        if (p.out_bf16) static_cast<__nv_bfloat16*>(o.c)[static_cast<int64_t>(row) * o.ldc + col] = __float2bfloat16_rn(v);
+        else static_cast<float*>(o.c)[static_cast<int64_t>(row) * o.ldc + col] = v;
       }
     }
   }
@@ -149,7 +169,7 @@ __device__ __forceinline__ void epilogue_direct(const GemmArgs& p, float (&acc)[
 
 template <bool kTf32, int NT>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-linear_wgmma_kernel(const __grid_constant__ GemmMaps maps, const GemmArgs p) {
+linear_wgmma_kernel(const __grid_constant__ GemmMaps maps, const __grid_constant__ GemmArgs p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte alignment of the swizzled tiles
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
@@ -164,15 +184,19 @@ linear_wgmma_kernel(const __grid_constant__ GemmMaps maps, const GemmArgs p) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int n_tiles = (p.m + kBlockM - 1) / kBlockM;
   const int kb_total = p.kb_end[p.n_src - 1];
+  const int prob = blockIdx.x % p.n_prob;                   // this CTA's problem (gridDim.x is a multiple of n_prob)
+  const int tile0 = blockIdx.x / p.n_prob, tile_step = gridDim.x / p.n_prob;
+  const GemmOut& o = p.out[prob];
+  const CUtensorMap* map_b = maps.b + prob * p.n_src;
 
   if (warp == 0 && lane == 0) {
     for (int s = 0; s < p.n_src; ++s) {
       asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&maps.a[s])) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&maps.b[s])) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map_b + s)) : "memory");
     }
   }
   for (int i = threadIdx.x; i < 256; i += kGemmThreads)
-    s_bias[i] = (p.bias != nullptr && i < p.n) ? __ldg(p.bias + i) : 0.f;
+    s_bias[i] = (o.bias != nullptr && i < p.n) ? __ldg(o.bias + i) : 0.f;
   if (warp == 1 && lane == 0) {
     for (int s = 0; s < kStages; ++s) {
       mbar_init(smem_u32(full_bar + s), 1);
@@ -188,7 +212,7 @@ linear_wgmma_kernel(const __grid_constant__ GemmMaps maps, const GemmArgs p) {
     if (warp == 0 && lane == 0) {
       int stage = 0;
       uint32_t phase = 0;
-      for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+      for (int tile = tile0; tile < n_tiles; tile += tile_step) {
         const int m0 = tile * kBlockM;
         int src = 0, kb_begin = 0;
         for (int kb = 0; kb < kb_total; ++kb) {
@@ -199,7 +223,7 @@ linear_wgmma_kernel(const __grid_constant__ GemmMaps maps, const GemmArgs p) {
           const uint32_t sa = smem_u32(smem + stage * kStageBytes);
           const uint32_t sb = sa + kABytes;
           tma_load_2d(sa, &maps.a[src], fb, (kb - kb_begin) * p.k_elems, m0);
-          tma_load_2d(sb, &maps.b[src], fb, (kb - kb_begin) * p.k_elems, 0);
+          tma_load_2d(sb, map_b + src, fb, (kb - kb_begin) * p.k_elems, 0);
           if (++stage == kStages) { stage = 0; phase ^= 1; }
         }
       }
@@ -210,12 +234,13 @@ linear_wgmma_kernel(const __grid_constant__ GemmMaps maps, const GemmArgs p) {
     const int wg = (warp >> 2) - 1;                          // 0 | 1: rows [64 wg, 64 wg + 64) of the tile
     const int cw = warp - 4;                                 // consumer warp 0..7: rows [16 cw, 16 cw + 16)
     uint8_t* warp_slabs = slabs + cw * 2 * kSlabBytes;
-    const uint32_t drop_hi = drop_seed_hi(p.drop);
+    const uint32_t drop_hi = drop_seed_hi(o.drop);
+    const int tma_store = o.tma_store;
     int stage = 0;
     uint32_t phase = 0;
     uint32_t ck = 0;                                         // chunks stored by this warp
     float acc[NT / 2];
-    for (int tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+    for (int tile = tile0; tile < n_tiles; tile += tile_step) {
       int prev = -1;                                         // stage whose MMAs are still in flight
       for (int kb = 0; kb < kb_total; ++kb) {
         mbar_wait(smem_u32(full_bar + stage), phase);
@@ -244,14 +269,14 @@ linear_wgmma_kernel(const __grid_constant__ GemmMaps maps, const GemmArgs p) {
       fence_accum(acc);
       if (lane == 0 && prev >= 0) mbar_arrive(smem_u32(empty_bar + prev));
       const int row0 = tile * kBlockM + cw * kSlabRows;
-      if (p.tma_store) {
-        if (p.out_bf16) epilogue_tma<NT, true>(maps, p, acc, s_bias, warp_slabs, ck, row0, lane, drop_hi);
-        else epilogue_tma<NT, false>(maps, p, acc, s_bias, warp_slabs, ck, row0, lane, drop_hi);
+      if (tma_store) {
+        if (p.out_bf16) epilogue_tma<NT, true>(&maps.c[prob], p, o, acc, s_bias, warp_slabs, ck, row0, lane, drop_hi);
+        else epilogue_tma<NT, false>(&maps.c[prob], p, o, acc, s_bias, warp_slabs, ck, row0, lane, drop_hi);
       } else {
-        epilogue_direct<NT>(p, acc, s_bias, row0, lane);
+        epilogue_direct<NT>(p, o, acc, s_bias, row0, lane);
       }
     }
-    if (p.tma_store && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
+    if (tma_store && lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
   }
 }
 
@@ -308,13 +333,25 @@ extern "C" int pg_linear(int dtype_in, int dtype_out, const pg_gemm_src* srcs, i
 extern "C" int pg_linear_drop(int dtype_in, int dtype_out, const pg_gemm_src* srcs, int32_t n_src, const float* bias,
                               const float* row_div, void* c, int64_t ldc, int32_t m, int32_t n, const pg_drop* drop,
                               int64_t drop_row0, void* stream) {
+  const pg_gemm_out out{bias, row_div, c, ldc, drop, drop_row0};
+  return pg_linear_group(dtype_in, dtype_out, srcs, n_src, 1, &out, m, n, stream);
+}
+
+extern "C" int pg_linear_group(int dtype_in, int dtype_out, const pg_gemm_src* srcs, int32_t n_src, int32_t n_prob,
+                               const pg_gemm_out* outs, int32_t m, int32_t n, void* stream) {
   using namespace pg;
-  PG_REQUIRE(srcs && c, "pg_linear: null operand");
+  PG_REQUIRE(srcs && outs, "pg_linear: null operand");
   PG_REQUIRE(n_src >= 1 && n_src <= kMaxSrc, "pg_linear: 1..%d operand pairs, got %d", kMaxSrc, n_src);
+  PG_REQUIRE(n_prob >= 1 && n_prob <= kMaxProb && n_prob * n_src <= kMaxB,
+             "pg_linear_group: 1..%d problems of at most %d operand pairs in all, got %d x %d", kMaxProb, kMaxB, n_prob,
+             n_src);
   PG_REQUIRE(m >= 0 && n > 0 && n <= 256, "pg_linear: unsupported shape m=%d n=%d (n <= 256)", m, n);
   PG_REQUIRE(dtype_in == PG_F32 || dtype_in == PG_BF16, "pg_linear: bad input dtype");
   PG_REQUIRE(dtype_out == PG_F32 || dtype_out == PG_BF16, "pg_linear: bad output dtype");
-  PG_REQUIRE(ldc >= n, "pg_linear: ldc < n");
+  for (int q = 0; q < n_prob; ++q) {
+    PG_REQUIRE(outs[q].c, "pg_linear: null output %d", q);
+    PG_REQUIRE(outs[q].ldc >= n, "pg_linear: ldc < n");
+  }
   if (m == 0) return PG_OK;
   const bool tf32 = dtype_in == PG_F32;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
@@ -323,46 +360,66 @@ extern "C" int pg_linear_drop(int dtype_in, int dtype_out, const pg_gemm_src* sr
   p.m = m; p.n = n;
   const int nt = tile_n(n);
   p.n_src = n_src;
+  p.n_prob = n_prob;
   p.k_elems = kRowBytes / (tf32 ? 4 : 2);
   int kb = 0, rc;
   for (int s = 0; s < kMaxSrc; ++s) {
     if (s < n_src) {
-      PG_REQUIRE(srcs[s].a && srcs[s].b && srcs[s].k > 0, "pg_linear: operand pair %d is empty", s);
+      PG_REQUIRE(srcs[s].a && srcs[s].k > 0, "pg_linear: operand pair %d is empty", s);
       kb += (srcs[s].k + p.k_elems - 1) / p.k_elems;
       if ((rc = make_map(&maps.a[s], srcs[s].a, srcs[s].lda, m, srcs[s].k, kBlockM, tf32)) != PG_OK) return rc;
-      if ((rc = make_map(&maps.b[s], srcs[s].b, srcs[s].ldb, n, srcs[s].k, nt, tf32)) != PG_OK) return rc;
     } else {
       maps.a[s] = maps.a[0];
-      maps.b[s] = maps.b[0];
     }
     p.kb_end[s] = kb;
   }
-  p.bias = bias; p.row_div = row_div; p.c = c; p.ldc = ldc; p.out_bf16 = dtype_out == PG_BF16;
-  {
+  for (int i = 0; i < kMaxB; ++i) {
+    if (i < n_prob * n_src) {
+      const pg_gemm_src& src = srcs[i];
+      const pg_gemm_src& first = srcs[i % n_src];
+      PG_REQUIRE(src.b, "pg_linear: operand pair %d is empty", i);
+      PG_REQUIRE(src.a == first.a && src.lda == first.lda && src.k == first.k,
+                 "pg_linear_group: problem %d, pair %d does not share problem 0's A operand", i / n_src, i % n_src);
+      if ((rc = make_map(&maps.b[i], src.b, src.ldb, n, src.k, nt, tf32)) != PG_OK) return rc;
+    } else {
+      maps.b[i] = maps.b[0];
+    }
+  }
+  p.out_bf16 = dtype_out == PG_BF16;
+  p.epi_slabs = g_gemm_epi_slabs;
+  const int eso = p.out_bf16 ? 2 : 4;
+  p.drop_nvec = static_cast<int>(round_up(n, p.out_bf16 ? 8 : 4) / (p.out_bf16 ? 8 : 4));
+  for (int q = 0; q < kMaxProb; ++q) {
+    GemmOut& o = p.out[q];
+    if (q >= n_prob) {
+      o = p.out[0];
+      maps.c[q] = maps.c[0];
+      continue;
+    }
+    const pg_gemm_out& in = outs[q];
+    o.bias = in.bias; o.row_div = in.row_div; o.c = in.c; o.ldc = in.ldc;
     // TMA-store epilogue when the output rows are 16-byte aligned (always true for engine buffers)
-    const int eso = p.out_bf16 ? 2 : 4;
-    p.tma_store = ((reinterpret_cast<uintptr_t>(c) & 15) == 0 && (ldc * eso) % 16 == 0) ? 1 : 0;
-    p.epi_slabs = g_gemm_epi_slabs;
-    if (p.tma_store) {
+    o.tma_store = ((reinterpret_cast<uintptr_t>(in.c) & 15) == 0 && (in.ldc * eso) % 16 == 0) ? 1 : 0;
+    if (o.tma_store) {
       EncodeTiledFn enc = get_encode();
       cuuint64_t gdim[2] = {static_cast<cuuint64_t>(n), static_cast<cuuint64_t>(m)};
-      cuuint64_t gstride[1] = {static_cast<cuuint64_t>(ldc) * eso};
+      cuuint64_t gstride[1] = {static_cast<cuuint64_t>(in.ldc) * eso};
       cuuint32_t box[2] = {static_cast<cuuint32_t>(kRowBytes / eso), kSlabRows};
       cuuint32_t estr[2] = {1, 1};
-      CUresult r = enc(&maps.c, p.out_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, c,
-                       gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
+      CUresult r = enc(&maps.c[q], p.out_bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2,
+                       in.c, gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                        CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
       if (r != CUDA_SUCCESS) { set_error("cuTensorMapEncodeTiled(output) failed (%d)", (int)r); return PG_ERR_CUDA; }
     } else {
-      maps.c = maps.a[0];
+      maps.c[q] = maps.a[0];
     }
+    o.drop = make_drop(in.drop);
+    o.drop_row0 = in.drop_row0;
+    PG_REQUIRE(o.drop.thresh16 == 0u || o.tma_store, "pg_linear_drop: the fused dropout needs 16-byte aligned output rows");
   }
-  p.drop = make_drop(drop);
-  p.drop_row0 = drop_row0;
-  p.drop_nvec = static_cast<int>(round_up(n, p.out_bf16 ? 8 : 4) / (p.out_bf16 ? 8 : 4));
-  PG_REQUIRE(p.drop.thresh16 == 0u || p.tma_store, "pg_linear_drop: the fused dropout needs 16-byte aligned output rows");
+  // a multiple of n_prob CTAs: CTA b serves problem b % n_prob only, and the n_prob CTAs of one M tile are adjacent
   const int n_tiles = (m + kBlockM - 1) / kBlockM;
-  const int grid = std::min(n_tiles, sm_count());
+  const int grid = std::min(n_tiles, std::max(1, sm_count() / n_prob)) * n_prob;
   const size_t smem = static_cast<size_t>(kStages) * (kABytes + nt * kRowBytes) + kSlabsTotal /*staging*/ +
                       1024 /*bias*/ + 256 /*barriers*/ + 1024 /*align*/;
   return tf32 ? launch_linear<true>(nt, grid, smem, st, maps, p) : launch_linear<false>(nt, grid, smem, st, maps, p);

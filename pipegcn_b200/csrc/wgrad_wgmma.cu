@@ -14,6 +14,11 @@
 // accumulator is what the registers of two warpgroups hold), accumulates its partial D and writes it to a workspace;
 // a second kernel sums the partials in split order (deterministic).  With n > 128 the two CTAs of a row range read
 // the same X rows at the same time, the second one from L2.
+// Grouped form: up to kWgMaxProb products of the same n x k shape in one launch, each with its own rows, split-K
+// partition and workspace.  CTA order: row slice (split) slowest, then the 128-output tile, then the product, so the
+// CTAs of all products over one row slice run side by side and an operand they share (g of g^T x and g^T ah) comes
+// from HBM once.  Every CTA computes what it computes in a lone launch; the reduction sums each product's partials
+// in split order, so the bits are those of separate launches.
 //   warpgroup 0: TMA producer (one thread)   warpgroups 1-2: wgmma m64nNTk16 on 64 outputs each, then the store
 #include <algorithm>
 
@@ -28,24 +33,34 @@ constexpr int kWgRows = 64;              // rows of m per pipeline stage
 constexpr int kWgBox = kWgRows * 128;    // bytes of one TMA box: 64 elements of n or k x 64 rows of m
 constexpr int kWgTileN = 128;            // outputs (rows of D) per CTA
 constexpr int kWgMaxSplits = 132;
+constexpr int kWgMaxProb = 2;
 
 struct WgradMaps {
-  CUtensorMap a[kWgMaxSrc];   // G_s: dims {n, m}, box {128 B of n, 64 rows}
-  CUtensorMap b[kWgMaxSrc];   // X_s: dims {k, m}, box {128 B of k, 64 rows}
+  CUtensorMap a[kWgMaxProb * kWgMaxSrc];   // G_{q,s} at q * n_src + s: dims {n, m}, box {128 B of n, 64 rows}
+  CUtensorMap b[kWgMaxProb * kWgMaxSrc];   // X_{q,s}: dims {k, m}, box {128 B of k, 64 rows}
+};
+
+struct WgradProb {
+  int m;
+  int splits;
+  int rows_per_split;        // multiple of kWgRows
+  float* partial;            // [splits][rows_pad][k_pad]
+  float* out;
+  int64_t ldo;
 };
 
 struct WgradArgs {
-  int m;
   int n_src;
+  int n_prob;
+  int n_tiles;               // 128-output tiles of D
   int k_pad;                 // row length of the partials: k rounded up to 16
-  int rows_pad;              // rows of one partial: gridDim.y * 128
-  int rows_per_split;        // multiple of kWgRows
-  float* partial;            // [splits][rows_pad][k_pad]
+  int rows_pad;              // rows of one partial: n_tiles * 128
+  WgradProb prob[kWgMaxProb];
 };
 
 template <int NT>
 __global__ void __launch_bounds__(kWgThreads, 1)
-wgrad_wgmma_kernel(const __grid_constant__ WgradMaps maps, const WgradArgs p) {
+wgrad_wgmma_kernel(const __grid_constant__ WgradMaps maps, const __grid_constant__ WgradArgs p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   constexpr int kABytes = (kWgTileN / 64) * kWgBox, kBBytes = (NT / 64) * kWgBox;
@@ -55,16 +70,23 @@ wgrad_wgmma_kernel(const __grid_constant__ WgradMaps maps, const WgradArgs p) {
   uint64_t* empty_bar = bars + kWgStages;    // [kWgStages]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int row_begin = blockIdx.x * p.rows_per_split;
-  const int row_end = min(p.m, row_begin + p.rows_per_split);
+  // blockIdx.x = (split * n_tiles + tile) * n_prob + problem
+  const int qi = blockIdx.x % p.n_prob, rest = blockIdx.x / p.n_prob;
+  const int split = rest / p.n_tiles;
+  const WgradProb& pr = p.prob[qi];
+  if (split >= pr.splits) return;                           // a product with fewer row slices than the largest
+  const CUtensorMap* map_a = maps.a + qi * p.n_src;
+  const CUtensorMap* map_b = maps.b + qi * p.n_src;
+  const int row_begin = split * pr.rows_per_split;
+  const int row_end = min(pr.m, row_begin + pr.rows_per_split);
   const int n_kb = row_end > row_begin ? (row_end - row_begin + kWgRows - 1) / kWgRows : 0;
   const int total_it = n_kb * p.n_src;
-  const int n0 = blockIdx.y * kWgTileN;
+  const int n0 = (rest - split * p.n_tiles) * kWgTileN;
 
   if (warp == 0 && lane == 0) {
     for (int s = 0; s < p.n_src; ++s) {
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&maps.a[s])) : "memory");
-      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&maps.b[s])) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map_a + s)) : "memory");
+      asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(map_b + s)) : "memory");
     }
   }
   if (warp == 1 && lane == 0) {
@@ -89,8 +111,8 @@ wgrad_wgmma_kernel(const __grid_constant__ WgradMaps maps, const WgradArgs p) {
         mbar_expect_tx(fb, static_cast<uint32_t>(kStageBytes));
         const uint32_t sa = smem_u32(smem + stage * kStageBytes);
         const uint32_t sb = sa + kABytes;
-        for (int blk = 0; blk < kWgTileN / 64; ++blk) tma_load_2d(sa + blk * kWgBox, &maps.a[src], fb, n0 + blk * 64, m0);
-        for (int blk = 0; blk < NT / 64; ++blk) tma_load_2d(sb + blk * kWgBox, &maps.b[src], fb, blk * 64, m0);
+        for (int blk = 0; blk < kWgTileN / 64; ++blk) tma_load_2d(sa + blk * kWgBox, map_a + src, fb, n0 + blk * 64, m0);
+        for (int blk = 0; blk < NT / 64; ++blk) tma_load_2d(sb + blk * kWgBox, map_b + src, fb, blk * 64, m0);
         if (++stage == kWgStages) { stage = 0; phase ^= 1; }
       }
     }
@@ -128,7 +150,7 @@ wgrad_wgmma_kernel(const __grid_constant__ WgradMaps maps, const WgradArgs p) {
     // this thread's rows of D (accumulator layout in tc_common.cuh), all 128 rows of the tile are written
     const int q = lane & 3;
     const int row = n0 + (warp - 4) * 16 + (lane >> 2);
-    float* out = p.partial + (static_cast<int64_t>(blockIdx.x) * p.rows_pad + row) * p.k_pad;
+    float* out = pr.partial + (static_cast<int64_t>(split) * p.rows_pad + row) * p.k_pad;
 #pragma unroll
     for (int j = 0; j < NT / 8; ++j) {
       const int col = 8 * j + 2 * q;
@@ -140,15 +162,19 @@ wgrad_wgmma_kernel(const __grid_constant__ WgradMaps maps, const WgradArgs p) {
   }
 }
 
-// out[n, k] = sum over splits of partial[split][n][k], in split order (eight partials in flight per thread)
+// out[n, k] = sum over splits of partial[split][n][k], in split order (eight partials in flight per thread);
+// blockIdx.y = product
 __global__ void __launch_bounds__(256)
-wgrad_reduce_kernel(const float* __restrict__ partial, int splits, int rows_pad, int k_pad, float* __restrict__ out,
-                    int64_t ldo, int n, int k) {
+wgrad_reduce_kernel(const __grid_constant__ WgradArgs a, int n, int k) {
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= n * k) return;
+  const WgradProb& q = a.prob[blockIdx.y];
+  const int splits = q.splits;
+  float* __restrict__ out = q.out;
+  const int64_t ldo = q.ldo;
   const int r = idx / k, c = idx % k;
-  const float* p = partial + static_cast<int64_t>(r) * k_pad + c;
-  const int64_t stride = static_cast<int64_t>(rows_pad) * k_pad;
+  const float* p = q.partial + static_cast<int64_t>(r) * a.k_pad + c;
+  const int64_t stride = static_cast<int64_t>(a.rows_pad) * a.k_pad;
   float s = 0.f;
   int sp = 0;
   for (; sp + 8 <= splits; sp += 8) {
@@ -196,7 +222,7 @@ static int wgrad_max_splits(int n_tiles, bool query_device) {
 }
 
 template <int NT>
-static int launch_wgrad(dim3 grid, cudaStream_t st, const WgradMaps& maps, const WgradArgs& p) {
+static int launch_wgrad(int grid, cudaStream_t st, const WgradMaps& maps, const WgradArgs& p) {
   const size_t smem = static_cast<size_t>(kWgStages) * (kWgTileN / 64 + NT / 64) * kWgBox + 256 /*barriers*/ + 1024 /*align*/;
   static bool attr_set = false;       // once: opt in to the full 227 KB of shared memory (not a stream operation)
   if (!attr_set) {
@@ -221,44 +247,66 @@ extern "C" int64_t pg_wgrad_workspace(int32_t m, int32_t n, int32_t k, int dtype
 
 extern "C" int pg_wgrad(int dtype_in, const pg_gemm_src* srcs, int32_t n_src, float* out, int64_t ldo, int32_t m,
                         int32_t n, int32_t k, float* workspace, int64_t workspace_floats, void* stream) {
+  const pg_wgrad_out o{out, ldo, m, workspace, workspace_floats};
+  return pg_wgrad_group(dtype_in, srcs, n_src, 1, &o, n, k, stream);
+}
+
+extern "C" int pg_wgrad_group(int dtype_in, const pg_gemm_src* srcs, int32_t n_src, int32_t n_prob,
+                              const pg_wgrad_out* outs, int32_t n, int32_t k, void* stream) {
   using namespace pg;
-  PG_REQUIRE(srcs && out, "pg_wgrad: null operand");
+  PG_REQUIRE(srcs && outs, "pg_wgrad: null operand");
   PG_REQUIRE(n_src >= 1 && n_src <= kWgMaxSrc, "pg_wgrad: 1..%d operand pairs, got %d", kWgMaxSrc, n_src);
-  PG_REQUIRE(m >= 0 && n > 0 && n <= 256 && k > 0 && k <= 256, "pg_wgrad: unsupported shape m=%d n=%d k=%d (n, k <= 256)", m, n, k);
+  PG_REQUIRE(n_prob >= 1 && n_prob <= kWgMaxProb, "pg_wgrad_group: 1..%d products, got %d", kWgMaxProb, n_prob);
+  PG_REQUIRE(n > 0 && n <= 256 && k > 0 && k <= 256, "pg_wgrad: unsupported shape n=%d k=%d (n, k <= 256)", n, k);
   if (dtype_in != PG_BF16) {
     set_error("pg_wgrad: bf16 operands only (the tensor core transposes 16-bit operands only); pass fp32 as bf16 terms");
     return PG_ERR_UNSUPPORTED;
   }
-  PG_REQUIRE(ldo >= k, "pg_wgrad: ldo < k");
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (m == 0) {
-    PG_CHECK_CUDA(cudaMemset2DAsync(out, ldo * sizeof(float), 0, k * sizeof(float), n, st));
-    return PG_OK;
-  }
   WgradArgs p;
   WgradMaps maps;
   const int n_tiles = (n + kWgTileN - 1) / kWgTileN;
-  p.m = m; p.n_src = n_src;
+  p.n_src = n_src;
+  p.n_tiles = n_tiles;
   p.k_pad = static_cast<int>(round_up(k, 16));
   p.rows_pad = n_tiles * kWgTileN;
-  const int splits = wgrad_splits(m, wgrad_max_splits(n_tiles, true), &p.rows_per_split);
-  const int64_t need = static_cast<int64_t>(splits) * p.rows_pad * p.k_pad;
-  PG_REQUIRE(workspace != nullptr && workspace_floats >= need,
-             "pg_wgrad: workspace too small (%lld floats, need %lld: pg_wgrad_workspace)", (long long)workspace_floats,
-             (long long)need);
-  p.partial = workspace;
-  int rc;
-  for (int s = 0; s < kWgMaxSrc; ++s) {
-    if (s < n_src) {
-      PG_REQUIRE(srcs[s].a && srcs[s].b, "pg_wgrad: operand pair %d is empty", s);
-      if ((rc = make_mn_map(&maps.a[s], srcs[s].a, srcs[s].lda, m, n)) != PG_OK) return rc;
-      if ((rc = make_mn_map(&maps.b[s], srcs[s].b, srcs[s].ldb, m, k)) != PG_OK) return rc;
-    } else {
-      maps.a[s] = maps.a[0];
-      maps.b[s] = maps.b[0];
+  const int max_splits = wgrad_max_splits(n_tiles, true);
+  int np = 0, splits_max = 0, rc;
+  for (int i = 0; i < n_prob; ++i) {
+    const pg_wgrad_out& o = outs[i];
+    PG_REQUIRE(o.out && o.m >= 0, "pg_wgrad: bad output %d", i);
+    PG_REQUIRE(o.ldo >= k, "pg_wgrad: ldo < k");
+    if (o.m == 0) {                                       // no rows: the gradient is zero
+      PG_CHECK_CUDA(cudaMemset2DAsync(o.out, o.ldo * sizeof(float), 0, k * sizeof(float), n, st));
+      continue;
     }
+    WgradProb& q = p.prob[np];
+    q.m = o.m;
+    q.splits = wgrad_splits(o.m, max_splits, &q.rows_per_split);
+    const int64_t need = static_cast<int64_t>(q.splits) * p.rows_pad * p.k_pad;
+    PG_REQUIRE(o.workspace != nullptr && o.workspace_floats >= need,
+               "pg_wgrad: workspace too small (%lld floats, need %lld: pg_wgrad_workspace)", (long long)o.workspace_floats,
+               (long long)need);
+    q.partial = o.workspace;
+    q.out = o.out;
+    q.ldo = o.ldo;
+    for (int s = 0; s < n_src; ++s) {
+      const pg_gemm_src& src = srcs[i * n_src + s];
+      PG_REQUIRE(src.a && src.b, "pg_wgrad: operand pair %d of product %d is empty", s, i);
+      if ((rc = make_mn_map(&maps.a[np * n_src + s], src.a, src.lda, o.m, n)) != PG_OK) return rc;
+      if ((rc = make_mn_map(&maps.b[np * n_src + s], src.b, src.ldb, o.m, k)) != PG_OK) return rc;
+    }
+    splits_max = std::max(splits_max, q.splits);
+    ++np;
   }
-  const dim3 grid(splits, n_tiles);
+  if (np == 0) return PG_OK;
+  p.n_prob = np;
+  for (int i = np; i < kWgMaxProb; ++i) p.prob[i] = p.prob[0];
+  for (int i = np * n_src; i < kWgMaxProb * kWgMaxSrc; ++i) {
+    maps.a[i] = maps.a[0];
+    maps.b[i] = maps.b[0];
+  }
+  const int grid = splits_max * n_tiles * np;
   switch (tile_n(k)) {
     case 64: rc = launch_wgrad<64>(grid, st, maps, p); break;
     case 128: rc = launch_wgrad<128>(grid, st, maps, p); break;
@@ -267,7 +315,7 @@ extern "C" int pg_wgrad(int dtype_in, const pg_gemm_src* srcs, int32_t n_src, fl
   }
   if (rc != PG_OK) return rc;
   const int total = n * k;
-  wgrad_reduce_kernel<<<(total + 255) / 256, 256, 0, st>>>(workspace, splits, p.rows_pad, p.k_pad, out, ldo, n, k);
+  wgrad_reduce_kernel<<<dim3((total + 255) / 256, np), 256, 0, st>>>(p, n, k);
   PG_LAUNCH_CHECK();
   return PG_OK;
 }

@@ -445,54 +445,78 @@ def gemm_nt(a0, b0, a1=None, b1=None, bias=None, row_div=None, out=None, out_dty
     """out[m, n] = a0 @ b0^T (+ a1 @ b1^T) (+ bias) (/ row_div[:, None]) on the tensor cores.  Operands may be
     `Split` objects (fp32 operands split once by the caller).  `drop`: dropout mask applied to `out` as it is written
     (out's first row is row `drop_row0` of the tensor the mask is defined on)."""
-    raw = [(a0, b0)] + ([(a1, b1)] if a1 is not None else [])
-    a0, b0 = _plain(a0), _plain(b0)
-    pairs = [(_rows(_plain(a)), _rows(_plain(b))) for a, b in raw]
-    m, n = a0.shape[0], b0.shape[0]
-    for a, b in pairs:
-        assert a.shape[0] == m and b.shape[0] == n and a.shape[1] == b.shape[1] and a.dtype == b.dtype == a0.dtype
+    a, b = ([a0, a1], [b0, b1]) if a1 is not None else ([a0], [b0])
+    return _gemm(a, [dict(b=b, bias=bias, row_div=row_div, out=out, drop=drop, drop_row0=drop_row0)], out_dtype)[0]
+
+
+def gemm_nt_group(a, bs, row_divs=None, outs=None, out_dtype=None) -> list:
+    """[a @ b^T (/ row_div[:, None]) for b in bs] (at most four products of the same width) in ONE launch: the
+    products share their A operand, and the CTAs that multiply the same rows of it run together, so `a` is read from
+    HBM once for all of them.  Each output has the bits of its own `gemm_nt` call."""
+    row_divs = row_divs or [None] * len(bs)
+    outs = outs or [None] * len(bs)
+    return _gemm([a], [dict(b=[b], bias=None, row_div=r, out=o, drop=None, drop_row0=0)
+                       for b, r, o in zip(bs, row_divs, outs)], out_dtype)
+
+
+def _gemm(raw_a, probs, out_dtype):
+    """pg_linear_group: every problem (dict of b, bias, row_div, out, drop, drop_row0) multiplies the A operands
+    `raw_a` by its own B operands."""
+    a0 = _plain(raw_a[0])
+    m, n = a0.shape[0], _plain(probs[0]["b"][0]).shape[0]
+    for pr in probs:
+        for a, b in zip(raw_a, pr["b"]):
+            a, b = _rows(_plain(a)), _rows(_plain(b))
+            assert a.shape[0] == m and b.shape[0] == n and a.shape[1] == b.shape[1] and a.dtype == b.dtype == a0.dtype
+    outs = []
+    for pr in probs:
+        out = pr["out"]
+        if out is None:
+            out = alloc_rows(m, n, out_dtype or a0.dtype, a0.device)
+        assert out.shape == (m, n) and out.stride(1) == 1 and out.dtype == (outs[0].dtype if outs else out.dtype)
+        outs.append(out)
     if n > 256:
         # one N tile holds at most 256 columns: split the weight rows, each product writing its 256-column slice of
         # one output (padded rows like every other output: 16-byte aligned, usable by the row kernels and TMA)
-        assert drop is None or drop.p == 0, "fused dropout with n > 256 is not supported"
-        if out is None:
-            out = alloc_rows(m, n, out_dtype or a0.dtype, a0.device)
-        assert out.shape == (m, n) and out.stride(1) == 1
+        assert all(pr["drop"] is None or pr["drop"].p == 0 for pr in probs), "fused dropout with n > 256 is not supported"
         for i in range(0, n, 256):
-            gemm_nt(raw[0][0], b0[i:i + 256], raw[1][0] if len(raw) > 1 else None,
-                    None if len(raw) == 1 else _plain(raw[1][1])[i:i + 256],
-                    None if bias is None else bias[i:i + 256], row_div, out[:, i:i + 256], out_dtype)
-        return out
-    if out is None:
-        out = alloc_rows(m, n, out_dtype or a0.dtype, a0.device)
-    assert out.shape == (m, n) and out.stride(1) == 1
+            _gemm(raw_a, [dict(pr, b=[_plain(b)[i:i + 256] for b in pr["b"]], out=out[:, i:i + 256], drop=None,
+                               bias=None if pr["bias"] is None else pr["bias"][i:i + 256])
+                          for pr, out in zip(probs, outs)], out_dtype)
+        return outs
     if m == 0:
-        return out
+        return outs
     if a0.dtype == torch.float32 and FP32_GEMM == "3xtf32":
-        split = []
-        for a, b in raw:
-            (ah, al), (bh, bl) = _halves(a), _halves(b)
-            split += [(ah, bh), (ah, bl), (al, bh)]
-        pairs = split
+        a_halves = [_halves(a) for a in raw_a]
+        pairs = []
+        for pr in probs:
+            for (ah, al), b in zip(a_halves, pr["b"]):
+                bh, bl = _halves(b)
+                pairs += [(ah, bh), (ah, bl), (al, bh)]
     else:
-        pairs = [(_tma_ready(a), _tma_ready(b)) for a, b in pairs]
+        a_ready = [_tma_ready(_rows(_plain(a))) for a in raw_a]
+        pairs = [(a, _tma_ready(_rows(_plain(b)))) for pr in probs for a, b in zip(a_ready, pr["b"])]
     srcs = (_C.pg_gemm_src * len(pairs))(*[_C.pg_gemm_src(a.data_ptr(), a.stride(0), b.data_ptr(), b.stride(0),
                                                             a.shape[1]) for a, b in pairs])
-    if bias is not None:
-        bias = bias.detach().to(torch.float32).contiguous()
+    keep, couts = [], []
+    for pr, out in zip(probs, outs):
+        bias, drop = pr["bias"], pr["drop"]
+        if bias is not None:
+            bias = bias.detach().to(torch.float32).contiguous()
+            keep.append(bias)
+        dc = None
+        if drop is not None and drop.p > 0:
+            dc = drop.c()
+            keep.append(dc)
+        couts.append(_C.pg_gemm_out(bias.data_ptr() if bias is not None else None,
+                                    pr["row_div"].data_ptr() if pr["row_div"] is not None else None,
+                                    out.data_ptr(), out.stride(0), C.addressof(dc) if dc is not None else None,
+                                    int(pr["drop_row0"])))
     _C.count()
-    if drop is not None and drop.p > 0:
-        _C.check(_C.lib.pg_linear_drop(_C.dtype_code(a0.dtype), _C.dtype_code(out.dtype), srcs, len(pairs),
-                                       bias.data_ptr() if bias is not None else None,
-                                       row_div.data_ptr() if row_div is not None else None,
-                                       out.data_ptr(), out.stride(0), m, n, C.byref(drop.c()), int(drop_row0),
-                                       _C.stream_ptr()), "pg_linear_drop")
-        return out
-    _C.check(_C.lib.pg_linear(_C.dtype_code(a0.dtype), _C.dtype_code(out.dtype), srcs, len(pairs),
-                              bias.data_ptr() if bias is not None else None,
-                              row_div.data_ptr() if row_div is not None else None,
-                              out.data_ptr(), out.stride(0), m, n, _C.stream_ptr()), "pg_linear")
-    return out
+    _C.check(_C.lib.pg_linear_group(_C.dtype_code(a0.dtype), _C.dtype_code(outs[0].dtype), srcs,
+                                    len(pairs) // len(probs), len(probs), (_C.pg_gemm_out * len(couts))(*couts), m, n,
+                                    _C.stream_ptr()), "pg_linear_group")
+    return outs
 
 
 def _split_bf16(x: torch.Tensor, terms: int):
@@ -511,38 +535,70 @@ def wgrad(g: torch.Tensor, x: torch.Tensor) -> torch.Tensor:
     """g^T @ x  -> fp32 [n, k]: the weight gradient of `x @ W^T` on the tensor cores (pg_wgrad: MN-major bf16
     operands straight from the row-major activations, split-K over the rows, fixed-order reduction).  The tensor core
     transposes 16-bit operands only, so fp32 activations go in as sums of bf16 terms."""
-    g, x = _rows(_plain(g)), _rows(_plain(x))
-    m, n, k = g.shape[0], g.shape[1], x.shape[1]
-    assert x.shape[0] == m and g.dtype == x.dtype
-    out = torch.empty(n, k, dtype=torch.float32, device=g.device)
-    if m == 0:
-        return out.zero_()
-    if g.dtype == torch.float32 and FP32_GEMM == "3xtf32":
-        # fp32 = b0 + b1 + b2 exactly (three bf16 terms): six bf16 products carry the product to ~2^-24
-        g3, x3 = _split_bf16(g, 3), _split_bf16(x, 3)
-        pairs = [(g3[0], x3[0]), (g3[0], x3[1]), (g3[1], x3[0]), (g3[0], x3[2]), (g3[2], x3[0]), (g3[1], x3[1])]
-    elif g.dtype == torch.float32:
-        # one-pass mode: two bf16 terms, three products (~2^-16, finer than one tf32 pass)
-        g2, x2 = _split_bf16(g, 2), _split_bf16(x, 2)
-        pairs = [(g2[0], x2[0]), (g2[0], x2[1]), (g2[1], x2[0])]
-    else:
-        pairs = [(_tma_ready(g), _tma_ready(x))]
-    code = _C.dtype_code(pairs[0][0].dtype)
+    return wgrad_group([(g, x)])[0]
+
+
+def wgrad_group(pairs) -> list:
+    """[g^T @ x for g, x in pairs] (one or two products of the same n and k; the rows may differ) with the products
+    in ONE launch per 256 x 256 block of the output (pg_wgrad_group): the CTAs of both products over the same rows run
+    together, so an operand they share is read from HBM once.  Each output has the bits of its own `wgrad` call."""
+    assert 1 <= len(pairs) <= 2
+    ps = [(_rows(_plain(g)), _rows(_plain(x))) for g, x in pairs]
+    n, k, dt = ps[0][0].shape[1], ps[0][1].shape[1], ps[0][0].dtype
+    for g, x in ps:
+        assert x.shape[0] == g.shape[0] and g.shape[1] == n and x.shape[1] == k and g.dtype == x.dtype == dt
+    outs = [torch.empty(n, k, dtype=torch.float32, device=g.device) for g, _ in ps]
+    live = []
+    for out, (g, x) in zip(outs, ps):
+        if g.shape[0] == 0:
+            out.zero_()
+        else:
+            live.append((out, g, x))
+    if not live:
+        return outs
+    terms = {}
+
+    def split(t, n_terms):      # one split of an operand the products share
+        key = (t.data_ptr(), tuple(t.shape), t.stride(0))
+        if key not in terms:
+            terms[key] = _split_bf16(t, n_terms)
+        return terms[key]
+
+    prob_pairs = []
+    for _, g, x in live:
+        if dt == torch.float32 and FP32_GEMM == "3xtf32":
+            # fp32 = b0 + b1 + b2 exactly (three bf16 terms): six bf16 products carry the product to ~2^-24
+            g3, x3 = split(g, 3), split(x, 3)
+            prob_pairs.append([(g3[0], x3[0]), (g3[0], x3[1]), (g3[1], x3[0]), (g3[0], x3[2]), (g3[2], x3[0]),
+                               (g3[1], x3[1])])
+        elif dt == torch.float32:
+            # one-pass mode: two bf16 terms, three products (~2^-16, finer than one tf32 pass)
+            g2, x2 = split(g, 2), split(x, 2)
+            prob_pairs.append([(g2[0], x2[0]), (g2[0], x2[1]), (g2[1], x2[0])])
+        else:
+            prob_pairs.append([(_tma_ready(g), _tma_ready(x))])
+    code = _C.dtype_code(prob_pairs[0][0][0].dtype)
+    es = prob_pairs[0][0][0].element_size()
+    n_src = len(prob_pairs[0])
     for n0 in range(0, n, 256):
         for k0 in range(0, k, 256):
             nn, kk = min(256, n - n0), min(256, k - k0)
-            # split-K partials: a fresh block per call (the caching allocator is stream-aware; several simulated
-            # ranks run on their own streams in one process and must not share scratch)
-            ws = torch.empty(int(_C.lib.pg_wgrad_workspace(m, nn, kk, code)), dtype=torch.float32, device=g.device)
-            es = pairs[0][0].element_size()
-            srcs = (_C.pg_gemm_src * len(pairs))(*[
-                _C.pg_gemm_src(a.data_ptr() + n0 * es, a.stride(0), b.data_ptr() + k0 * es, b.stride(0), m)
-                for a, b in pairs])
-            o = out[n0:n0 + nn, k0:k0 + kk]
+            srcs = (_C.pg_gemm_src * (n_src * len(live)))(*[
+                _C.pg_gemm_src(a.data_ptr() + n0 * es, a.stride(0), b.data_ptr() + k0 * es, b.stride(0), a.shape[0])
+                for pp in prob_pairs for a, b in pp])
+            wss, couts = [], []
+            for out, g, _ in live:
+                m = g.shape[0]
+                # split-K partials: a fresh block per call (the caching allocator is stream-aware; several simulated
+                # ranks run on their own streams in one process and must not share scratch)
+                ws = torch.empty(int(_C.lib.pg_wgrad_workspace(m, nn, kk, code)), dtype=torch.float32, device=g.device)
+                wss.append(ws)
+                o = out[n0:n0 + nn, k0:k0 + kk]
+                couts.append(_C.pg_wgrad_out(o.data_ptr(), o.stride(0), m, ws.data_ptr(), ws.numel()))
             _C.count(2)
-            _C.check(_C.lib.pg_wgrad(code, srcs, len(pairs), o.data_ptr(), o.stride(0), m, nn, kk, ws.data_ptr(),
-                                     ws.numel(), _C.stream_ptr()), "pg_wgrad")
-    return out
+            _C.check(_C.lib.pg_wgrad_group(code, srcs, n_src, len(live), (_C.pg_wgrad_out * len(couts))(*couts), nn,
+                                           kk, _C.stream_ptr()), "pg_wgrad_group")
+    return outs
 
 
 class _Linear(torch.autograd.Function):
@@ -577,10 +633,11 @@ class SageLayerFn(torch.autograd.Function):
         ah  = (A @ feat) / in_deg                         pg_aggregate
         out = feat[:N_in] @ W1^T + ah @ W2^T + (b1 + b2)  pg_linear, two sources, one kernel
 
-        g_feat[:N_in] = g @ W1                            pg_linear
-        gs            = (g @ W2) / in_deg                 pg_linear with the row scale fused
+        g_feat[:N_in] = g @ W1                            pg_linear_group: one launch for both, g read once,
+        gs            = (g @ W2) / in_deg                 the row scale fused into the second product
         g_feat       += A^T @ gs                          pg_aggregate accumulating into rows < N_in
-        gW1 = g^T feat[:N_in], gW2 = g^T ah, gb = sum g   library GEMM / reduction
+        gW1 = g^T feat[:N_in], gW2 = g^T ah               pg_wgrad_group: one launch for both, g read once
+        gb = sum g                                        column sums of the LayerNorm backward
     """
 
     @staticmethod
@@ -614,11 +671,12 @@ class SageLayerFn(torch.autograd.Function):
         if ctx.needs_input_grad[0]:
             d_in = x.shape[1]
             g_feat = alloc_rows(ctx.num_all, d_in, x.dtype, x.device)
-            gemm_nt(gsp, padded_weight(w1, x.dtype, transpose=True), out=g_feat[:graph.num_in])
-            gs = gemm_nt(gsp, padded_weight(w2, x.dtype, transpose=True), row_div=deg_f)
+            _, gs = gemm_nt_group(gsp, [padded_weight(w1, x.dtype, transpose=True),
+                                        padded_weight(w2, x.dtype, transpose=True)],
+                                  row_divs=[None, deg_f], outs=[g_feat[:graph.num_in], None])
             aggregate(graph.bwd, gs, out=g_feat, acc_rows=graph.num_in, drop=ctx.drop_bwd)
-        gw1 = wgrad(gsp, x).to(w1.dtype)
-        gw2 = wgrad(gsp, ah).to(w2.dtype)
+        gw1, gw2 = wgrad_group([(gsp, x), (gsp, ah)])
+        gw1, gw2 = gw1.to(w1.dtype), gw2.to(w2.dtype)
         gb = (colsum if colsum is not None else g.float().sum(0)) if ctx.has_bias else None
         return g_feat, None, None, gw1, gb, gw2, gb, None
 
@@ -696,8 +754,9 @@ class SageLayerNarrowFn(torch.autograd.Function):
                 gemm_nt(dzsp.rows(n_in) if is_split else dz[n_in:], w2t, out=g_feat[n_in:], drop=db, drop_row0=n_in)
             if db is None and ctx.drop_bwd is not None and ctx.drop_bwd.p > 0:
                 dropout_rows(g_feat, ctx.drop_bwd, out=g_feat)
-        gw1 = wgrad(gsp, fsp.rows(0, n_in) if is_split else feat[:n_in]).to(w1.dtype)
-        gw2 = wgrad(dzsp, fsp).to(w2.dtype)
+        # one launch for both: feat is read from HBM once
+        gw1, gw2 = wgrad_group([(gsp, fsp.rows(0, n_in) if is_split else feat[:n_in]), (dzsp, fsp)])
+        gw1, gw2 = gw1.to(w1.dtype), gw2.to(w2.dtype)
         gb = (colsum if colsum is not None else g.float().sum(0)) if ctx.has_bias else None
         return g_feat, None, None, gw1, gb, gw2, gb, None
 
