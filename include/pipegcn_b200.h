@@ -712,6 +712,53 @@ int pg_resgated_bwd_src(const pg_csr* gt, const void* qv, int64_t ldqv, const vo
                         void* dqv, int64_t lddqv, float* scratch, int64_t ld_scratch, void* stream);
 
 /* ------------------------------------------------------------------------------------------
+ * Gaussian mixture model convolution (Monti et al., CVPR 2017; DGL GMMConv, mean aggregator) with the degree
+ * pseudo-coordinates e_uv = (c[u], c[v]) of an edge u -> v, over the `_U` rows [inner | halo] of one partition.  c is
+ * fp32 [num_all] (c = clamp(deg, 1)^-1/2 of every row), rdeg fp32 [N_in] (1 / the CSR row length of every inner row),
+ * mu and inv_sigma fp32 [k, 2] in device memory (a captured CUDA graph reads their current values), 1 <= k <= 8:
+ *   w_k(e) = exp(-1/2 sum_j ((e_j - mu[k, j]) inv_sigma[k, j])^2)   (fp32, one expf per kernel and edge)
+ * Operands with k slices hold slice q at columns [q slice, q slice + d); slice is a multiple of 16 bytes and reaches the
+ * last 16-byte vector of d.  Every operand is fp32 or bf16 (`dtype`), rows start on 16-byte boundaries with strides
+ * that are multiples of 16 bytes; each row's last vector is written whole, the columns past d as 0.  Sums are fp32
+ * with one multiply-add per term in CSR (CSC) order; long rows come as segments whose partials a fix-up adds in
+ * segment order; every result is rounded once.  No atomics: the same bits from run to run.  The plans must carry the
+ * chunk table; scratch is fp32 [n_seg][ld_scratch] (may be NULL when n_seg == 0).
+ * The backward passes also write dmu and dinv_sigma (fp32 [k, 2]), with s_k(e) the per-edge dot product below:
+ *   dmu[k, j] = inv_sigma^2 sum_e s_k w_k (e_j - mu[k, j]),  dinv_sigma[k, j] = -inv_sigma sum_e s_k w_k (e_j - mu)^2
+ * Each warp writes its chunk's 4 k sums (fp32, a fixed shuffle tree) to `partial`, then one small kernel adds them
+ * in a fixed order in fp64 and rounds once.
+ * ---------------------------------------------------------------------------------------- */
+/* loads every MoNet kernel (call it before any halo wait can spin: a first launch may wait for the device) */
+int pg_monet_preload(void);
+/* floats of the `partial` workspace of a backward pass over the plan gt at width d */
+int64_t pg_monet_workspace(const pg_csr* gt, int32_t d, int dtype, int32_t k);
+/* aggregate first, over the forward CSR g:  out[v][q] = rdeg[v] sum_u w_q(e_uv) x[u]   (x [num_all, d], out [N_in]
+ * with k slices).  ld_scratch >= k d */
+int pg_monet_agg_k(const pg_csr* g, const void* x, int64_t ldx, int32_t d, int dtype, int32_t k, const float* c,
+                   const float* rdeg, const float* mu, const float* inv_sigma, void* out, int64_t ldo, int64_t slice,
+                   float* scratch, int64_t ld_scratch, void* stream);
+/* transform first, over the forward CSR g:  out[v] = rdeg[v] sum_u sum_q w_q(e_uv) z[u][q] (+ bias)   (z [num_all]
+ * with k slices, bias fp32 [d] or NULL, out [N_in, d]).  ld_scratch >= d */
+int pg_monet_agg_sum(const pg_csr* g, const void* z, int64_t ldz, int64_t slice, int32_t d, int dtype, int32_t k,
+                     const float* c, const float* rdeg, const float* mu, const float* inv_sigma, const float* bias,
+                     void* out, int64_t ldo, float* scratch, int64_t ld_scratch, void* stream);
+/* transform-first backward, over the CSC row u of gt (rows = all num_all `_U` rows, entries the destinations v):
+ *   dz[u][q] = sum_v w_q(e_uv) rdeg[v] G[v],   s_q(e_uv) = <G[v], z[u][q]> rdeg[v]
+ * (G = grad [N_in, d]; z and dz [num_all] with k slices).  ld_scratch >= k d */
+int pg_monet_bwd_k(const pg_csr* gt, const void* grad, int64_t ldg, const void* z, int64_t ldz, int64_t slice,
+                   int32_t d, int dtype, int32_t k, const float* c, const float* rdeg, const float* mu,
+                   const float* inv_sigma, void* dz, int64_t lddz, float* scratch, int64_t ld_scratch, float* partial,
+                   int64_t n_partial, float* dmu, float* dinv_sigma, void* stream);
+/* aggregate-first backward, over the CSC row u of gt:
+ *   dh[u] = dropout(sum_v rdeg[v] sum_q w_q(e_uv) dA[v][q]),   s_q(e_uv) = <dA[v][q], h[u]> rdeg[v]
+ * (dA [N_in] with k slices, h and dh [num_all, d]); drop (may be NULL) is the dropout key of the layer input, applied
+ * as pg_dropout_rows does (row u, 16-byte vectors).  ld_scratch >= d */
+int pg_monet_bwd_sum(const pg_csr* gt, const void* da, int64_t ldda, int64_t slice, const void* h, int64_t ldh,
+                     int32_t d, int dtype, int32_t k, const float* c, const float* rdeg, const float* mu,
+                     const float* inv_sigma, const pg_drop* drop, void* dh, int64_t lddh, float* scratch,
+                     int64_t ld_scratch, float* partial, int64_t n_partial, float* dmu, float* dinv_sigma, void* stream);
+
+/* ------------------------------------------------------------------------------------------
  * Symmetric heap: device memory that peers map through CUDA IPC (host pointers out).
  * ---------------------------------------------------------------------------------------- */
 #define PG_IPC_HANDLE_BYTES 64

@@ -169,6 +169,16 @@ def _load():
                                          vp]),
         "pg_genconv_bwd_src": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, vp, i32, vp, i64, vp, i64, vp, i64, vp, i64,
                                          i32, C.POINTER(pg_drop), i32, C.c_int, vp, i64, vp, i64, vp]),
+        "pg_monet_preload": (C.c_int, []),
+        "pg_monet_workspace": (i64, [C.POINTER(pg_csr), i32, C.c_int, i32]),
+        "pg_monet_agg_k": (C.c_int, [C.POINTER(pg_csr), vp, i64, i32, C.c_int, i32, vp, vp, vp, vp, vp, i64, i64, vp,
+                                     i64, vp]),
+        "pg_monet_agg_sum": (C.c_int, [C.POINTER(pg_csr), vp, i64, i64, i32, C.c_int, i32, vp, vp, vp, vp, vp, vp,
+                                       i64, vp, i64, vp]),
+        "pg_monet_bwd_k": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, i64, i32, C.c_int, i32, vp, vp, vp, vp, vp,
+                                     i64, vp, i64, vp, i64, vp, vp, vp]),
+        "pg_monet_bwd_sum": (C.c_int, [C.POINTER(pg_csr), vp, i64, i64, vp, i64, i32, C.c_int, i32, vp, vp, vp, vp,
+                                       C.POINTER(pg_drop), vp, i64, vp, i64, vp, i64, vp, vp, vp]),
         "pg_resgated_preload": (C.c_int, []),
         "pg_resgated_aggregate": (C.c_int, [C.POINTER(pg_csr), vp, i64, vp, i64, i32, i32, C.c_int, vp, i32, vp, i64,
                                             vp, i64, vp]),

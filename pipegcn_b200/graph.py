@@ -174,6 +174,13 @@ class PartGraph:
             self._row_deg_f = (self.fwd.indptr[1:] - self.fwd.indptr[:-1]).to(torch.float32).contiguous()
         return self._row_deg_f
 
+    def inv_row_degrees(self) -> torch.Tensor:
+        """1 / clamp(CSR row length, min=1), fp32 [num_in] (MoNet's mean over the in-edges), kept at this address:
+        captured CUDA graphs read it."""
+        if not hasattr(self, "_inv_row_deg_f"):
+            self._inv_row_deg_f = torch.div(1.0, torch.clamp(self.row_degrees(), min=1.0)).contiguous()
+        return self._inv_row_deg_f
+
     def set_sym_norm(self, c: torch.Tensor):
         """GraphConv's c = deg^-1/2 of every [inner | halo] row: fp32 [num_all], the halo rows' values from their
         owners (`train._sym_norm_steps`).  Set once; captured CUDA graphs read it at this address."""

@@ -64,6 +64,13 @@ and cannot be combined with --use-pp or --aggregator pool.
 PyG's ResGatedGraphConv): every layer sums the values val_u of its in-edges, each weighted by its own per-channel gate
 sigmoid(k_v + q_u), and adds a skip linear of h_v and a bias.  It has no flags of its own (--n-heads is ignored).  It
 works with boundary-node sampling and cannot be combined with --use-pp or --aggregator pool.
+
+`--model monet` (not in the reference) trains the Gaussian mixture model convolution of MoNet (Monti et al., CVPR 2017;
+DGL's GMMConv with the mean aggregator) on the degree pseudo-coordinates e_uv = (c_u, c_v), c = deg^-1/2 (the halo
+rows' degrees supplied by their owners): every layer averages over the in-edges sum_k w_k(e_uv) h_u W_k^T, with K
+Gaussian weights w_k of learnt means mu and inverse widths inv_sigma.  `--monet-kernels K` (an integer 1 <= K <= 8,
+default 3) sets K; suppressed like `--sampling-rate`: read it with getattr(args, 'monet_kernels', 3).  --n-heads is
+ignored.  It cannot be combined with --use-pp, --aggregator pool or --sampling-rate < 1.
 """
 import argparse
 
@@ -72,8 +79,8 @@ _FLAGS = [
     ("dataset", dict(type=str, default='reddit', help="the input dataset (or synthetic:<shape>)")),
     ("graph-name", dict(type=str, default='')),
     ("model", dict(type=str, default='graphsage', help="model for training (graphsage | gcn | gat | gatv2 | transformer | "
-                                                              "graphconv | gcnii | pna | genconv | resgatedgcn; gcn is "
-                                                              "GraphSAGE)")),
+                                                              "graphconv | gcnii | pna | genconv | resgatedgcn | monet; "
+                                                              "gcn is GraphSAGE)")),
     ("dropout", dict(type=float, default=0.5, help="dropout probability")),
     ("lr", dict(type=float, default=1e-2, help="learning rate")),
     ("n-epochs", dict(type=int, default=200, help="the number of training epochs")),
@@ -157,6 +164,16 @@ def _genconv_t(text):
     return t
 
 
+def _monet_kernels(text):
+    try:
+        k = int(text)
+    except ValueError:
+        raise argparse.ArgumentTypeError(f"invalid number of MoNet kernels '{text}'")
+    if not 1 <= k <= 8:               # the kernel counts csrc/monet.cu is compiled for
+        raise argparse.ArgumentTypeError(f"--monet-kernels {text}: expected 1 to 8 mixture kernels")
+    return k
+
+
 def build_parser():
     parser = argparse.ArgumentParser(description='PipeGCN on H100')
     for flag, kw in _FLAGS:
@@ -192,6 +209,8 @@ def build_parser():
                         help="--model genconv: softmax temperature t (finite, default 1.0)")
     parser.add_argument('--genconv-learn-t', '--genconv_learn_t', action='store_true', default=argparse.SUPPRESS,
                         help="--model genconv: learn t (one scalar per graph layer, initialised to --genconv-t)")
+    parser.add_argument('--monet-kernels', '--monet_kernels', type=_monet_kernels, default=argparse.SUPPRESS,
+                        help="--model monet: Gaussian mixture kernels per layer (1 to 8, default 3)")
     return parser
 
 

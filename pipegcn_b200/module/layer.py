@@ -120,6 +120,36 @@ keys are ResGatedGraphConv's: `lin_key.*`, `lin_query.*`, `lin_value.*` (weights
 (kaiming_uniform_(a=sqrt(5)), then its bias U(-1/sqrt(d_in), 1/sqrt(d_in))), in the order lin_key, lin_query,
 lin_value, lin_skip, then bias = 0.  PyG draws the linears twice (at construction and in reset_parameters), so equal
 seeds do not give PyG's initial weights.
+
+`MoNetLayer` (not in the reference): the Gaussian mixture model convolution of MoNet (Monti et al., "Geometric deep
+learning on graphs and manifolds using mixture model CNNs", CVPR 2017), DGL's `GMMConv(d_in, d_out, dim=2,
+n_kernels=K, aggregator_type='mean', residual=False, bias=True)` with the degree pseudo-coordinates of DGL's MoNet
+citation example (without its per-layer `pseudo_proj`), over the same rows.  c = clamp(deg, min=1)^(-1/2) of every
+[inner | halo] row (deg: in-degree with the self loop in the whole graph; the halo rows' values come from their
+owners, `PartGraph.sym_norm`), deg_v the CSR row length of v:
+
+    e_uv   = (c[u], c[v])                                                 pseudo-coordinates of u -> v
+    w_k(e) = exp(-1/2 sum_j (e_j - mu[k, j])^2 inv_sigma[k, j]^2)         k = 0..K-1, j = 0, 1
+    z_u[k] = h[u] @ W_k^T,   W_k = fc.weight[k d_out:(k + 1) d_out]       (fc has no bias)
+    out[v] = (1/deg_v) sum_{u -> v} sum_k w_k(e_uv) z_u[k] + bias
+
+It aggregates first when d_in <= K d_out (A_v[k] = (1/deg_v) sum_u w_k(e_uv) h[u], then one GEMM of A [N_in, K d_in]
+with the k-major B[k d_in + i, m] = W_k[m, i]), and transforms first otherwise (z over every row, then the
+mixture-weighted mean of its K slices); the rule follows from the shapes alone.  The gradients, with G = dL/d out and
+s_k(e_uv) = dL/dw_k(e_uv):
+
+    aggregate first:  dA_v[k] = G_v @ W_k,  s_k(e_uv) = <dA_v[k], h[u]> / deg_v,
+                      dh[u] = sum_{v: u -> v} (1/deg_v) sum_k w_k(e_uv) dA_v[k],  dfc = G^T A (permuted back)
+    transform first:  dz_u[k] = sum_{v: u -> v} (w_k(e_uv) / deg_v) G_v,  s_k(e_uv) = <G_v, z_u[k]> / deg_v,
+                      dh = dz @ fc.weight,  dfc = dz^T h
+    both:             dmu[k, j] = sum_e s_k w_k (e_j - mu[k, j]) inv_sigma[k, j]^2
+                      dinv_sigma[k, j] = -sum_e s_k w_k (e_j - mu[k, j])^2 inv_sigma[k, j],  dbias = sum_v G_v
+
+Every edge lives in the CSR of its destination's rank, so each rank's mu / inv_sigma gradient covers its own edges and
+the all-reduce of the gradients sums them.  State-dict keys are GMMConv's: `mu` [K, 2], `inv_sigma` [K, 2],
+`fc.weight` [K d_out, d_in], `bias` [d_out].  Initialisation follows GMMConv's constructor and draw order: fc is built
+as `nn.Linear(bias=False)` (drawing its default initialisation), then reset_parameters draws
+xavier_normal_(fc.weight, gain=calculate_gain('relu')), then normal_(mu, 0, 0.1), then inv_sigma = 1 and bias = 0.
 """
 import math
 
@@ -404,3 +434,30 @@ class ResGatedLayer(nn.Module):
         return ops.resgated_layer(feat, graph, keep, self.lin_key.weight, self.lin_key.bias, self.lin_query.weight,
                                   self.lin_query.bias, self.lin_value.weight, self.lin_value.bias,
                                   self.lin_skip.weight, self.bias, drop_bwd)
+
+
+class MoNetLayer(nn.Module):
+    """GMMConv(in_feats, out_feats, dim=2, n_kernels, aggregator_type='mean') on the degree pseudo-coordinates: module
+    docstring."""
+
+    def __init__(self, in_feats, out_feats, n_kernels=3):
+        super().__init__()
+        self.in_feats, self.out_feats, self.n_kernels = in_feats, out_feats, n_kernels
+        self.mu = nn.Parameter(torch.empty(n_kernels, 2))
+        self.inv_sigma = nn.Parameter(torch.empty(n_kernels, 2))
+        self.fc = nn.Linear(in_feats, n_kernels * out_feats, bias=False)
+        self.bias = nn.Parameter(torch.empty(out_feats))
+        self.reset_parameters()
+
+    def reset_parameters(self):
+        """GMMConv.reset_parameters."""
+        nn.init.xavier_normal_(self.fc.weight, gain=nn.init.calculate_gain('relu'))
+        nn.init.normal_(self.mu.data, 0, 0.1)
+        nn.init.constant_(self.inv_sigma.data, 1)
+        nn.init.zeros_(self.bias.data)
+
+    def forward(self, graph, feat, in_deg=None, drop_bwd=None):
+        """`feat`: the [num_all, d_in] rows of `graph`; returns the [N_in, d_out] inner rows.  `in_deg` is unused: the
+        pseudo-coordinates are `graph.sym_norm()` and the mean divides by the CSR row lengths.  `drop_bwd` as
+        GraphSAGELayer.forward."""
+        return ops.monet_layer(feat, graph, self.fc.weight, self.mu, self.inv_sigma, self.bias, drop_bwd)

@@ -53,14 +53,20 @@ memory, so a captured CUDA graph sees the optimizer's updates of it.
 module/layer.py); a last graph layer that produces the logits is a ResGatedLayer(d_in, n_class).  Like `GENConv`, with
 boundary-node sampling its layers take the buffer's keep mask of the halo rows, and unkept rows are absent from every
 sum.
+
+`MoNet(GraphSAGE)` (not in the reference) is the same layer loop with `MoNetLayer`s (DGL's GMMConv with the mean
+aggregator on the degree pseudo-coordinates, module/layer.py); a last graph layer that produces the logits is a
+MoNetLayer(d_in, n_class).  Like `GraphConv`, the layers read c = deg^-1/2 from the graph (`PartGraph.sym_norm`,
+the halo rows' values from their owners).  mu and inv_sigma are read by the kernels from device memory, so a captured
+CUDA graph sees the optimizer's updates of them.
 """
 import torch
 from torch import nn
 import torch.nn.functional as F
 
 from ..helper import context as ctx
-from .layer import (GATLayer, GATv2Layer, GCNIILayer, GENConvLayer, GraphConvLayer, GraphSAGELayer, PNALayer,
-                    ResGatedLayer, TransformerLayer)
+from .layer import (GATLayer, GATv2Layer, GCNIILayer, GENConvLayer, GraphConvLayer, GraphSAGELayer, MoNetLayer,
+                    PNALayer, ResGatedLayer, TransformerLayer)
 
 
 class GNNBase(nn.Module):
@@ -462,3 +468,34 @@ class ResGatedGCN(_KeepMaskLayers):
     def _preload(self):
         from .. import ops
         ops.resgated_preload()
+
+
+class MoNet(GraphSAGE):
+
+    def __init__(self, layer_size, activation, dropout=0.5, norm='layer', train_size=None, n_linear=0, buffer=None,
+                 dtype=torch.float32, n_kernels=3):
+        self.n_kernels = int(n_kernels)
+        super().__init__(layer_size, activation, False, dropout=dropout, norm=norm, train_size=train_size,
+                         n_linear=n_linear, buffer=buffer, dtype=dtype)
+
+    def _graph_layer(self, i, d_in, d_out):
+        return MoNetLayer(d_in, d_out, self.n_kernels)
+
+    def _layer_arg(self, in_deg):
+        """MoNet layers take no degrees: the pseudo-coordinates and the row lengths live on the graph."""
+        return None
+
+    def _prepare(self, g):
+        """Loads the kernels and the graph's reciprocal row lengths before any halo wait can spin (both may wait for
+        the device)."""
+        from .. import ops
+        ops.monet_preload()
+        g.inv_row_degrees()
+
+    def forward(self, g, feat, in_deg=None):
+        self._prepare(g)
+        return super().forward(g, feat, in_deg)
+
+    def forward_partitioned(self, g, xch, pp_feat=None, push0=False):
+        self._prepare(g)
+        return (yield from super().forward_partitioned(g, xch, pp_feat, push0))

@@ -2254,6 +2254,247 @@ def resgated_layer(feat, graph, keep, w_k, b_k, w_q, b_q, w_v, b_v, w_s, bias, d
     return ResGatedLayerFn.apply(feat, graph, keep, w_k, b_k, w_q, b_q, w_v, b_v, w_s, bias, drop_bwd)
 
 
+# ---- Gaussian mixture model convolution, GMMConv (csrc/monet.cu) ------------------------------------------
+MONET_MAX_K = 8                    # the kernel counts csrc/monet.cu is compiled for
+
+
+def monet_preload():
+    """Load every MoNet kernel now (see gat_preload)."""
+    _C.check(_C.lib.pg_monet_preload(), "pg_monet_preload")
+
+
+def monet_slice(d: int, dtype) -> int:
+    """Column distance of the K slices of a MoNet operand of width d: d rounded up to whole 16-byte vectors."""
+    v = 16 // torch.empty(0, dtype=dtype).element_size()
+    return -(-int(d) // v) * v
+
+
+def monet_aggregate_first(d_in: int, d_out: int, k: int) -> bool:
+    """The layer's evaluation order: gather the d_in-wide input rows once into K accumulators when d_in <= K d_out,
+    else transform first and gather the K d_out-wide slices."""
+    return d_in <= k * d_out
+
+
+def _mix_params(mu: torch.Tensor, inv_sigma: torch.Tensor):
+    """mu, inv_sigma as the kernels read them: fp32 [K, 2], contiguous (the parameters themselves, so a captured CUDA
+    graph reads the values the optimiser wrote)."""
+    mu, inv_sigma = mu.detach(), inv_sigma.detach()
+    assert mu.dtype == inv_sigma.dtype == torch.float32 and mu.is_contiguous() and inv_sigma.is_contiguous()
+    assert mu.shape == inv_sigma.shape and mu.dim() == 2 and mu.shape[1] == 2 and 1 <= mu.shape[0] <= MONET_MAX_K
+    return mu, inv_sigma
+
+
+def _monet_common(graph: PartGraph, x: torch.Tensor):
+    c = graph.sym_norm()
+    rdeg = graph.inv_row_degrees()
+    assert c.numel() == graph.num_all and rdeg.numel() == graph.num_in
+    return c, rdeg
+
+
+def monet_agg_k(graph: PartGraph, x: torch.Tensor, mu, inv_sigma) -> torch.Tensor:
+    """A [N_in, K slice] (x's dtype, slice = monet_slice(d)): A[v][k] = (1/deg_v) sum_u w_k(c_u, c_v) x[u] over the
+    forward CSR (pg_monet_agg_k); the columns between d and the next slice are 0."""
+    mu, inv_sigma = _mix_params(mu, inv_sigma)
+    x = _tma_ready(_rows(x))           # whole 16-byte vectors per row (whole-graph evaluation may hand [N, d] rows)
+    c, rdeg = _monet_common(graph, x)
+    plan, d, k = graph.fwd, x.shape[1], mu.shape[0]
+    sl = monet_slice(d, x.dtype)
+    out = alloc_rows(plan.n_rows, k * sl, x.dtype, x.device)
+    scratch = plan.scratch(k * d)
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_monet_agg_k(C.byref(plan.c), x.data_ptr(), x.stride(0), d, _C.dtype_code(x.dtype), k,
+                                   c.data_ptr(), rdeg.data_ptr(), mu.data_ptr(), inv_sigma.data_ptr(), out.data_ptr(),
+                                   out.stride(0), sl, _ptr(scratch), _scratch_ld(k * d), _C.stream_ptr()),
+             "pg_monet_agg_k")
+    return out
+
+
+def monet_agg_sum(graph: PartGraph, z: torch.Tensor, d: int, mu, inv_sigma, bias=None) -> torch.Tensor:
+    """out [N_in, d] = (1/deg_v) sum_u sum_k w_k(c_u, c_v) z[u][k] (+ bias) over the forward CSR (pg_monet_agg_sum);
+    z [num_all, K slice] holds slice k at columns [k slice, k slice + d)."""
+    mu, inv_sigma = _mix_params(mu, inv_sigma)
+    c, rdeg = _monet_common(graph, z)
+    plan, k = graph.fwd, mu.shape[0]
+    sl = monet_slice(d, z.dtype)
+    out = alloc_rows(plan.n_rows, d, z.dtype, z.device)
+    if bias is not None:
+        bias = bias.detach()
+        assert bias.dtype == torch.float32 and bias.is_contiguous() and bias.numel() == d
+    scratch = plan.scratch(d)
+    _C.count(2 if plan.n_long else 1)
+    _C.check(_C.lib.pg_monet_agg_sum(C.byref(plan.c), z.data_ptr(), z.stride(0), sl, int(d), _C.dtype_code(z.dtype),
+                                     k, c.data_ptr(), rdeg.data_ptr(), mu.data_ptr(), inv_sigma.data_ptr(),
+                                     _ptr(bias), out.data_ptr(), out.stride(0), _ptr(scratch), _scratch_ld(d),
+                                     _C.stream_ptr()), "pg_monet_agg_sum")
+    return out
+
+
+def _mix_grads(plan: CsrPlan, d: int, dtype, k: int, device):
+    n = int(_C.lib.pg_monet_workspace(C.byref(plan.c), int(d), _C.dtype_code(dtype), int(k)))
+    partial = torch.empty(max(n, 1), dtype=torch.float32, device=device)
+    dmu = torch.empty(k, 2, dtype=torch.float32, device=device)
+    dinv = torch.empty(k, 2, dtype=torch.float32, device=device)
+    return partial, n, dmu, dinv
+
+
+def monet_bwd_k(graph: PartGraph, g: torch.Tensor, z: torch.Tensor, mu, inv_sigma):
+    """(dz, dmu, dinv_sigma) of the transform-first layer over the CSC (pg_monet_bwd_k): dz [num_all, K slice] (g's
+    dtype) = sum_v (w_k(c_u, c_v) / deg_v) g[v]; the mixture gradients with s_k = <g[v], z[u][k]> / deg_v."""
+    mu, inv_sigma = _mix_params(mu, inv_sigma)
+    g = _tma_ready(_rows(g))
+    c, rdeg = _monet_common(graph, g)
+    _rows(z)
+    plan, d, k = graph.bwd, g.shape[1], mu.shape[0]
+    sl = monet_slice(d, g.dtype)
+    dz = alloc_rows(plan.n_rows, k * sl, g.dtype, g.device)
+    scratch = plan.scratch(k * d)
+    partial, n, dmu, dinv = _mix_grads(plan, d, g.dtype, k, g.device)
+    _C.count((2 if plan.n_long else 1) + 1)
+    _C.check(_C.lib.pg_monet_bwd_k(C.byref(plan.c), g.data_ptr(), g.stride(0), z.data_ptr(), z.stride(0), sl, d,
+                                   _C.dtype_code(g.dtype), k, c.data_ptr(), rdeg.data_ptr(), mu.data_ptr(),
+                                   inv_sigma.data_ptr(), dz.data_ptr(), dz.stride(0), _ptr(scratch),
+                                   _scratch_ld(k * d), partial.data_ptr(), n, dmu.data_ptr(), dinv.data_ptr(),
+                                   _C.stream_ptr()), "pg_monet_bwd_k")
+    return dz, dmu, dinv
+
+
+def monet_bwd_sum(graph: PartGraph, da: torch.Tensor, h: torch.Tensor, mu, inv_sigma, drop: DropSpec = None):
+    """(dh, dmu, dinv_sigma) of the aggregate-first layer over the CSC (pg_monet_bwd_sum): dh [num_all, d] (h's dtype)
+    = dropout(sum_v (1/deg_v) sum_k w_k(c_u, c_v) dA[v][k]) under the key `drop`; the mixture gradients with
+    s_k = <dA[v][k], h[u]> / deg_v.  dA [N_in, K slice]."""
+    mu, inv_sigma = _mix_params(mu, inv_sigma)
+    h = _tma_ready(_rows(h))
+    c, rdeg = _monet_common(graph, h)
+    _rows(da)
+    plan, d, k = graph.bwd, h.shape[1], mu.shape[0]
+    sl = monet_slice(d, h.dtype)
+    dh = alloc_rows(plan.n_rows, d, h.dtype, h.device)
+    scratch = plan.scratch(d)
+    partial, n, dmu, dinv = _mix_grads(plan, d, h.dtype, k, h.device)
+    dc = C.byref(drop.c()) if drop is not None and drop.p > 0 else None
+    _C.count((2 if plan.n_long else 1) + 1)
+    _C.check(_C.lib.pg_monet_bwd_sum(C.byref(plan.c), da.data_ptr(), da.stride(0), sl, h.data_ptr(), h.stride(0), d,
+                                     _C.dtype_code(h.dtype), k, c.data_ptr(), rdeg.data_ptr(), mu.data_ptr(),
+                                     inv_sigma.data_ptr(), dc,
+                                     dh.data_ptr(), dh.stride(0), _ptr(scratch), _scratch_ld(d), partial.data_ptr(), n,
+                                     dmu.data_ptr(), dinv.data_ptr(), _C.stream_ptr()), "pg_monet_bwd_sum")
+    return dh, dmu, dinv
+
+
+def monet_weight_b(fc_weight: torch.Tensor, k: int, dtype, transpose: bool = False) -> torch.Tensor:
+    """The aggregate-first B operand of `A @ B`, as a padded copy in the activation dtype: Bt [d_out, K slice] with
+    Bt[m, q slice + i] = W_q[m, i] (W_q = fc.weight[q d_out:(q + 1) d_out]), 0 in the pad columns; its transpose B
+    [K slice, d_out] with `transpose`."""
+    kd, d_in = fc_weight.shape
+    d_out, sl = kd // k, monet_slice(d_in, dtype)
+    bt = alloc_rows(d_out, k * sl, dtype, fc_weight.device, zero=sl != d_in)
+    bt.view(d_out, k, sl)[:, :, :d_in].copy_(fc_weight.detach().view(k, d_out, d_in).permute(1, 0, 2))
+    return padded_weight(bt, dtype, transpose=True) if transpose else bt
+
+
+def monet_weight_z(fc_weight: torch.Tensor, k: int, dtype, transpose: bool = False) -> torch.Tensor:
+    """The transform-first weight, as a padded copy in the activation dtype: Wp [K slice, d_in] with row q slice + m =
+    W_q[m] (0 in the pad rows), so z = h @ Wp^T has its K slices `slice` apart; its transpose with `transpose`."""
+    kd, d_in = fc_weight.shape
+    d_out = kd // k
+    sl = monet_slice(d_out, dtype)
+    wp = alloc_rows(k * sl, d_in, dtype, fc_weight.device, zero=sl != d_out)
+    wp.view(k, sl, d_in)[:, :d_out].copy_(fc_weight.detach().view(k, d_out, d_in))
+    return padded_weight(wp, dtype, transpose=True) if transpose else wp
+
+
+class MoNetLayerFn(torch.autograd.Function):
+    """GMMConv (mean aggregator, degree pseudo-coordinates) aggregating first, d_in <= K d_out:
+
+        A   = pg_monet_agg_k over the CSR         [N_in, K slice]   A[v][k] = (1/deg_v) sum_u w_k(e_uv) h[u]
+        out = A @ B + bias                        pg_linear, B the permuted padded copy of fc.weight (monet_weight_b)
+
+        dA  = G @ B^T                             pg_linear
+        dh, dmu, dinv_sigma = pg_monet_bwd_sum over the CSC, the dropout backward in its store
+        dfc = G^T A (pg_wgrad), permuted back to fc.weight's layout; dbias = sum G
+    """
+
+    @staticmethod
+    def forward(ctx, feat, graph, fc_weight, mu, inv_sigma, bias, drop_bwd=None):
+        feat = _tma_ready(feat if feat.stride(1) == 1 else feat.contiguous())
+        k = mu.shape[0]
+        a = monet_agg_k(graph, feat, mu, inv_sigma)
+        out = gemm_nt(a, monet_weight_b(fc_weight, k, feat.dtype), bias=bias)
+        ctx.graph, ctx.drop_bwd, ctx.has_bias = graph, drop_bwd, bias is not None
+        ctx.save_for_backward(feat, a, fc_weight, mu, inv_sigma)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        feat, a, fc_weight, mu, inv_sigma = ctx.saved_tensors
+        k, (kd, d_in) = mu.shape[0], fc_weight.shape
+        d_out, sl = kd // k, monet_slice(d_in, feat.dtype)
+        colsum = _take_colsum(g)
+        g = _tma_ready(g if g.dtype == feat.dtype else g.to(feat.dtype))
+        gsp = presplit(g)
+        da = gemm_nt(gsp, monet_weight_b(fc_weight, k, feat.dtype, transpose=True))
+        g_feat, dmu, dinv = monet_bwd_sum(ctx.graph, da, feat, mu, inv_sigma, ctx.drop_bwd)
+        gw = wgrad(gsp, a).view(d_out, k, sl)[:, :, :d_in].permute(1, 0, 2).reshape(kd, d_in).to(fc_weight.dtype)
+        gb = (colsum if colsum is not None else g.float().sum(0)) if ctx.has_bias else None
+        return (g_feat if ctx.needs_input_grad[0] else None), None, gw, dmu, dinv, gb, None
+
+
+class MoNetLayerNarrowFn(torch.autograd.Function):
+    """The same function transform-first, d_in > K d_out:
+
+        z   = h @ Wp^T                            [num_all, K slice]   pg_linear, Wp = monet_weight_z(fc.weight)
+        out = pg_monet_agg_sum over the CSR       (1/deg_v) sum_u sum_k w_k(e_uv) z[u][k] + bias
+
+        dz, dmu, dinv_sigma = pg_monet_bwd_k over the CSC
+        dh  = dz @ Wp                             pg_linear, dropout backward in its epilogue
+        dfc = dz^T h (pg_wgrad), the pad rows dropped; dbias = sum G
+    """
+
+    @staticmethod
+    def forward(ctx, feat, graph, fc_weight, mu, inv_sigma, bias, drop_bwd=None):
+        if feat.stride(1) != 1:
+            feat = feat.contiguous()
+        k = mu.shape[0]
+        d_out = fc_weight.shape[0] // k
+        z = gemm_nt(feat, monet_weight_z(fc_weight, k, feat.dtype))
+        out = monet_agg_sum(graph, z, d_out, mu, inv_sigma, bias)
+        ctx.graph, ctx.drop_bwd, ctx.has_bias = graph, drop_bwd, bias is not None
+        ctx.save_for_backward(feat, z, fc_weight, mu, inv_sigma)
+        return out
+
+    @staticmethod
+    def backward(ctx, g):
+        feat, z, fc_weight, mu, inv_sigma = ctx.saved_tensors
+        k, (kd, d_in) = mu.shape[0], fc_weight.shape
+        d_out = kd // k
+        sl = monet_slice(d_out, feat.dtype)
+        colsum = _take_colsum(g)
+        g = _tma_ready(g if g.dtype == feat.dtype else g.to(feat.dtype))
+        dz, dmu, dinv = monet_bwd_k(ctx.graph, g, z, mu, inv_sigma)
+        dzsp = presplit(dz)
+        g_feat = None
+        if ctx.needs_input_grad[0]:
+            g_feat = alloc_rows(feat.shape[0], d_in, feat.dtype, feat.device)
+            db = ctx.drop_bwd if (ctx.drop_bwd is not None and ctx.drop_bwd.p > 0 and d_in <= 256
+                                  and _drop_ok(g_feat)) else None   # dropout backward in the GEMM's epilogue
+            gemm_nt(dzsp, monet_weight_z(fc_weight, k, feat.dtype, transpose=True), out=g_feat, drop=db)
+            if db is None and ctx.drop_bwd is not None and ctx.drop_bwd.p > 0:
+                dropout_rows(g_feat, ctx.drop_bwd, out=g_feat)
+        gw = wgrad(dzsp, feat).view(k, sl, d_in)[:, :d_out].reshape(kd, d_in).to(fc_weight.dtype)
+        gb = (colsum if colsum is not None else g.float().sum(0)) if ctx.has_bias else None
+        return g_feat, None, gw, dmu, dinv, gb, None
+
+
+def monet_layer(feat, graph, fc_weight, mu, inv_sigma, bias, drop_bwd=None) -> torch.Tensor:
+    """GMMConv (mean aggregator) over the [num_all, d_in] rows `feat` of `graph` with the degree pseudo-coordinates
+    (c = graph.sym_norm()); fc_weight [K d_out, d_in], mu and inv_sigma [K, 2], bias [d_out] or None.  Returns the
+    [N_in, d_out] inner rows.  The order follows monet_aggregate_first."""
+    k = mu.shape[0]
+    if monet_aggregate_first(feat.shape[1], fc_weight.shape[0] // k, k):
+        return MoNetLayerFn.apply(feat, graph, fc_weight, mu, inv_sigma, bias, drop_bwd)
+    return MoNetLayerNarrowFn.apply(feat, graph, fc_weight, mu, inv_sigma, bias, drop_bwd)
+
+
 # ---- row-wise epilogues (csrc/rowops.cu) -------------------------------------------------------------------
 # column sums of a gradient tensor computed as a by-product by the kernel that produced it, keyed by the
 # tensor's address: the bias gradient of the linear upstream (saves a full pass over [N, d])

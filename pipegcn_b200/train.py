@@ -33,7 +33,7 @@ from .helper import context as ctx
 from .helper.feature_buffer import Buffer, EvalExchange, OneShotExchange, check_halo_bits, check_sampling
 from .helper.reducer import Reducer
 from .helper.timer.comm_timer import CommTimer
-from .module.model import GAT, GATv2, GCNII, GENConv, PNA, GraphConv, GraphSAGE, GraphTransformer, ResGatedGCN
+from .module.model import GAT, GATv2, GCNII, GENConv, PNA, GraphConv, GraphSAGE, GraphTransformer, MoNet, ResGatedGCN
 from .partition import PartitionLayout, get_layer_size
 
 
@@ -59,7 +59,10 @@ def check_model(args):
     precompute is a neighbour mean) and --sampling-rate < 1 (sampling changes the degrees, the scalers and the sources
     the extremes range over).  --model genconv refuses --use-pp (the precompute is a neighbour mean) and --aggregator
     pool (it has its own aggregator), and a temperature --genconv-t that is not finite.  --model resgatedgcn refuses
-    --use-pp (the precompute is a neighbour mean) and --aggregator pool (it has its own aggregator)."""
+    --use-pp (the precompute is a neighbour mean) and --aggregator pool (it has its own aggregator).  --model monet
+    refuses --use-pp (the precompute is a neighbour mean), --aggregator pool (it has its own aggregator),
+    --sampling-rate < 1 (its pseudo-coordinates and mean are defined on the full graph's degrees) and a --monet-kernels
+    outside 1..8 (the kernel counts its kernels are compiled for)."""
     attention = args.model in ('gat', 'gatv2', 'transformer')
     aggregator = getattr(args, 'aggregator', 'mean')
     if aggregator not in ('mean', 'pool'):
@@ -103,6 +106,18 @@ def check_model(args):
         if aggregator == 'pool':
             raise ValueError("--aggregator pool is a GraphSAGE aggregator; --model resgatedgcn has its own")
         return
+    if args.model == 'monet':
+        k = getattr(args, 'monet_kernels', 3)
+        if not 1 <= k <= 8:
+            raise ValueError(f"--monet-kernels {k}: expected 1 to 8 mixture kernels")
+        if args.use_pp:
+            raise NotImplementedError("--model monet with --use-pp: the precompute is a neighbour mean")
+        if aggregator == 'pool':
+            raise ValueError("--aggregator pool is a GraphSAGE aggregator; --model monet has its own")
+        if getattr(args, 'sampling_rate', 1.0) < 1.0:
+            raise NotImplementedError("--model monet with --sampling-rate < 1: the pseudo-coordinates and the mean are "
+                                      "defined on the full graph's degrees")
+        return
     if args.model == 'graphconv':
         if aggregator == 'pool':
             raise ValueError("--aggregator pool is a GraphSAGE aggregator; --model graphconv has none")
@@ -135,6 +150,9 @@ def create_model(layer_size, args, buffer=None, dtype=torch.float32):
     if args.model == 'graphconv':
         return GraphConv(layer_size, F.relu, args.use_pp, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
                          train_size=args.n_train, buffer=buffer, dtype=dtype)
+    if args.model == 'monet':
+        return MoNet(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
+                     train_size=args.n_train, buffer=buffer, dtype=dtype, n_kernels=getattr(args, 'monet_kernels', 3))
     if args.model == 'gcnii':
         return GCNII(layer_size, F.relu, norm=args.norm, dropout=args.dropout, n_linear=args.n_linear,
                      train_size=args.n_train, buffer=buffer, dtype=dtype, alpha=getattr(args, 'gcnii_alpha', 0.1),
@@ -271,12 +289,12 @@ class RankEngine:
 
     def _setup_steps(self, layout):
         """Collective set-up (generator): --model pna first derives delta from every rank's degree histogram,
-        --model graphconv and gcnii first exchange the halo rows' degrees; then the --use-pp
+        --model graphconv, gcnii and monet first exchange the halo rows' degrees; then the --use-pp
         precompute (train.py:169-189), cat(feat, neighbour mean) over the raw features' halo rows, or else the
         one-shot exchange of the static layer-0 halo rows (SURVEY.md §8f-2)."""
         if self.args.model == 'pna':
             yield from self._pna_delta_steps(layout)
-        sym = self.args.model in ('graphconv', 'gcnii')
+        sym = self.args.model in ('graphconv', 'gcnii', 'monet')
         if sym:
             yield from _sym_norm_steps(self.world, layout, self.graph, 'pipegcn.buffer.norm', self.buffer.timeout_ms)
             if self.args.model == 'gcnii':
@@ -463,7 +481,7 @@ class RankEngine:
             # one key per evaluation layout (every rank opens them in the same order): several may be alive at once
             self._n_eval_layouts = getattr(self, '_n_eval_layouts', 0) + 1
             key = 'pipegcn.eval.layout%d' % self._n_eval_layouts
-        sym = args.model in ('graphconv', 'gcnii')
+        sym = args.model in ('graphconv', 'gcnii', 'monet')
         st.xch = EvalExchange(self.world, lay.num_in, lay.num_all, lay.boundary, lay.recv_shape, widths, n_graph,
                               self.dtype, key=key, timeout_ms=self.buffer.timeout_ms)
         self.last_eval_exchange = st.xch
